@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py - images/sec of the MonoFlex per-image hot path on B200 (BASELINE.json), synthetic 384x1280 KITTI-shaped batches,
+"""bench.py - images/sec of the MonoFlex per-image hot path on H100 (BASELINE.json), synthetic 384x1280 KITTI-shaped batches,
 random-init weights of the reference architecture.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch 8] [--precision strict|fast] [--impl ours|reference|torch_gpu]
+                    [--dump-outputs DIR]
     python bench.py --train [--gpus N] [--graph 1|0] ...                       # BASELINE configs[2] / configs[4]
 
 Inference (configs[1]; --batch 32 = configs[3]): a "step" = one pass of DLA-34 + IDA-up + DCNv2 + predictor + NMS / top-k / 3D
@@ -20,6 +21,10 @@ decode over one batch. ONE JSON line (rank 0):
 --train: one step = train-mode forward + 11-term loss + whole-network backward + gradient exchange + AdamW (see bench_train).
 --impl reference: the reference's CPU path (oracle port; its native extension cannot be built on torch >= 1.11, DESIGN.md) with
 every useful host thread, each step one bounded sample (a batch-1 forward / train step); prints the steps it actually ran.
+--dump-outputs DIR: after the timed steps, the outputs of the last timed inference step (headline precision) as DIR/*.npy:
+  detections.npy [N, 14] float32 (the rows `forward` returns), counts.npy [B] float64 (detections per image) and heatmap.npy
+  [B, classes, H/4, W/4] float32 (the sigmoid class heat-map the decode reads). Inputs and weights are seeded, so two builds
+  run with the same arguments can be compared output for output.
 --impl torch_gpu: the same restated reference graph executed by stock PyTorch on the GPU (cuDNN convs + torchvision
 deform_conv2d), TF32 off and on - the "practical bar" of SURVEY 8d, stated as context, never the product path.
 """
@@ -46,12 +51,12 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), d.get("bf16_tflops", 1590.0), "measured"
-    return 6650.0, 1400.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), d.get("bf16_tflops", 989.0), "measured"
+    return 3350.0, 989.0, 989.0, "fallback (H100 SXM data sheet, dense bf16)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -457,8 +462,8 @@ def bench_train(args, rank, world, local_rank, config):
                                     "host-side target handling of batch i+1 overlaps step i; the image batch of step i+1 is copied host -> device on "
                                     "a second stream (double-buffered) while step i computes"},
                 "gpu_launches": (n_launch * args.steps) if n_launch else None,
-                "gpu_launches_note": "kernels of one step counted from the ncu launch list of tools/profile_train_step.py "
-                                     "(profiles/train_step_launches_r02.json); with --graph 1 they replay from ONE cudaGraphLaunch",
+                "gpu_launches_note": "kernels of one step from a launch list of tools/profile_train_step.py committed as "
+                                     "profiles/train_step_launches_r02.json (null without one); with --graph 1 they replay from ONE cudaGraphLaunch",
                 "cuda_graph": bool(tr.use_cuda_graph and tr._graph is not None), "cuda_graph_error": graph_err,
                 "skipped_steps": tr.optimizer.skipped_steps(), "final_loss": total,
                 "roofline": {"bound": "tensor", "kernel": "whole train step (conv fwd + dgrad + wgrad stack)",
@@ -486,7 +491,8 @@ def bench_train(args, rank, world, local_rank, config):
 
 # ------------------------------------------------------------------------------------------------ inference bench
 def time_inference(model, targets, host_imgs, dev_imgs, steps, B, dev, barrier):
-    """-> (ms device-resident, ms end-to-end, d2h bytes) for `steps` forwards of `model` in its current precision"""
+    """-> (ms device-resident, ms end-to-end, d2h bytes, handle of the last device-resident step) for `steps` forwards of
+    `model` in its current precision"""
     import torch
     n_in = len(dev_imgs)
     with torch.no_grad():
@@ -498,10 +504,13 @@ def time_inference(model, targets, host_imgs, dev_imgs, steps, B, dev, barrier):
     e0.record()
     with torch.no_grad():
         for i in range(steps):
-            model.forward_async(dev_imgs[i % n_in], targets)          # no host sync inside the device-resident loop
+            last = model.forward_async(dev_imgs[i % n_in], targets)   # no host sync inside the device-resident loop
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1)
+    # host copies of the last step's outputs now: later forwards re-use the decode workspace and the pinned staging buffers
+    det, counts = last.result()
+    last_out = (det.clone(), list(counts), last.heat.float().cpu())
     barrier()
     # end to end: pinned host -> H2D (copy stream, one batch ahead) -> model -> D2H of the detections
     copy_stream = torch.cuda.Stream(device=dev)
@@ -544,7 +553,17 @@ def time_inference(model, targets, host_imgs, dev_imgs, steps, B, dev, barrier):
     torch.cuda.synchronize()
     ms_e2e = t0.elapsed_time(t1)
     barrier()
-    return ms, ms_e2e, B * 50 * 14 * 4 + 4 * B
+    return ms, ms_e2e, B * 50 * 14 * 4 + 4 * B, last_out
+
+
+def dump_outputs(out_dir, last):
+    """the arrays the timed path returned in its last step (see --dump-outputs)"""
+    import numpy as np
+    det, counts, heat = last
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "detections.npy"), det.float().numpy())
+    np.save(os.path.join(out_dir, "counts.npy"), np.asarray(counts, dtype=np.float64))
+    np.save(os.path.join(out_dir, "heatmap.npy"), heat.numpy())
 
 
 def main():
@@ -562,21 +581,25 @@ def main():
     ap.add_argument("--sync-bn", type=int, default=1, help="--train, N > 1: SyncBatchNorm like the reference's yaml (1, default) or per-GPU statistics (0)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--dump-launches", default=None, help="write the per-launch timing table (json) to this path")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the outputs of the last timed inference step to DIR/*.npy (float32 / float64)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.train or args.impl != "ours"):
+        ap.error("--dump-outputs writes the outputs of the inference path of this project (--impl ours, without --train)")
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
     cores = cpu_threads()
     cfg_name = "configs[3]" if args.batch == 32 else "configs[1]"
-    config = {"workload": "DLA-34+DCNv2+heads+decode inference, batch %d/GPU, 384x1280 synthetic, %dxB200 (BASELINE %s)"
+    config = {"workload": "DLA-34+DCNv2+heads+decode inference, batch %d/GPU, 384x1280 synthetic, %dxH100 (BASELINE %s)"
               % (args.batch, args.gpus, cfg_name), "batch_per_gpu": args.batch, "height": H, "width": W,
               "parallelism": "replicas x%d (images shard across GPUs, no data-path collective)" % args.gpus,
-              "l2": "4 rotating input batches (189 MB at B=8) + >= 1.8 GB activation working set >> 126 MB L2"}
+              "l2": "4 rotating input batches (189 MB at B=8) + >= 1.8 GB activation working set >> 50 MB L2"}
     if args.train:
-        config["workload"] = ("full train step (fwd+bwd+AdamW), batch %d/GPU, 384x1280 synthetic KITTI labels, %dxB200 (BASELINE %s)"
+        config["workload"] = ("full train step (fwd+bwd+AdamW), batch %d/GPU, 384x1280 synthetic KITTI labels, %dxH100 (BASELINE %s)"
                               % (args.batch, args.gpus, "configs[2]" if args.gpus == 1 else "configs[4]: DDP, NCCL grad all-reduce"))
         config["parallelism"] = "dp%d (batch dim sharded, gradient all-reduce)" % args.gpus
-        config["l2"] = "3 rotating batches; ~10 GB activation + gradient working set >> 126 MB L2"
+        config["l2"] = "3 rotating batches; ~10 GB activation + gradient working set >> 50 MB L2"
 
     if args.impl == "reference":
         if rank == 0:
@@ -621,7 +644,9 @@ def main():
     with torch.no_grad():
         for i in range(max(3, args.warmup)):
             model(dev_imgs[i % n_in], targets)
-    ms, ms_e2e, d2h = time_inference(model, targets, host_imgs, dev_imgs, args.steps, B, dev, barrier)
+    ms, ms_e2e, d2h, last = time_inference(model, targets, host_imgs, dev_imgs, args.steps, B, dev, barrier)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     launches_per_step = model.backbone.last_plan.n_launch + model.heads.predictor.last_plan.n_launch + 1 + 2
     if rank == 0:
         sampler.stop_flag = True
@@ -694,7 +719,7 @@ def main():
     # ---------------------------------------------------------------- the other precision (fewer steps: context number)
     model.set_precision(other)
     steps2 = max(5, args.steps // 2)
-    ms2, ms2_e2e, _ = time_inference(model, targets, host_imgs, dev_imgs, steps2, B, dev, barrier)
+    ms2, ms2_e2e, _, _ = time_inference(model, targets, host_imgs, dev_imgs, steps2, B, dev, barrier)
     ms2, ms2_e2e = parallel.max_over_ranks([ms2, ms2_e2e], device=dev)
     modes[other] = {"value": world * B * steps2 / (ms2 * 1e-3), "e2e": world * B * steps2 / (ms2_e2e * 1e-3),
                     "ms_per_step": ms2 / steps2, "steps": steps2}
@@ -711,8 +736,8 @@ def main():
                 "n_gpus": world, "steps": args.steps,
                 "warmup": max(3, args.warmup), "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
                 "vs_baseline": None, "precision": args.precision,
-                "dtype": ("f16 hi/lo pair operands (3 products per K step), f32 accumulate (tcgen05 kind::f16): fp32-grade"
-                          if args.precision == "strict" else "f16 operands, f32 accumulate (tcgen05 kind::f16)"),
+                "dtype": ("f16 hi/lo pair operands (3 products per K step), f32 accumulate (wgmma): fp32-grade"
+                          if args.precision == "strict" else "f16 operands, f32 accumulate (wgmma)"),
                 "data": "synthetic", "config": config, "clocks": sampler.summary(),
                 "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": B * 3 * H * W * 4,
                         "d2h_bytes_per_step": d2h, "ms_per_step": ms_e2e / args.steps},

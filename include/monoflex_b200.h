@@ -1,4 +1,4 @@
-/* libmonoflex_b200.so — C ABI of the B200-native MonoFlex hot path.
+/* libmonoflex_b200.so — C ABI of the H100-native (sm_90a) MonoFlex hot path.
  *
  * Conventions (all entry points):
  *   - plain device pointers and sizes; no torch / ATen types. Every buffer (inputs, outputs, workspaces) is allocated
@@ -23,13 +23,14 @@ extern "C" {
 /* ---- library state ------------------------------------------------------------------------------------------ */
 const char* mf_last_error(void);
 int mf_version(void);
-/* 0 = tcgen05 tensor-core implicit GEMM (default, the product), 1 = CUDA-core cross-check kernels (diagnostics). */
+/* 0 = wgmma tensor-core implicit GEMM (default, the product), 1 = CUDA-core cross-check kernels (diagnostics). */
 int mf_set_conv_impl(int impl);
 /* performance tunables (experiments; results never depend on them): id 0/1 = extra dynamic shared memory (bytes) for
  * DCN / conv CTAs (fewer resident CTAs, larger L1); id 2 = unused (was the first-generation non-persistent GEMM kernel, removed);
  * id 3 = 1 disables the TMA-store epilogue; id 4 = 1 disables the im2col-TMA A operand (cp.async gather instead); id 5 = 1 also uses
- * im2col TMA for Cin 8/16/32 (request-bound, slower); id 6 = 1 enables the A-stationary schedule of wide-N GEMMs (measured slower: too
- * few B bytes in flight); id 7 = 2 runs the DCN gather with 8 producer warps instead of 16; id 8 = 1 launches with programmatic dependent launch (no measured gain under graph replay);
+ * im2col TMA for Cin 8/16/32 (request-bound, slower); ids 6, 7 and 12 = unused (the A-stationary schedule, the DCN producer-warp
+ * count and 256-column predictor tiles do not fit the sm_90a register / shared-memory budget); id 8 = 1 launches with programmatic
+ * dependent launch (no measured gain under graph replay);
  * id 9 = 1 runs the fused head as 2-CTA clusters that TMA-multicast the 3x3 weight boxes (halves their L2->SM traffic). */
 int mf_set_tunable(int id, int value);
 /* N tile (16/32/64/128) the conv kernels use for `cout`; packed weights / scale / shift are padded to a multiple. */
@@ -60,7 +61,7 @@ int mf_pack_conv_weight_dgrad(const float* w_oihw, int Cout, int Cin, int kh, in
  * pointer, Cout | Cin << 32, (kh*kw) | cin_pad << 32, n_pad | k_pad << 32. */
 int mf_pack_conv_weights_batched(const void* descs_dev, int n, void* stream);
 
-/* Conv2d + per-channel affine (folded BatchNorm / bias) + optional residual + activation as one tcgen05 implicit GEMM.
+/* Conv2d + per-channel affine (folded BatchNorm / bias) + optional residual + activation as one wgmma implicit GEMM.
  * Replaces nn.Conv2d -> BatchNorm2d -> (+=residual) -> ReLU chains: dla_dcn.py:84-98 (BasicBlock), :195-203 (Root),
  * :268-322 (base layers), DCN.conv_offset_mask dcn_v2.py:106-122 (MF_ACT_OFFMASK, MF_OUT_F32_NHWC, y_ld = 32),
  * head 3x3 + InPlaceABN detector_predictor.py:47-75 (MF_ACT_LEAKY), head 1x1 :52,:83 (MF_OUT_F32_NCHW).
@@ -71,7 +72,7 @@ int mf_conv2d_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, co
 
 /* Full-resolution stem convolutions (DLA base_layer 7x7 3->16, level0 3x3 16->16, level1 3x3/2 16->32,
  * dla_dcn.py:268-282) on "planar" tensors [B][H][G][W/npar][8] fp16 (G = Cin/8 channel planes x npar column parities):
- * every input row segment is loaded once by TMA and the taps are read through shifted no-swizzle UMMA descriptors, no
+ * every input row segment is loaded once by TMA and the taps are read through shifted no-swizzle wgmma descriptors, no
  * im2col copies. Cin in {8, 16}; stride 1 (in_npar 1) or 2 (in_npar 2, 3x3, pad 1). Cin = 8 weights are packed with kw
  * padded to 8. Output: planar for the next stem layer (out_planar = 1, out_npar 1 or 2) or NHWC rows (y_ld). */
 int mf_conv2d_rows_f16(const void* x, int B, int H, int W, int Cin, int in_npar, const void* w_packed, int n_pad, int k_pad,
@@ -131,7 +132,7 @@ int mf_split_to_nchw_f32(const void* x, int x_ld, int x_lo, float* y, int B, int
 
 /* Fused predictor head (detector_predictor.py:121-135): `nbranch` shared-input 3x3 convs (Cin -> 256 each) + InPlaceABN
  * (scale/shift, leaky 0.01) + the 1x1 output convs of every branch in one persistent kernel; the 256-channel hidden
- * activations stay on chip (staged in smem as the A operand of a second tcgen05.mma) except for branches with
+ * activations stay on chip (staged in smem as the A operand of a second wgmma) except for branches with
  * hid_col[i] >= 0, which are also stored to `hid` [B*H*W, hid_ld] at that column (edge fusion reads them).
  * w3_packed [nbranch*256, 9*Cin] fp16 (k = tap*Cin + c); w2_packed [nbranch*32, 256] fp16 (rows >= out_nch[i] zero);
  * bias2 [nbranch*32]; out_ptrs[i] = fp32 NCHW base pointer of branch i's first output channel (host array of device
@@ -187,7 +188,7 @@ int mf_focal_loss_backward(const float* pred, const float* target, long long n, 
 /* Convolution weight gradient (backward of `nn.Conv2d` in BasicBlock / Root / IDA nodes, model/backbone/dla_dcn.py:69-203):
  *   dw[co, ci, ky, kx] = sum_{b, oy, ox} dy[b, oy, ox, co] * x[b, oy*stride - pad + ky, ox*stride - pad + kx, ci]
  * x [B*H*W, x_ld], dy [B*Ho*Wo, dy_ld] fp16 NHWC rows; dw fp32 OIHW, overwritten. Cin, Cout multiples of 64, square kernel.
- * tcgen05 GEMM with MN-major operands fed by im2col / tiled TMA, split-K with fp32 atomics (summation order not fixed). */
+ * wgmma GEMM with MN-major operands fed by im2col / tiled TMA, split-K with fp32 atomics (summation order not fixed). */
 int mf_conv2d_wgrad_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, const void* dy, int dy_ld, int Cout, int k,
                              int stride, int pad, float* dw, void* stream);
 /* same with a rectangular kernel / padding (the edge fusion's Conv1d(256, 256, 3) is a 1 x 3 convolution over [B, 1, K+2, 256]) */
@@ -268,7 +269,7 @@ int mf_bn_sync_backward_apply(const void* x, int x_ld, const void* dy, int dy_ld
                               void* dx, int dx_ld, void* dres, int dres_ld, float* workspace, void* stream);
 
 /* diagnostics: D[128,128] = A^T B with A [64,128] and B [64,128] fp16 row-major (reduction index = rows), computed with
- * MN-major tcgen05 operand descriptors - the operand form the weight-gradient GEMM of the training path needs */
+ * MN-major wgmma operand descriptors - the operand form the weight-gradient GEMM of the training path needs */
 int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* stream);
 
 /* Loss_Computation.__call__ (model/head/detector_loss.py:267-493, prepare_predictions :116-265, Real_MultiBin_loss

@@ -96,7 +96,7 @@ def load():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise RuntimeError("monoflex_b200: %s not built - run `python __graft_entry__.py` (nvcc, sm_100a). "
+            raise RuntimeError("monoflex_b200: %s not built - run `python __graft_entry__.py` (nvcc, sm_90a). "
                                "There is no CPU or PyTorch fallback." % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         lib.mf_last_error.restype = ctypes.c_char_p
@@ -106,7 +106,7 @@ def load():
             fn.argtypes = args
             fn.restype = _SZ if name.endswith("_workspace") else _I
         _lib = lib
-        for i, name in enumerate(("MF_DCN_EXTRA_SMEM", "MF_CONV_EXTRA_SMEM", "MF_UNUSED_2", "MF_NO_TMA_STORE", "MF_NO_TMA_IM2COL", "MF_TMA_SMALL_C", "MF_A_STATIONARY", "MF_DCN_WARPS_MODE", "MF_PDL", "MF_HEAD_CLUSTER", "MF_WGRAD_NO_NARROW", "MF_SPLIT_KCONCAT", "MF_HEAD2_BN256", "MF_PATCH")):     # experiments only
+        for i, name in enumerate(("MF_DCN_EXTRA_SMEM", "MF_CONV_EXTRA_SMEM", "MF_UNUSED_2", "MF_NO_TMA_STORE", "MF_NO_TMA_IM2COL", "MF_TMA_SMALL_C", "MF_UNUSED_6", "MF_UNUSED_7", "MF_PDL", "MF_HEAD_CLUSTER", "MF_WGRAD_NO_NARROW", "MF_SPLIT_KCONCAT", "MF_UNUSED_12", "MF_PATCH")):     # experiments only
             if os.environ.get(name):
                 lib.mf_set_tunable(i, int(os.environ[name]))
         if os.environ.get("MF_CONV_IMPL"):            # diagnostics only: 1 = CUDA-core cross-check kernels

@@ -2,7 +2,7 @@
 them from cuDNN through autograd, engine/trainer.py:116-117). Both run on the hand-written tensor-core kernels:
 
   * conv2d_wgrad : dW from NHWC fp16 activations and output gradients - `mf_conv2d_wgrad_nhwc_f16` (csrc/mf_wgrad.cu:
-                   tcgen05 GEMM whose MN-major operands come straight from im2col / tiled TMA boxes, split-K);
+                   wgmma GEMM whose MN-major operands come straight from im2col / tiled TMA boxes, split-K);
   * conv2d_dgrad : dX of a stride-1 convolution = the forward implicit-GEMM kernel (csrc/mf_igemm2.cu) run on dY with the
                    180-degree rotated, in/out-transposed weights and padding k-1-p (no new kernel); 3x3 stride-2 layers
                    use the four-parity decomposition (`conv2d_dgrad_stride2`).

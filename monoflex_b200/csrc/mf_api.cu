@@ -12,7 +12,7 @@
 namespace mf {
 
 static thread_local char g_err[512] = "";
-static int g_conv_impl = 0;  // 0 = tcgen05 implicit GEMM, 1 = CUDA-core cross-check
+static int g_conv_impl = 0;  // 0 = wgmma implicit GEMM, 1 = CUDA-core cross-check
 
 void set_error(const char* fmt, ...) {
   va_list ap;

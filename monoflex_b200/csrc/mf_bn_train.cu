@@ -277,7 +277,7 @@ static int bn_grid(long long M, int C, long long& rows_per_cta, int& threads, si
   // (1.6 per SM, ~26 KB in flight per SM) and 60 for level 3 - the statistics passes ran at ~1 TB/s.
   const long long group = 4ll * RL;
   long long ncta = (M + group - 1) / group;
-  if (ncta > 148 * 8) ncta = 148 * 8;
+  if (ncta > 132 * 8) ncta = 132 * 8;
   if (ncta < 1) ncta = 1;
   rows_per_cta = (M + ncta - 1) / ncta;
   rows_per_cta = (rows_per_cta + group - 1) / group * group;

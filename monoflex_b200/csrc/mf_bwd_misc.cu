@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(256) column_sum_partial_kernel(const __half* _
 }
 static int colsum_grid(long long M, long long& rpc) {
   long long n = (M + 63) / 64;                              // up to 8 CTAs per SM (see bn_grid in mf_bn_train.cu)
-  if (n > 148 * 8) n = 148 * 8;
+  if (n > 132 * 8) n = 132 * 8;
   if (n < 1) n = 1;
   rpc = (M + n - 1) / n;
   return static_cast<int>((M + rpc - 1) / rpc);

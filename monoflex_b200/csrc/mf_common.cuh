@@ -1,5 +1,5 @@
-// Common device helpers for the sm_100a kernels of monoflex_b200: mbarrier / cp.async / TMA / tcgen05 PTX.
-// Everything here is hand-written inline PTX (no CUTLASS); compile with -gencode arch=compute_100a,code=sm_100a.
+// Common device helpers for the sm_90a kernels of monoflex_b200: mbarrier / cp.async / TMA / wgmma PTX.
+// Everything here is hand-written inline PTX (no CUTLASS); compile with -gencode arch=compute_90a,code=sm_90a.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -71,7 +71,7 @@ MF_DEVINL void mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
-// generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 MF_DEVINL void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ------------------------------------------------------------------------------------------------ explicit shared-space ld/st
@@ -95,27 +95,10 @@ MF_DEVINL void sts128f(uint32_t addr, const float4& v) {
 }
 MF_DEVINL void sts32f(uint32_t addr, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory"); }
 
-// ------------------------------------------------------------------------------------------------ packed fp32 math (sm_100: FFMA2 / FMUL2)
-MF_DEVINL unsigned long long f2_pack(float a, float b) {
-  unsigned long long r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-MF_DEVINL float2 f2_unpack(unsigned long long v) {
-  float2 r;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(r.x), "=f"(r.y) : "l"(v));
-  return r;
-}
-MF_DEVINL unsigned long long f2_mul(unsigned long long a, unsigned long long b) {
-  unsigned long long d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-MF_DEVINL unsigned long long f2_fma(unsigned long long a, unsigned long long b, unsigned long long c) {
-  unsigned long long d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
+// ------------------------------------------------------------------------------------------------ two-lane fp32 math
+// (a pair of channels per call; sm_90 has no packed fp32 FMA, so these are two scalar FFMAs with round-to-nearest)
+MF_DEVINL float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+MF_DEVINL float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
 // ------------------------------------------------------------------------------------------------ cp.async
 // 16-byte global->shared copy; src_bytes == 0 zero-fills the destination (used for conv padding / K tail).
@@ -144,10 +127,9 @@ MF_DEVINL void tma_load_2d(uint32_t dst_smem, const CUtensorMap* m, uint64_t* ba
       : "memory");
 }
 
-// One lane of a fully converged warp. The MMA / TMA issuing warps walk their loops with ALL lanes (warp-uniform control flow
+// One lane of a fully converged warp. The TMA issuing warps walk their loops with ALL lanes (warp-uniform control flow
 // keeps descriptors and addresses in uniform registers) and issue under `if (elect_one())`: under `if (lane == 0)` ptxas
-// wraps every UTCHMMA / UTMALDG in an ELECT + R2UR + BRA.U.ANY "waterfall" loop (~8 dependent instructions per MMA, which
-// made the issuing thread the bottleneck of every tile narrower than ~256 columns).
+// wraps every UTMALDG in an ELECT + R2UR + BRA.U.ANY "waterfall" loop.
 MF_DEVINL bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -178,12 +160,16 @@ MF_DEVINL void tma_load_2d_mc(uint32_t dst_smem, const CUtensorMap* m, uint64_t*
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
       : "memory");
 }
-// tcgen05.commit arriving on the mbarrier at this offset in every CTA of `cta_mask`
-MF_DEVINL void umma_commit_mc(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(cta_mask)
-               : "memory");
+// arrive on the mbarrier at the same smem offset in CTA `cta` of this cluster
+MF_DEVINL void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n"
+      ".reg .b32 remote;\n"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [remote];\n"
+      "}\n" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
 }
 
 // ------------------------------------------------------------------------------------------------ named barriers, TMA store, im2col-mode TMA load
@@ -223,76 +209,92 @@ MF_DEVINL void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0
 MF_DEVINL void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 
-// ------------------------------------------------------------------------------------------------ tcgen05
-MF_DEVINL void tmem_alloc(uint32_t* dst_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_in_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-MF_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-MF_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-MF_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+// ------------------------------------------------------------------------------------------------ wgmma (sm_90a)
+// D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands from shared memory, fp32 accumulators in the registers of the
+// issuing warpgroup (4 consecutive warps, the first one's index a multiple of 4). TA / TB = 1: the operand is MN-major.
+// Accumulator fragment of thread t (warp w = t / 32 of the warpgroup, lane l): d[4 j + 2 h + e] is row 16 w + l / 4 + 8 h,
+// column 8 j + 2 (l % 4) + e.
+template <int N> struct Gmma;
+template <> struct Gmma<16> {
+  template <int TA, int TB>
+  MF_DEVINL static void mma(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %10, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1, %11, %12;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Gmma<32> {
+  template <int TA, int TB>
+  MF_DEVINL static void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %18, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1, %19, %20;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Gmma<64> {
+  template <int TA, int TB>
+  MF_DEVINL static void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
+template <> struct Gmma<128> {
+  template <int TA, int TB>
+  MF_DEVINL static void mma(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %66, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
+  }
+};
 
-// D[tmem] (+)= A[smem] * B[smem], kind::f16 (fp16/bf16 operands, fp32 accumulate), one CTA.
-MF_DEVINL void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+MF_DEVINL void gmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+MF_DEVINL void gmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+MF_DEVINL void gmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// arrive on an mbarrier once every previously issued tcgen05.mma of this thread has completed
-MF_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+template <int R>
+MF_DEVINL void gmma_hold(float (&d)[R]) {      // keeps the accumulators in place across gmma_wait (no reordering)
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread i <-> TMEM lane base+i)
-MF_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-MF_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-MF_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major operand tile in shared memory, 128-byte swizzle, rows of 64 fp16 (=128 B), 8-row atoms of 1024 B.
-// Descriptor fields (sm_100 "SmemDescriptor"): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46) | version=1 [46,48)
-// | layout_type=2 (SWIZZLE_128B) [61,64). LBO is ignored for swizzled K-major; SBO = 1024 B between 8-row atoms.
-MF_DEVINL uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+// Shared-memory matrix descriptor (sm_90 "GmmaDescriptor"): start>>4 [0,14) | LBO>>4 [16,30) | SBO>>4 [32,46)
+// | layout_type [62,64) (1 = SWIZZLE_128B, 2 = 64B, 3 = 32B, 0 = none).
+// K-major operand tile, 128-byte swizzle, rows of 64 fp16 (=128 B), 8-row atoms of 1024 B: LBO unused, SBO = 1024 B.
+MF_DEVINL uint64_t gmma_desc_sw128(uint32_t smem_addr) {
+  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// generic K-major descriptor: layout_type 0 = no swizzle (LBO = byte distance between the two 16-byte K chunks of an MMA,
-// SBO = distance between 8-row groups), 6 / 4 / 2 = 32B / 64B / 128B swizzle (LBO ignored, SBO = 8 * row bytes)
-MF_DEVINL uint64_t umma_desc_kmajor(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout_type) {
+// generic descriptor; `swz` = 0 (no swizzle: LBO = byte distance between the two 16-byte K chunks of a K-major MMA, SBO =
+// distance between 8-row groups), 32 / 64 / 128 (K-major: LBO unused, SBO = 8 * row bytes; MN-major: LBO = distance
+// between MN atoms, SBO = distance between 8-row K groups)
+MF_DEVINL uint64_t gmma_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, int swz) {
+  const uint64_t lt = swz == 128 ? 1ull : swz == 64 ? 2ull : swz == 32 ? 3ull : 0ull;
   return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-         (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32) | (1ull << 46) |
-         (static_cast<uint64_t>(layout_type) << 61);
+         (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32) | (lt << 62);
 }
-// kind::f16 instruction descriptor: D=f32 (bit 4), A=B=f16 (0), both K-major, N>>3 at [17,23), M>>4 at [24,29).
-MF_DEVINL constexpr uint32_t umma_idesc_f16(int m, int n) {
-  return (1u << 4) | (static_cast<uint32_t>(n >> 3) << 17) | (static_cast<uint32_t>(m >> 4) << 24);
+// accumulator fragment of a m64nN tile -> rows [64][ld] fp32 at `base` (thread-per-row epilogues read it back); ld % 32 == 4
+// makes both the float2 stores here and row-wise float4 loads conflict-free
+template <int N>
+MF_DEVINL void gmma_store_rows(const float (&d)[N / 2], uint32_t base, int ld) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  const uint32_t r0 = base + ((16 * w + (l >> 2)) * ld + 2 * (l & 3)) * 4;
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + j * 32), "f"(d[4 * j]), "f"(d[4 * j + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + (8 * ld + 8 * j) * 4), "f"(d[4 * j + 2]), "f"(d[4 * j + 3]) : "memory");
+  }
 }
+
 // byte offset of 16-byte chunk `c` (0..7) of row `r` inside a [rows x 64 fp16] SWIZZLE_128B tile
 MF_DEVINL uint32_t sw128_off(int r, int c) { return (r >> 3) * 1024 + (r & 7) * 128 + ((c ^ (r & 7)) << 4); }
 

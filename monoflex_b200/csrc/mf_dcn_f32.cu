@@ -363,7 +363,7 @@ static int make_geom(DcnGeom& g, int B, int C, int H, int W, int Co, int kh, int
 static int wgrad_splits(const DcnGeom& g) {
   const int taps = g.kh * g.kw, cpg = g.C / g.dg;
   const long long tiles = static_cast<long long>(g.dg) * taps * ((cpg + TN - 1) / TN) * ((g.Co + TM - 1) / TM);
-  long long S = (148LL * 4 + tiles - 1) / tiles;
+  long long S = (132LL * 4 + tiles - 1) / tiles;
   const long long nchunks = ((static_cast<long long>(g.Ho) * g.Wo + TK - 1) / TK) * g.B;
   if (S > nchunks) S = nchunks;
   if (S > 64) S = 64;

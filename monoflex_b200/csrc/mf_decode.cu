@@ -24,7 +24,7 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
                        float* __restrict__ out_score, int* __restrict__ out_idx) {
   pdl_wait();
   // blockIdx.x = plane * slabs + slab; a slab is a contiguous pixel range [lo, hi) of one (image, class) plane. The union
-  // of the per-slab top-K sets contains the plane's top-K, so splitting only adds parallelism (148 SMs instead of B*C).
+  // of the per-slab top-K sets contains the plane's top-K, so splitting only adds parallelism (all SMs instead of B*C).
   const int HW = H * W;
   const int plane = blockIdx.x / slabs, slab = blockIdx.x - plane * slabs;
   const int chunk = (HW + slabs - 1) / slabs;
@@ -423,30 +423,35 @@ int launch_decode(const float* heat, const float* reg, const float* calib, const
                   const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
                   float* s1_score, int* s1_idx, float* scores, long long* inds, float* clses, float* ys, float* xs,
                   float* pois, float* result, int* count, cudaStream_t st) {
+  // score bits of the slab's pixels + the staged slab with its one-row halo
+  auto smem_for = [&](int s) {
+    const int items = ((H * W + s - 1) / s + S1_THREADS - 1) / S1_THREADS;
+    return items * S1_THREADS * static_cast<int>(sizeof(unsigned int)) + ((H * W + s - 1) / s + 2 * W + 2) * static_cast<int>(sizeof(float));
+  };
   // slabs per (image, class) plane: more slabs = shorter per-CTA scans but more CTAs; one CTA of 1024 threads per SM, so a second
-  // wave doubles the kernel (the fixed S = 8 of round 1 put 192 CTAs on 148 SMs at B = 8). Pick the S <= 8 that minimises
-  // waves x (items per thread + the ~6 items' worth of radix-pass overhead).
-  int S = 1, best = 1 << 30, nsm_dec = 148;
+  // wave doubles the kernel (a fixed S = 8 puts 192 CTAs on the SMs at B = 8). Pick the S <= 8 that minimises
+  // waves x (items per thread + the ~6 items' worth of radix-pass overhead) among those whose slab fits in shared memory
+  // (a whole 96 x 320 plane does not: 248 KB).
+  int S = 0, best = 1 << 30, nsm_dec = 132, smem_max = 227 * 1024;
   {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&nsm_dec, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&smem_max, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
     for (int s = 1; s <= MF_DECODE_SLABS; ++s) {
       if (C * s * K > S2_KEYS) break;
+      if (smem_for(s) > smem_max) continue;
       const int waves = (B * C * s + nsm_dec - 1) / nsm_dec;
       const int items = ((H * W + s - 1) / s + S1_THREADS - 1) / S1_THREADS;
       const int cost = waves * (items + 6);
       if (cost < best) { best = cost; S = s; }
     }
   }
-  if (H * W > 32768 || C > 3 || C * S * K > S2_KEYS || K > 64 || R != 50) {
+  if (S == 0 || H * W > 32768 || C > 3 || C * S * K > S2_KEYS || K > 64 || R != 50) {
     set_error("decode: unsupported shape H*W=%d C=%d K=%d R=%d", H * W, C, K, R);
     return -1;
   }
-  const int n_items = ((H * W + S - 1) / S + S1_THREADS - 1) / S1_THREADS;
-  // score bits of the slab's pixels + the staged slab with its one-row halo
-  const int s1_smem = n_items * S1_THREADS * static_cast<int>(sizeof(unsigned int)) +
-                      ((H * W + S - 1) / S + 2 * W + 2) * static_cast<int>(sizeof(float));
+  const int s1_smem = smem_for(S);
   static int s1_attr = 0;
   if (s1_smem > s1_attr) {
     if (check_cuda(cudaFuncSetAttribute(nms_topk_stage1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, s1_smem),

@@ -434,7 +434,7 @@ __global__ void focal_loss_kernel(const float* __restrict__ pred, const float* _
 int launch_focal_loss(const float* pred, const float* tgt, long long n, float* out2, cudaStream_t st) {
   if (check_cuda(cudaMemsetAsync(out2, 0, 2 * sizeof(float), st), "focal memset")) return -1;
   long long blocks = (n + 1023) / 1024;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   (void)launch_k(focal_loss_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, pred, tgt, n, out2);
   return check_cuda(cudaGetLastError(), "focal_loss");
 }

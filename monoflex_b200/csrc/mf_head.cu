@@ -3,14 +3,13 @@
 // B = 8) is never written to HBM except for the two branches the edge-fusion gather needs.
 //
 // Per CTA (one per SM): for every 128-pixel m-tile, for every 128-channel n-tile nt (branch b = nt/2, half h = nt%2):
-//   main GEMM   TMA warp: im2col-mode TMA A boxes + weight boxes -> 4-stage ring; MMA thread: tcgen05.mma into one of two
-//               128-column TMEM accumulators (exactly the MODE_CONV_TMA pipeline of mf_igemm2.cu)
-//   epilogue    8 warps: tcgen05.ld -> |gamma| BN affine -> leaky 0.01 -> fp16 -> 128B-swizzled smem staging. The staged
-//               128 x 128 tile IS a canonical K-major UMMA A operand (two 64-channel sub-tiles), so ...
-//   stage 2     ... the MMA thread contracts it with the branch's 1x1 weights (32 x 256, TMA-loaded per branch into a
-//               2-deep ring) into a 32-column TMEM accumulator D2, accumulating over the branch's two n-tiles. It is
-//               issued one tile late (after the next tile's main MMAs) so it never stalls the main pipeline.
-//   epilogue 2  4 warps read D2, add the 1x1 bias and write the fp32 NCHW `cls` / `reg` channels of that branch.
+//   main GEMM   TMA warp: im2col-mode TMA A boxes + weight boxes -> 4-stage ring; two consumer warpgroups (rows 0-63 and
+//               64-127 of the tile) issue wgmma m64n128k16 with fp32 accumulators in registers
+//   epilogue    the same warpgroups: |gamma| BN affine -> leaky 0.01 -> fp16 -> 128B-swizzled smem staging. The staged
+//               128 x 128 tile IS a canonical K-major wgmma A operand (two 64-channel sub-tiles), so ...
+//   stage 2     ... each warpgroup contracts its 64 staged rows with the branch's 1x1 weights (32 x 256, TMA-loaded per
+//               branch into a 2-deep ring) into a 64 x 32 register accumulator, accumulating over the branch's two n-tiles,
+//               and after the second one adds the 1x1 bias and writes the fp32 NCHW `cls` / `reg` channels of that branch.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 #include <cstring>
@@ -25,7 +24,7 @@ static constexpr int H_OUT = 2 * H_ASTAGE;              // staged 128 x 128 fp16
 static constexpr int H_W2 = 4 * 32 * 128;               // 1x1 weights of one branch: 4 K blocks x [32 rows x 128 B]
 static constexpr int H_MAXBR = 16;
 static constexpr int H_SMEM = H_STAGES * (H_ASTAGE + H_BSTAGE) + H_OUT + 2 * H_W2 + 2048 + 1024;
-static constexpr int H_TMEM_D2 = 256;                   // D2 accumulators live at TMEM columns [256, 320)
+static constexpr int H_THREADS = 288;                   // 8 consumer warps + the TMA warp
 
 struct HeadParams {
   int B, H, W, Cin;              // feature map [B,H,W,Cin] fp16 rows, x_ld given to the tensor map
@@ -44,10 +43,10 @@ struct HeadParams {
 
 // CL = true: launched as clusters of 2 CTAs that work on two consecutive m-tiles in lock-step. Every 3x3-weight (B) box is
 // then fetched from L2 ONCE per cluster - each CTA loads 64 of its 128 rows and TMA-multicasts them into both CTAs' stage -
-// which halves the B-operand L2->SM traffic (half of this kernel's total; it is L2-bandwidth bound: 10.2 GB per B = 8
-// launch at ~12.4 TB/s). A stage is recycled only when BOTH CTAs' MMAs have released it (multicast tcgen05.commit).
+// which halves the B-operand L2->SM traffic. A stage is recycled only when the consumers of BOTH CTAs have released it
+// (each consumer warp arrives on the empty barrier of both CTAs).
 template <bool CL>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(H_THREADS, 1)
 head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                   const __grid_constant__ CUtensorMap tmap_w2, const __grid_constant__ CUtensorMap tmap_hid,
                   const __grid_constant__ HeadParams p) {
@@ -61,17 +60,8 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   uint8_t* w2_smem = o_smem + H_OUT;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(w2_smem + 2 * H_W2);
   uint64_t* empty_bar = full_bar + H_STAGES;
-  uint64_t* acc_full = empty_bar + H_STAGES;    // [2]
-  uint64_t* acc_empty = acc_full + 2;           // [2]
-  uint64_t* w2_full = acc_empty + 2;            // [2]
+  uint64_t* w2_full = empty_bar + H_STAGES;     // [2]
   uint64_t* w2_empty = w2_full + 2;             // [2]
-  uint64_t* d2_full = w2_empty + 2;             // [2]
-  uint64_t* d2_empty = d2_full + 2;             // [2]
-  uint64_t* s2_full = d2_empty + 2;             // staging written  (epilogue -> MMA)
-  uint64_t* s2_done = s2_full + 1;              // staging consumed (MMA -> epilogue)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(s2_done + 1);
-  float* sc_s = reinterpret_cast<float*>(w2_smem + 2 * H_W2 + 1024);
-  float* sh_s = sc_s + HBN;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   const int ntn = p.nbranch * 2;
@@ -79,26 +69,17 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   const int HW = p.H * p.W;
   const int nkb = p.nkb;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_w2); tma_prefetch_desc(&tmap_hid);
-    for (int s = 0; s < H_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL ? 2 : 1); }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], 256);
-      mbar_init(&w2_full[a], 1); mbar_init(&w2_empty[a], 1);
-      mbar_init(&d2_full[a], 1); mbar_init(&d2_empty[a], 128);
-    }
-    mbar_init(s2_full, 1); mbar_init(s2_done, 1);
+    for (int s = 0; s < H_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL ? 16 : 8); }
+    for (int a = 0; a < 2; ++a) { mbar_init(&w2_full[a], 1); mbar_init(&w2_empty[a], 8); }
     fence_mbar_init();
   }
-  if (warp == 5) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
   if (CL) cluster_sync_all();          // the peer's mbarriers are initialised before anything is multicast to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================================================================ TMA producer (all lanes walk the loops, one issues)
     {
       int stage = 0, bc = 0;
@@ -140,169 +121,110 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================================================ MMA issuer (main GEMM + deferred stage 2): every lane
-    // walks the loops and waits, one elected lane issues (see elect_one in mf_common.cuh)
-    {
-      constexpr uint32_t idesc = umma_idesc_f16(HBM, HBN);
-      constexpr uint32_t idesc2 = umma_idesc_f16(HBM, 32);
-      const uint64_t a_d0 = umma_desc_sw128(smem_u32(a_smem)), b_d0 = umma_desc_sw128(smem_u32(b_smem));
-      const uint64_t o_d0 = umma_desc_sw128(smem_u32(o_smem)), w2_d0 = umma_desc_sw128(smem_u32(w2_smem));
-      int stage = 0, ti = 0;
-      uint32_t phase = 0;
-      auto stage2 = [&](int tj) {                                  // 1x1 contraction of the staged tile of global tile tj
-        const int h = tj & 1, bcj = tj >> 1, buf = bcj & 1;        // ntn is even: tile parity == branch half
-        if (h == 0) {
-          mbar_wait(&d2_empty[buf], ((bcj >> 1) & 1) ^ 1);         // epilogue 2 has drained this D2 buffer
-          mbar_wait(&w2_full[buf], (bcj >> 1) & 1);
-        }
-        mbar_wait(s2_full, tj & 1);
-        tc_fence_after();
-        const uint32_t d2 = tmem_base + H_TMEM_D2 + buf * 32;
-        if (elect_one()) {
-#pragma unroll
-          for (int s = 0; s < 2; ++s)
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4)
-              umma_f16(d2, o_d0 + ((s * H_ASTAGE) >> 4) + 2 * k4,
-                       w2_d0 + ((buf * H_W2 + (2 * h + s) * 32 * 128) >> 4) + 2 * k4, idesc2, (h | s | k4) != 0 ? 1u : 0u);
-          umma_commit(s2_done);
-          if (h == 1) { umma_commit(&d2_full[buf]); umma_commit(&w2_empty[buf]); }
-        }
-        __syncwarp();
-      };
-      for (int mt = blockIdx.x; mt - crank < ntm; mt += gridDim.x) {   // CL: the pair runs the same trip count
-        for (int nt = 0; nt < ntn; ++nt, ++ti) {
-          const int acc = ti & 1;
-          mbar_wait(&acc_empty[acc], ((ti >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t d_tmem = tmem_base + acc * HBN;
-          for (int kb = 0; kb < nkb; ++kb) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint64_t a_off = static_cast<uint64_t>((stage * H_ASTAGE) >> 4);
-            const uint64_t b_off = static_cast<uint64_t>((stage * H_BSTAGE) >> 4);
-            if (elect_one()) {
-#pragma unroll
-              for (int k4 = 0; k4 < HBK / 16; ++k4)
-                umma_f16(d_tmem, a_d0 + a_off + 2 * k4, b_d0 + b_off + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-              if (CL) umma_commit_mc(&empty_bar[stage], static_cast<uint16_t>(3));
-              else umma_commit(&empty_bar[stage]);
-              if (kb == nkb - 1) umma_commit(&acc_full[acc]);
-            }
-            __syncwarp();
-            if (++stage == H_STAGES) { stage = 0; phase ^= 1; }
-          }
-          if (ti >= 1) stage2(ti - 1);
-        }
-      }
-      if (ti >= 1) stage2(ti - 1);
-    }
   } else {
-    // ================================================================ epilogue: warps 6-9 = group 0, warps 0-3 = group 1
-    const int group = warp < 4 ? 1 : 0;
-    const int et = group * 128 + (warp & 3) * 32 + lane;   // group 0 covers et 0..127 (its warp & 3 spans 2,3,0,1)
-    const int quad = warp & 3, row = quad * 32 + lane;
-    const uint32_t sc_u = smem_u32(sc_s), sh_u = smem_u32(sh_s), o_u = smem_u32(o_smem);
+    // ================================================================ consumers: warpgroup wg owns tile rows [64 wg, 64 wg + 64)
+    const int wg = warp >> 2, w = warp & 3;
+    const uint32_t o_u = smem_u32(o_smem);
+    const uint64_t a_d0 = gmma_desc_sw128(smem_u32(a_smem) + wg * 64 * 128), b_d0 = gmma_desc_sw128(smem_u32(b_smem));
+    const uint64_t o_d0 = gmma_desc_sw128(o_u + wg * 64 * 128), w2_d0 = gmma_desc_sw128(smem_u32(w2_smem));
+    float d[HBN / 2], d2[16];
+    int stage = 0, ti = 0;
+    uint32_t phase = 0;
     bool store_pending = false;
-    int ti = 0;
-    auto epilogue2 = [&](int tj, int mtj) {                // 1x1 outputs of the branch whose second half was tile tj
-      if (group != 0) return;
-      const int bcj = tj >> 1, buf = bcj & 1, br = (tj % ntn) >> 1;
-      mbar_wait(&d2_full[buf], (bcj >> 1) & 1);
-      tc_fence_after();
-      uint32_t r[32];
-      tmem_ld32(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + H_TMEM_D2 + buf * 32, r);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&d2_empty[buf]);
-      const int m = mtj * HBM + row;
-      if (m < p.M) {
-        const int img = m / HW, pix = m - img * HW;
-        float* yp = p.out[br] + static_cast<long long>(img) * p.out_ctot[br] * HW + pix;
-        const int nch = p.out_nch[br];
-#pragma unroll
-        for (int n = 0; n < 32; ++n)
-          if (n < nch) yp[static_cast<long long>(n) * HW] = __uint_as_float(r[n]) + __ldg(p.bias2 + br * 32 + n);
-      }
-    };
-    int prev_mt = 0;
     for (int mt = blockIdx.x; mt - crank < ntm; mt += gridDim.x) {   // CL: the pair runs the same trip count
       for (int nt = 0; nt < ntn; ++nt, ++ti) {
-        const int acc = ti & 1, br = nt >> 1, n0 = nt * HBN;
-        if (store_pending && et == 0) bulk_wait_read0();
-        if (et < HBN) {
-          sts32f(sc_u + et * 4, __ldg(p.scale + n0 + et));
-          sts32f(sh_u + et * 4, __ldg(p.shift + n0 + et));
-        }
-        bar_sync_named(1, 256);
-        mbar_wait(&acc_full[acc], (ti >> 1) & 1);
-        tc_fence_after();
-        // this group converts two of the four 32-column chunks: group 0 -> chunks 0, 2; group 1 -> chunks 1, 3
-        float v[2][32];
+        const int br = nt >> 1, h = nt & 1, n0 = nt * HBN, bcj = ti >> 1, buf = bcj & 1;   // ntn is even: tile parity == half
+        gmma_fence();
+        for (int kb = 0; kb < nkb; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint64_t a_off = static_cast<uint64_t>((stage * H_ASTAGE) >> 4);
+          const uint64_t b_off = static_cast<uint64_t>((stage * H_BSTAGE) >> 4);
 #pragma unroll
-        for (int c2 = 0; c2 < 2; ++c2) {
-          const int ch = c2 * 2 + group;
-          uint32_t r[32];
-          tmem_ld32(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * HBN + ch * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 32; i += 4) {
-            const float4 s4 = lds128f(sc_u + (ch * 32 + i) * 4), h4 = lds128f(sh_u + (ch * 32 + i) * 4);
-            float t0 = __uint_as_float(r[i]) * s4.x + h4.x, t1 = __uint_as_float(r[i + 1]) * s4.y + h4.y;
-            float t2 = __uint_as_float(r[i + 2]) * s4.z + h4.z, t3 = __uint_as_float(r[i + 3]) * s4.w + h4.w;
-            v[c2][i] = fmaxf(t0, 0.01f * t0); v[c2][i + 1] = fmaxf(t1, 0.01f * t1);     // leaky_relu(0.01)
-            v[c2][i + 2] = fmaxf(t2, 0.01f * t2); v[c2][i + 3] = fmaxf(t3, 0.01f * t3);
+          for (int k4 = 0; k4 < HBK / 16; ++k4)
+            Gmma<HBN>::mma<0, 0>(d, a_d0 + a_off + 2 * k4, b_d0 + b_off + 2 * k4, (kb | k4) != 0 ? 1u : 0u);
+          gmma_commit();
+          gmma_wait<0>();
+          gmma_hold(d);
+          __syncwarp();
+          if (lane == 0) {
+            if (CL) { mbar_arrive_cluster(&empty_bar[stage], 0); mbar_arrive_cluster(&empty_bar[stage], 1); }
+            else mbar_arrive(&empty_bar[stage]);
           }
+          if (++stage == H_STAGES) { stage = 0; phase ^= 1; }
         }
-        tc_fence_before();
-        mbar_arrive(&acc_empty[acc]);                          // accumulator is in registers: hand it back
-        if (ti >= 1) mbar_wait(s2_done, (ti - 1) & 1);         // stage 2 of the previous tile no longer reads the staging
-        __half* hid_row = nullptr;                             // this thread's pixel is one the edge fusion will gather
-        if (p.hid_mask != nullptr && p.hid_col[br] >= 0) {
-          const int m = mt * HBM + row;
-          if (m < p.M && __ldg(p.hid_mask + m))
-            hid_row = p.hid + static_cast<long long>(m) * p.hid_ld + p.hid_col[br] + (nt & 1) * HBN;
-        }
+        // ---- epilogue: affine + leaky -> fp16 staging (and the hidden rows the edge fusion gathers)
+        if (store_pending && threadIdx.x == 0) bulk_wait_read0();  // previous tile's TMA store has read the staging
+        bar_sync_named(1, 256);
 #pragma unroll
-        for (int c2 = 0; c2 < 2; ++c2) {
-          const int ch = c2 * 2 + group;
-          const uint32_t sub = o_u + (ch >> 1) * H_ASTAGE;
+        for (int hh = 0; hh < 2; ++hh) {
+          const int row = wg * 64 + 16 * w + (lane >> 2) + 8 * hh;
+          __half* hid_row = nullptr;                           // this thread's pixel is one the edge fusion will gather
+          if (p.hid_mask != nullptr && p.hid_col[br] >= 0) {
+            const int m = mt * HBM + row;
+            if (m < p.M && __ldg(p.hid_mask + m)) hid_row = p.hid + static_cast<long long>(m) * p.hid_ld + p.hid_col[br] + h * HBN;
+          }
 #pragma unroll
-          for (int i = 0; i < 32; i += 8) {
-            __half2 o[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) o[e] = __floats2half2_rn(v[c2][i + 2 * e], v[c2][i + 2 * e + 1]);
-            sts128(sub + sw128_off(row, (ch & 1) * 4 + (i >> 3)), *reinterpret_cast<uint4*>(o));
-            if (hid_row != nullptr) *reinterpret_cast<uint4*>(hid_row + ch * 32 + i) = *reinterpret_cast<uint4*>(o);
+          for (int j = 0; j < HBN / 8; ++j) {
+            const int c = 8 * j + 2 * (lane & 3);
+            const float2 s2 = __ldg(reinterpret_cast<const float2*>(p.scale + n0 + c));
+            const float2 h2 = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + c));
+            const float t0 = d[4 * j + 2 * hh] * s2.x + h2.x, t1 = d[4 * j + 2 * hh + 1] * s2.y + h2.y;
+            const __half2 o = __floats2half2_rn(fmaxf(t0, 0.01f * t0), fmaxf(t1, 0.01f * t1));     // leaky_relu(0.01)
+            const uint32_t addr = o_u + (j >> 3) * H_ASTAGE + sw128_off(row, j & 7) + 2 * (c & 7);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(*reinterpret_cast<const uint32_t*>(&o)) : "memory");
+            if (hid_row != nullptr) *reinterpret_cast<__half2*>(hid_row + c) = o;
           }
         }
         fence_proxy_async();
         bar_sync_named(1, 256);
-        if (et == 0) {
+        if (threadIdx.x == 0) {
           store_pending = false;
           if (p.hid_col[br] >= 0 && p.hid_mask == nullptr) {   // unmasked: store the whole tile of hidden activations
-            const int col = p.hid_col[br] + (nt & 1) * HBN;
+            const int col = p.hid_col[br] + h * HBN;
             tma_store_2d(&tmap_hid, o_u, col, mt * HBM);
             tma_store_2d(&tmap_hid, o_u + H_ASTAGE, col + 64, mt * HBM);
             bulk_commit();
             store_pending = true;
           }
-          mbar_arrive(s2_full);
         }
-        // the previous tile closed a branch: its 1x1 result is complete once stage2(ti-1) (issued after this tile's main
-        // MMAs) has run - it has, or is about to: wait on d2_full
-        if (ti >= 1 && ((ti - 1) & 1) == 1) epilogue2(ti - 1, (nt == 0) ? prev_mt : mt);
+        // ---- stage 2: this warpgroup's 64 staged rows x the branch's 1x1 weights (K = 128 hidden channels of this half)
+        if (h == 0) mbar_wait(&w2_full[buf], (bcj >> 1) & 1);
+        gmma_fence();
+#pragma unroll
+        for (int s = 0; s < 2; ++s)
+#pragma unroll
+          for (int k4 = 0; k4 < 4; ++k4)
+            Gmma<32>::mma<0, 0>(d2, o_d0 + ((s * H_ASTAGE) >> 4) + 2 * k4,
+                                w2_d0 + ((buf * H_W2 + (2 * h + s) * 32 * 128) >> 4) + 2 * k4, (h | s | k4) != 0 ? 1u : 0u);
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_hold(d2);
+        if (h == 1) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&w2_empty[buf]);
+          // ---- 1x1 outputs of the branch: bias, fp32 NCHW
+          const int nch = p.out_nch[br];
+#pragma unroll
+          for (int hh = 0; hh < 2; ++hh) {
+            const int m = mt * HBM + wg * 64 + 16 * w + (lane >> 2) + 8 * hh;
+            if (m >= p.M) continue;
+            const int img = m / HW, pix = m - img * HW;
+            float* yp = p.out[br] + static_cast<long long>(img) * p.out_ctot[br] * HW + pix;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = 8 * j + 2 * (lane & 3) + e;
+                if (n < nch) yp[static_cast<long long>(n) * HW] = d2[4 * j + 2 * hh + e] + __ldg(p.bias2 + br * 32 + n);
+              }
+          }
+        }
       }
-      prev_mt = mt;
     }
-    if (ti >= 1) epilogue2(ti - 1, prev_mt);
-    if (store_pending && et == 0) bulk_wait0();
+    if (store_pending && threadIdx.x == 0) bulk_wait0();
   }
-  tc_fence_before();
   __syncthreads();
-  if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it
-  if (warp == 5) tmem_dealloc(tmem_base, 512);
+  if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -371,19 +293,19 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     if (check_cuda(cudaFuncSetAttribute(head_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, H_SMEM), "head smem")) return -1;
     attr = true;
   }
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int ntm = (p.M + HBM - 1) / HBM;
   if (!cl) {
     const int grid = ntm < nsm ? ntm : nsm;
-    return check_cuda(launch_k(head_fused_kernel<false>, dim3(grid), dim3(320), H_SMEM, st, tx, tw, tw2, th, p), "head_fused launch");
+    return check_cuda(launch_k(head_fused_kernel<false>, dim3(grid), dim3(H_THREADS), H_SMEM, st, tx, tw, tw2, th, p), "head_fused launch");
   }
   int grid = (ntm + 1) & ~1;                               // whole pairs; an odd last tile gets an all-out-of-range partner
   if (grid > (nsm & ~1)) grid = nsm & ~1;
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(320); cfg.dynamicSmemBytes = H_SMEM; cfg.stream = st;
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(H_THREADS); cfg.dynamicSmemBytes = H_SMEM; cfg.stream = st;
   cudaLaunchAttribute la[1];
   la[0].id = cudaLaunchAttributeClusterDimension;
   la[0].val.clusterDim.x = 2; la[0].val.clusterDim.y = 1; la[0].val.clusterDim.z = 1;

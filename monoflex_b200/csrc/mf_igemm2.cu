@@ -1,8 +1,8 @@
-// Persistent, warp-specialised implicit-GEMM convolution / fused DCNv2 for sm_100a (second generation of mf_igemm.cu).
+// Persistent, warp-specialised implicit-GEMM convolution / fused DCNv2 for sm_90a.
 //
 //   D[m, n] = sum_k A[m, k] * Wp[n, k]      m = output pixel, n = output channel, k = (tap, cin) cin fastest
 //
-// One CTA per SM (two for the narrow-N stem tiles) loops over 128 x BLOCK_N output tiles, n fastest:
+// One CTA per SM (two for the narrow-N tiles) loops over 128 x BLOCK_N output tiles, n fastest:
 //   warps [0, NPW)        A producers. MODE_CONV: 16-byte cp.async gathers of the zero-padded taps into the 128B-swizzled
 //                         K-major stage (Cin < 64 layers). MODE_DCN: per (pixel, tap) 4 neighbour NHWC vectors, fp32
 //                         bilinear blend * mask, fp16, st.shared; a tile is an 8x16 pixel block so its neighbourhood
@@ -10,12 +10,14 @@
 //                         fetches each (tap, 64-channel) A block with ONE im2col-mode cp.async.bulk.tensor.4d (zero
 //                         padding, strides and row/image wrap-around done by the TMA unit) and these warps become a
 //                         second epilogue group.
-//   warp NPW              weight tiles by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B), same mbarrier ring as A
-//   warp NPW+1            single-thread tcgen05.mma (kind::f16) into one of TWO TMEM accumulators
-//   warps [NPW+2, NPW+6)  epilogue: tcgen05.ld -> scale/shift (+residual) -> activation -> fp16 -> swizzled smem staging
+//   warps [NPW, NPW+8)    two consumer warpgroups: wgmma (m64 x BLOCK_N x k16, fp32 accumulators in registers), warpgroup
+//                         wg owning rows [64 wg, 64 wg + 64) of the tile; at the end of a tile they hand the accumulators
+//                         over in 32-column chunks through one fp32 smem slot and go on with the next tile's main loop
+//   warp NPW+8            weight tiles by TMA (cp.async.bulk.tensor.2d, SWIZZLE_128B), same mbarrier ring as A
+//   warps [NPW+9, NPW+13) epilogue: chunk slot -> scale/shift (+residual) -> activation -> fp16 -> swizzled smem staging
 //                         -> one TMA store per 64-channel sub-tile (fp32 NHWC / NCHW outputs: direct stores)
-// The accumulator double buffer lets the epilogue of tile i overlap the main loop of tile i+1; the smem ring and the
-// barriers persist across tiles, so the per-tile cost is the MMA time, not a pipeline fill + drain.
+// Registers + the chunk slot act as a double buffer: the epilogue of tile i overlaps the main loop of tile i+1; the smem ring
+// and the barriers persist across tiles, so the per-tile cost is the MMA time, not a pipeline fill + drain.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 
@@ -25,7 +27,7 @@ static constexpr int BM = 128;
 static constexpr int BK = 64;
 static constexpr int A_STAGE = BM * BK * 2;   // 16 KB
 
-static constexpr int AS_MAX_KB = 9;          // A-stationary mode: at most 9 resident K blocks (3x3 taps of 64 channels)
+static constexpr int MAX_A_SLOTS = 8;        // patch mode: A slots (and their full / empty barriers) per CTA
 
 // MODE_CONV_PATCH (3x3, stride 1, pad 1, Cin % 64 == 0): an m-tile is a 16 x 8 pixel patch (as in MODE_DCN) and the A operand
 // is NOT fetched tap by tap. Per 64-channel chunk (and per hi / lo half) three "slots" are loaded, one per kx: the tiled TMA box
@@ -42,26 +44,63 @@ static constexpr int PATCH_SLOT = 10 * 16 * 128;     // 20 KB
 template <int BLOCK_N, int MODE, int EPI = 0>
 struct Cfg2 {
   static constexpr bool SPLIT = EPI == 1;
-  static constexpr bool A_STAT = MODE == MODE_CONV_TMA_AS;
   static constexpr bool PATCH = MODE == MODE_CONV_PATCH;
   // patch mode: ring of A slots + ring of weight stages (one stage = the BLOCK_N x 64 block of one tap / chunk / half)
-  static constexpr int NSLOT = !PATCH ? 0 : (BLOCK_N >= 128 ? (EPI == 2 ? 6 : 4) : (BLOCK_N >= 64 ? 6 : 8));
-  static constexpr int PSTAGES = BLOCK_N >= 128 ? (EPI == 2 ? 6 : 4) : (BLOCK_N >= 64 ? 6 : 8);
-  static constexpr int STAGES0 = PATCH ? PSTAGES : A_STAT ? 3 : (MODE == MODE_DCN ? 4 : (BLOCK_N >= 256 ? 4 : BLOCK_N >= 128 ? 5 : (BLOCK_N >= 64 ? 6 : (BLOCK_N >= 32 ? 5 : 6))));
-  static constexpr int STAGES = PATCH ? STAGES0 : (SPLIT && BLOCK_N >= 64) ? ((MODE == MODE_DCN && BLOCK_N < 128) ? STAGES0 : STAGES0 - 1) : STAGES0;
-  static constexpr int A_REGION = PATCH ? NSLOT * PATCH_SLOT : (A_STAT ? AS_MAX_KB : STAGES) * A_STAGE;
-  static constexpr int LAG = BLOCK_N >= 64 ? 3 : (BLOCK_N >= 32 ? 3 : 4);   // cp.async groups in flight per producer thread
   static constexpr int CTAS_PER_SM = (BLOCK_N >= 64 || PATCH) ? 1 : 2;
+  static constexpr int LAG = BLOCK_N >= 64 ? 3 : (BLOCK_N >= 32 ? 3 : 4);   // cp.async groups in flight per producer thread
   static constexpr int B_STAGE = BLOCK_N * BK * 2;
   static constexpr int OUT_HALF = BLOCK_N >= 64 ? (BLOCK_N / 64) * A_STAGE : 0;     // staging of one fp16 tile
   static constexpr int OUT_STAGE = EPI == 2 ? 0 : (SPLIT ? 2 * OUT_HALF : OUT_HALF);
-  static constexpr int BAR_BYTES = 384;                         // barriers + tmem ptr
+  static constexpr int BAR_BYTES = 384;                         // barriers
   static constexpr int PRM_BYTES = MODE == MODE_DCN ? 9 * BM * 32 : 0;   // DCN sampling records
-  static constexpr int SMEM = A_REGION + STAGES * B_STAGE + OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + 1024;
-  static_assert(SMEM <= 227 * 1024, "shared memory budget");
-  static constexpr int ACC_COLS = BLOCK_N < 32 ? 32 : BLOCK_N;  // columns per accumulator
-  static constexpr int TMEM_COLS = 2 * ACC_COLS;                // power of two >= 32 for every BLOCK_N used
+  static constexpr int CHUNK = BLOCK_N >= 32 ? 32 : 16;         // accumulator hand-over unit (columns)
+  static constexpr int ACC_LD = CHUNK + 4;                      // fp32 row stride of the chunk slot (conflict-free, see gmma_store_cols)
+  static constexpr int ACC_BYTES = BM * ACC_LD * 4;
+  static constexpr int BUDGET = (CTAS_PER_SM == 2 ? 113 : 227) * 1024;
+  static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + 1024;
+  // ring depths: the deepest of the preferred depth and what the shared-memory budget leaves
+  static constexpr int NSLOT = !PATCH ? 0 : (BLOCK_N >= 128 ? (EPI == 2 ? 6 : 4) : (BLOCK_N >= 64 ? 6 : 8));
+  static constexpr int PSTAGES0 = BLOCK_N >= 128 ? (EPI == 2 ? 6 : 4) : (BLOCK_N >= 64 ? 6 : 8);
+  static constexpr int STAGES0 = (MODE == MODE_DCN ? 4 : (BLOCK_N >= 128 ? 5 : (BLOCK_N >= 64 ? 6 : (BLOCK_N >= 32 ? 5 : 6))));
+  static constexpr int STAGES1 = (SPLIT && BLOCK_N >= 64) ? ((MODE == MODE_DCN && BLOCK_N < 128) ? STAGES0 : STAGES0 - 1) : STAGES0;
+  static_assert(NSLOT <= MAX_A_SLOTS, "patch-mode slot barriers");
+  static constexpr int FIT = PATCH ? (BUDGET - FIXED - NSLOT * PATCH_SLOT) / B_STAGE : (BUDGET - FIXED) / (A_STAGE + B_STAGE);
+  static constexpr int PREF = PATCH ? PSTAGES0 : STAGES1;
+  static constexpr int STAGES = PREF < FIT ? PREF : FIT;
+  static_assert(STAGES >= 2, "at least a double-buffered ring");
+  static constexpr int A_REGION = PATCH ? NSLOT * PATCH_SLOT : STAGES * A_STAGE;
+  static constexpr int SMEM = A_REGION + STAGES * B_STAGE + FIXED;
+  static_assert(SMEM <= BUDGET, "shared memory budget");
 };
+
+// fragment columns [8 j0, 8 j0 + 8 NJ) of a m64 x N accumulator -> chunk slot rows [64][ld] fp32 (see gmma_store_rows)
+template <int N, int J0, int NJ>
+MF_DEVINL void gmma_store_cols(const float (&d)[N / 2], uint32_t base, int ld) {
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  const uint32_t r0 = base + ((16 * w + (l >> 2)) * ld + 2 * (l & 3)) * 4;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + j * 32), "f"(d[4 * (J0 + j)]), "f"(d[4 * (J0 + j) + 1]) : "memory");
+    asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(r0 + (8 * ld + 8 * j) * 4), "f"(d[4 * (J0 + j) + 2]),
+                 "f"(d[4 * (J0 + j) + 3]) : "memory");
+  }
+}
+template <int N, int CHUNK, int CH>
+struct ChunkDump {                         // compile-time walk over the chunks of the accumulator
+  template <typename F>
+  MF_DEVINL static void run(const float (&d)[N / 2], F&& f) {
+    if constexpr (CH * CHUNK < N) {
+      f(CH, [&](uint32_t base, int ld) { gmma_store_cols<N, CH * CHUNK / 8, CHUNK / 8>(d, base, ld); });
+      ChunkDump<N, CHUNK, CH + 1>::run(d, f);
+    }
+  }
+};
+
+// warps of a CTA: NPW producers, 8 consumers, the weight-TMA warp (MODE_DCN: the producers issue the weight loads, which
+// keeps 640 threads and 96 registers for the consumers' 64 accumulators), 4 epilogue warps, the patch-mode A-slot warp
+__host__ __device__ constexpr int igemm2_warps(int mode, int npw) {
+  return npw + 8 + (mode == MODE_DCN ? 0 : 1) + 4 + (mode == MODE_CONV_PATCH ? 1 : 0);
+}
 
 template <int N>
 MF_DEVINL void act_chunk(float (&v)[N], int act, int nb) {
@@ -79,14 +118,13 @@ MF_DEVINL void act_chunk(float (&v)[N], int act, int nb) {
 
 // EPI: 0 = plain epilogue, 1 = SPLIT (staged hi/lo output tiles), 2 = HEAD2 (1x1 head contraction in the epilogue, see IgemmParams)
 template <int BLOCK_N, int MODE, int NPW, int EPI>
-__global__ void __launch_bounds__((NPW + (MODE == MODE_CONV_PATCH ? 7 : 6)) * 32, Cfg2<BLOCK_N, MODE, EPI>::CTAS_PER_SM)
+__global__ void __launch_bounds__(igemm2_warps(MODE, NPW) * 32, Cfg2<BLOCK_N, MODE, EPI>::CTAS_PER_SM)
 igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_y,
               const __grid_constant__ CUtensorMap tmap_x, const IgemmParams p, const int use_tma_store) {
   constexpr bool PATCH = (MODE == MODE_CONV_PATCH);     // 16 x 8 pixel m-tiles, A from kx-shifted patch slots (see PATCH_SLOT)
   constexpr bool PTILE = (MODE == MODE_DCN || PATCH);   // m-tile = 16 x 8 patch of one image
-  constexpr bool A_TMA = (MODE == MODE_CONV_TMA || MODE == MODE_CONV_TMA_AS || PATCH);
-  constexpr bool A_STAT = (MODE == MODE_CONV_TMA_AS);   // A tile of an m-tile stays resident while all n-tiles stream B
-  constexpr bool M_OUTER = A_STAT || PATCH;             // tile enumeration: m-tile strided over CTAs, n-tiles inside
+  constexpr bool A_TMA = (MODE == MODE_CONV_TMA || PATCH);
+  constexpr bool M_OUTER = PATCH;                       // tile enumeration: m-tile strided over CTAs, n-tiles inside
   constexpr int EPI_THREADS = A_TMA ? 128 + NPW * 32 : 128;
   constexpr bool SPLIT = EPI == 1;
   constexpr bool HEAD2 = EPI == 2;
@@ -99,6 +137,9 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   constexpr int NPT = NPW * 32;
   constexpr int RPP = NPT / 8;
   constexpr int PASSES = BM / RPP;
+  constexpr int W_TMA = NPW + 8;                                   // weight-TMA warp (not in MODE_DCN)
+  constexpr int W_EPI = NPW + 8 + (MODE == MODE_DCN ? 0 : 1);      // first warp of epilogue group 0
+  constexpr int W_PATCH = W_EPI + 4;                               // patch-mode A-slot warp
 
   pdl_launch_dependents();
   extern __shared__ uint8_t smem_raw[];
@@ -108,14 +149,14 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   uint8_t* o_smem = b_smem + STAGES * B_STAGE;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(o_smem + C::OUT_STAGE);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* acc_full = empty_bar + STAGES;     // [2]
-  uint64_t* acc_empty = acc_full + 2;          // [2]
-  uint64_t* a_full = acc_empty + 2;            // [AS_MAX_KB]  (A-stationary mode)
-  uint64_t* a_empty = a_full + AS_MAX_KB;      // [AS_MAX_KB]  ([0] only in A-stationary mode; one per slot in patch mode)
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(a_empty + AS_MAX_KB);
+  uint64_t* acc_full = empty_bar + STAGES;     // [2] chunk slot written (chunk parity)
+  uint64_t* acc_empty = acc_full + 2;          // [1] chunk slot read
+  uint64_t* a_full = acc_empty + 2;            // [MAX_A_SLOTS] patch-mode A slot filled
+  uint64_t* a_empty = a_full + MAX_A_SLOTS;    // [MAX_A_SLOTS] patch-mode A slot read
   float* sc_s = reinterpret_cast<float*>(o_smem + C::OUT_STAGE + C::BAR_BYTES);
   float* sh_s = sc_s + BLOCK_N;
   uint8_t* prm_smem = reinterpret_cast<uint8_t*>(sh_s + BLOCK_N);      // MODE_DCN only: 9*128 sampling records (36 KB)
+  const uint32_t acc_u = smem_u32(prm_smem + C::PRM_BYTES);           // chunk slot [128][ACC_LD] fp32
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);      // warp-uniform for the compiler as well
   const int lane = threadIdx.x & 31;
@@ -124,7 +165,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   const int ntm = PTILE ? p.B * tiles_x * tiles_y : (p.M + BM - 1) / BM;
   const int ntiles = ntn * ntm;
   const int nkb = p.nkb;
-  // tile enumeration: plain = tile t, t += grid (n fastest); A-stationary = m-tile outer (strided over CTAs), n inner
+  // tile enumeration: plain = tile t, t += grid (n fastest); patch mode = m-tile outer (strided over CTAs), n inner
   const int n_outer = M_OUTER ? ntm : ntiles, n_inner = M_OUTER ? ntn : 1;
 #define MF_TILE_LOOP                                                         \
   for (int outer = blockIdx.x; outer < n_outer; outer += gridDim.x)          \
@@ -141,36 +182,29 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
     if (A_TMA) tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], A_TMA ? 1 : NPT + 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);                                 // released by the 8 consumer warps
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&acc_full[a], 1);
-      mbar_init(&acc_empty[a], EPI_THREADS);
-    }
-    for (int a = 0; a < AS_MAX_KB; ++a) { mbar_init(&a_full[a], 1); mbar_init(&a_empty[a], 1); }
+    mbar_init(&acc_full[0], 8);
+    mbar_init(&acc_full[1], 8);
+    mbar_init(&acc_empty[0], 128);                                 // a chunk is read by one epilogue group
+    for (int a = 0; a < MAX_A_SLOTS; ++a) { mbar_init(&a_full[a], 1); mbar_init(&a_empty[a], 8); }
     fence_mbar_init();
   }
-  if (warp == NPW + 1) tmem_alloc(tmem_ptr_smem, C::TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();            // everything above overlapped the previous kernel's tail; from here on we touch its outputs
 
   // ================================================================ epilogue body (run by 1 or 2 warp groups)
   auto run_epilogue = [&](const int group, const int et) {
-    const int quad = warp & 3;
+    const int quad = warp & 3;                          // a permutation of 0..3 over the 4 warps of either group
     const int row = quad * 32 + lane;
-    constexpr int CHUNK = BLOCK_N >= 32 ? 32 : 16;
+    constexpr int CHUNK = C::CHUNK;
     constexpr int NCHUNK = BLOCK_N / CHUNK;
+    int use[2] = {0, 0};                                // completed waits per chunk-parity barrier
     constexpr int NGROUPS = EPI_THREADS / 128;
     const bool staged = use_tma_store != 0;             // host guarantees OUT_F16_NHWC && BLOCK_N >= 64
     const uint32_t sc_u = smem_u32(sc_s), sh_u = smem_u32(sh_s), o_u = smem_u32(o_smem);
-    int ti = -1;
     MF_TILE_LOOP {
-      ++ti;
       const int t = MF_TILE_INDEX;
-      const int acc = ti & 1;
       const int n0 = (t % ntn) * BLOCK_N;
       const int m_tile = t / ntn;
       int m = m_tile * BM + row;
@@ -191,34 +225,28 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
         sts32f(sh_u + et * 4, __ldg(p.shift + n0 + et));
       }
       bar_sync_named(1, EPI_THREADS);
-      mbar_wait(&acc_full[acc], (ti >> 1) & 1);
-      tc_fence_after();
-      if (group >= NCHUNK) {                                        // nothing to read: hand the accumulator back
-        tc_fence_before();
-        mbar_arrive(&acc_empty[acc]);
-      }
 #pragma unroll
       for (int ch0 = 0; ch0 < NCHUNK; ch0 += NGROUPS) {
         const int ch = ch0 + group;
         if (ch >= NCHUNK) break;
-        uint32_t r[CHUNK];
-        const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * C::ACC_COLS + ch * CHUNK;
-        if constexpr (CHUNK == 32) tmem_ld32(taddr, r); else tmem_ld16(taddr, r);
-        tmem_ld_wait();
-        if (ch + NGROUPS >= NCHUNK) {                    // last chunk of this thread: accumulator fully read
-          tc_fence_before();
-          mbar_arrive(&acc_empty[acc]);
-        }
-        const int nb = n0 + ch * CHUNK;
         float v[CHUNK];
+        mbar_wait(&acc_full[ch & 1], use[ch & 1] & 1);
+        ++use[ch & 1];
+#pragma unroll
+        for (int i = 0; i < CHUNK; i += 4) {
+          const float4 a4 = lds128f(acc_u + (row * C::ACC_LD + i) * 4);
+          v[i] = a4.x; v[i + 1] = a4.y; v[i + 2] = a4.z; v[i + 3] = a4.w;
+        }
+        mbar_arrive(acc_empty);                          // chunk slot free for the next hand-over
+        const int nb = n0 + ch * CHUNK;
 #pragma unroll
         for (int i = 0; i < CHUNK; i += 4) {
           const float4 s4 = lds128f(sc_u + (ch * CHUNK + i) * 4);
           const float4 h4 = lds128f(sh_u + (ch * CHUNK + i) * 4);
-          v[i] = __uint_as_float(r[i]) * s4.x + h4.x;
-          v[i + 1] = __uint_as_float(r[i + 1]) * s4.y + h4.y;
-          v[i + 2] = __uint_as_float(r[i + 2]) * s4.z + h4.z;
-          v[i + 3] = __uint_as_float(r[i + 3]) * s4.w + h4.w;
+          v[i] = v[i] * s4.x + h4.x;
+          v[i + 1] = v[i + 1] * s4.y + h4.y;
+          v[i + 2] = v[i + 2] * s4.z + h4.z;
+          v[i + 3] = v[i + 3] * s4.w + h4.w;
         }
         if (p.res != nullptr && mvalid) {
           const __half* rp = p.res + static_cast<long long>(m) * p.res_ld + nb;
@@ -462,6 +490,15 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         const int m_tile = t / ntn;
+        const int n0 = (t % ntn) * BLOCK_N;
+        // weight tile of K block kbb into `stage` (thread 0; its arrive_expect_tx is the extra arrival of full_bar)
+        auto load_w = [&](int kbb) {
+          if (tid == 0) {
+            mbar_arrive_expect_tx(&full_bar[stage], B_STAGE);
+            const int wk = p.pair ? (3 * (kbb >> 1) + ((kbb & 1) << 1)) : kbb;    // see the weight-TMA warp
+            tma_load_2d(smem_u32(b_smem + stage * B_STAGE), &tmap_w, &full_bar[stage], wk * BK, n0);
+          }
+        };
         const int tile_b = m_tile / (tiles_x * tiles_y);
         const int tile_t = m_tile - tile_b * (tiles_x * tiles_y);
         const int tile_y0 = (tile_t / tiles_x) << 3, tile_x0 = (tile_t % tiles_x) << 4;
@@ -531,16 +568,15 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
               __half2* ol = reinterpret_cast<__half2*>(&lo4[q]);
 #pragma unroll
               for (int e = 0; e < 4; ++e) {
-                unsigned long long acc = f2_pack(0.f, 0.f);
+                float2 acc = make_float2(0.f, 0.f);
                 __half2 lacc = __hmul2(wh2[0], reinterpret_cast<const __half2*>(&vl[0])[e]);
 #pragma unroll
                 for (int cn = 0; cn < 4; ++cn) {
                   const float2 fh = __half22float2(reinterpret_cast<const __half2*>(&vh[cn])[e]);
-                  const unsigned long long w2 = f2_pack(wv[cn], wv[cn]);
-                  acc = f2_fma(w2, f2_pack(fh.x, fh.y), acc);
+                  acc = f2_fma(make_float2(wv[cn], wv[cn]), fh, acc);
                   if (cn > 0) lacc = __hfma2(wh2[cn], reinterpret_cast<const __half2*>(&vl[cn])[e], lacc);
                 }
-                float2 r2 = f2_unpack(acc);
+                float2 r2 = acc;
                 const float2 lf = __half22float2(lacc);
                 r2.x += lf.x;
                 r2.y += lf.y;
@@ -551,8 +587,9 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
             }
 #pragma unroll
             for (int which = 0; which < 3; ++which) {
-              if (which == 2 && p.pair) break;               // pair schedule: the MMA warp re-uses the hi stage for A_hi W_lo
+              if (which == 2 && p.pair) break;               // pair schedule: the consumers re-use the hi stage for A_hi W_lo
               mbar_wait(&empty_bar[stage], phase ^ 1);
+              load_w(kb + which);
               const uint32_t a_stage = smem_u32(a_smem + stage * A_STAGE);
 #pragma unroll
               for (int q = 0; q < PASSES; ++q) sts128(a_stage + dst_off[q], which == 1 ? lo4[q] : hi4[q]);
@@ -566,6 +603,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
         } else
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
+          load_w(kb);
           const uint32_t a_stage = smem_u32(a_smem + stage * A_STAGE);
           uint4 v[PASSES][4];
           float4 wq[PASSES];
@@ -586,18 +624,18 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
             const __half2* h2 = reinterpret_cast<const __half2*>(&v[q][1]);
             const __half2* h3 = reinterpret_cast<const __half2*>(&v[q][2]);
             const __half2* h4 = reinterpret_cast<const __half2*>(&v[q][3]);
-            const unsigned long long w1 = f2_pack(wq[q].x, wq[q].x), w2 = f2_pack(wq[q].y, wq[q].y);
-            const unsigned long long w3 = f2_pack(wq[q].z, wq[q].z), w4 = f2_pack(wq[q].w, wq[q].w);
+            const float2 w1 = make_float2(wq[q].x, wq[q].x), w2 = make_float2(wq[q].y, wq[q].y);
+            const float2 w3 = make_float2(wq[q].z, wq[q].z), w4 = make_float2(wq[q].w, wq[q].w);
             __half2 o2[4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {                  // two channels per FFMA2 (packed fp32 math of sm_100)
+            for (int e = 0; e < 4; ++e) {                  // two channels per step
               const float2 f1 = __half22float2(h1[e]), f2 = __half22float2(h2[e]);
               const float2 f3 = __half22float2(h3[e]), f4 = __half22float2(h4[e]);
-              unsigned long long acc = f2_mul(w1, f2_pack(f1.x, f1.y));
-              acc = f2_fma(w2, f2_pack(f2.x, f2.y), acc);
-              acc = f2_fma(w3, f2_pack(f3.x, f3.y), acc);
-              acc = f2_fma(w4, f2_pack(f4.x, f4.y), acc);
-              const float2 r2 = f2_unpack(acc);
+              float2 acc = f2_mul(w1, f1);
+              acc = f2_fma(w2, f2, acc);
+              acc = f2_fma(w3, f3, acc);
+              acc = f2_fma(w4, f4, acc);
+              const float2 r2 = acc;
               o2[e] = __floats2half2_rn(r2.x, r2.y);
             }
             sts128(a_stage + dst_off[q], *reinterpret_cast<uint4*>(o2));
@@ -610,7 +648,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
         }
       }
     }
-  } else if (warp == NPW && PATCH) {
+  } else if (warp == W_TMA && PATCH) {
     // ================================================================ patch mode: this warp streams the weight stages ...
     {
       int stage = 0;
@@ -633,7 +671,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
             }
       }
     }
-  } else if (PATCH && warp == NPW + 6) {
+  } else if (PATCH && warp == W_PATCH) {
     // ================================================================ ... and an extra warp the A slots: two independent
     // in-order producers (in one warp the two wait loops would serialise: a try_wait suspends the whole warp)
     {
@@ -659,17 +697,17 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
               }
       }
     }
-  } else if (warp == NPW) {
+  } else if (warp == W_TMA && MODE != MODE_DCN) {
     // ================================================================ weight tiles by TMA (all lanes walk, one issues)
     {
-      int stage = 0, mi = 0;
+      int stage = 0;
       uint32_t phase = 0;
       const int kc = A_TMA ? p.kc : BK, nbox = BK / kc, box_bytes = BM * kc * 2, ntap = p.kh * p.kw;
       MF_TILE_LOOP {
         const int t = MF_TILE_INDEX;
         const int n0 = (t % ntn) * BLOCK_N;
         int cw = 0, chh = 0, cn = 0;
-        if (A_TMA && (!A_STAT || inner == 0)) {   // coordinates of the tile's first output pixel in input space (incl. -pad)
+        if (A_TMA) {                              // coordinates of the tile's first output pixel in input space (incl. -pad)
           const int m0 = (t / ntn) * BM;
           cn = m0 / HoWo;
           const int rem = m0 - cn * HoWo;
@@ -677,28 +715,13 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           cw = ox * p.stride - p.pad;
           chh = oy * p.stride - p.pad;
         }
-        if (A_STAT && inner == 0) {               // the whole A tile (all taps) once per m-tile, one barrier per K block
-          mbar_wait(a_empty, (mi & 1) ^ 1);
-          ++mi;
-          int tap = 0, c0 = 0, kx = 0, ky = 0;
-          for (int kb = 0; kb < nkb; ++kb) {
-            if (elect_one()) {
-              mbar_arrive_expect_tx(&a_full[kb], A_STAGE);
-              tma_load_im2col_4d(smem_u32(a_smem + kb * A_STAGE), &tmap_x, &a_full[kb], c0, cw, chh, cn,
-                                 static_cast<uint16_t>(kx), static_cast<uint16_t>(ky));
-            }
-            __syncwarp();
-            c0 += BK;
-            if (c0 >= p.Cin) { c0 = 0; ++tap; if (++kx == p.kw) { kx = 0; ++ky; } }
-          }
-        }
         int tap = 0, c0 = 0, kx = 0, ky = 0;            // running (tap, channel) cursor: no divisions in the K loop
         int which = 0;                                  // split_in: 0 = A_hi W_hi, 1 = A_lo W_hi, 2 = A_hi W_lo (same A box as 0)
         for (int kb = 0; kb < nkb; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           const bool issuer = elect_one();
-          if (issuer) mbar_arrive_expect_tx(&full_bar[stage], (A_TMA && !A_STAT) ? A_STAGE + B_STAGE : B_STAGE);
-          if (A_TMA && !A_STAT) {
+          if (issuer) mbar_arrive_expect_tx(&full_bar[stage], A_TMA ? A_STAGE + B_STAGE : B_STAGE);
+          if (A_TMA) {
             const uint32_t a_dst = smem_u32(a_smem + stage * A_STAGE);
             for (int jb = 0; jb < nbox; ++jb) {
               const bool valid = tap < ntap;              // K tail: channel coordinate out of range -> TMA zero fill
@@ -724,33 +747,34 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
         }
       }
     }
-  } else if (warp == NPW + 1) {
-    // ================================================================ MMA issuer: every lane walks the loops and waits on
-    // the barriers (warp-uniform control flow, descriptors in uniform registers), one elected lane issues (see elect_one)
+  } else if (warp < NPW + 8) {
+    // ================================================================ consumers: warpgroup wg issues the wgmmas of tile rows
+    // [64 wg, 64 wg + 64) and hands its accumulators to the epilogue chunk by chunk. Every MMA batch is waited for before
+    // the stage it read is released (empty barriers count the 8 consumer warps).
     {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, BLOCK_N);
+      const int wg = (warp - NPW) >> 2;
+      float d[BLOCK_N / 2];
+      auto mma = [&](uint64_t ad, uint64_t bd, uint32_t accum) { Gmma<BLOCK_N>::template mma<0, 0>(d, ad, bd, accum); };
+      auto done = [&]() { gmma_commit(); gmma_wait<0>(); gmma_hold(d); __syncwarp(); };
+      auto release = [&](uint64_t* bar) { if (lane == 0) mbar_arrive(bar); };
       // Descriptors are "base + small delta": everything except the 14-bit start-address field is loop invariant, and
       // the field is linear in the byte address, so the hot loop only does 64-bit adds.
       uint64_t a_d0[BK / 16];
-      const uint32_t a0 = smem_u32(a_smem), b0 = smem_u32(b_smem);
+      const uint32_t b0 = smem_u32(b_smem);
+      const uint32_t a0 = smem_u32(a_smem) + wg * 64 * ((!A_TMA || p.kc == 64) ? 128 : 2 * p.kc);   // this warpgroup's rows
 #pragma unroll
       for (int k4 = 0; k4 < BK / 16; ++k4) {
-        if (!A_TMA || p.kc == 64) a_d0[k4] = umma_desc_sw128(a0 + k4 * 32);
-        else if (p.kc == 32) a_d0[k4] = umma_desc_kmajor(a0 + (k4 >> 1) * (BM * 64) + (k4 & 1) * 32, 16, 512, 4);
-        else if (p.kc == 16) a_d0[k4] = umma_desc_kmajor(a0 + k4 * (BM * 32), 16, 256, 6);
-        else a_d0[k4] = umma_desc_kmajor(a0 + k4 * (2 * BM * 16), BM * 16, 128, 0);       // kc == 8: two boxes per MMA
+        if (!A_TMA || p.kc == 64) a_d0[k4] = gmma_desc_sw128(a0 + k4 * 32);
+        else if (p.kc == 32) a_d0[k4] = gmma_desc(a0 + (k4 >> 1) * (BM * 64) + (k4 & 1) * 32, 16, 512, 64);
+        else if (p.kc == 16) a_d0[k4] = gmma_desc(a0 + k4 * (BM * 32), 16, 256, 32);
+        else a_d0[k4] = gmma_desc(a0 + k4 * (2 * BM * 16), BM * 16, 128, 0);       // kc == 8: two boxes per MMA
       }
-      const uint64_t b_d0 = umma_desc_sw128(b0);
-      int stage = 0, ti = -1, mi = -1;
+      const uint64_t b_d0 = gmma_desc_sw128(b0);
+      int stage = 0, fills = 0;
       int fa = 0, fa_base = 0;                                       // patch mode: slot-fill counter (as in the A producer)
       uint32_t phase = 0;
       MF_TILE_LOOP {
-        ++ti;
-        if (inner == 0) ++mi;
-        const int acc = ti & 1;
-        mbar_wait(&acc_empty[acc], ((ti >> 1) & 1) ^ 1);          // epilogue has drained this accumulator
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * C::ACC_COLS;
+        gmma_fence();
         if constexpr (PATCH) {
           if (inner == 0) fa_base = fa;
           if (p_stat) fa = fa_base;                                  // the resident slots of this m-tile, again
@@ -766,45 +790,36 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
                 mbar_wait(&a_full[s_lo], (fa / NSL) & 1);
                 ++fa;
               }
-              tc_fence_after();
               for (int ky = 0; ky < 3; ++ky) {
                 const uint64_t a_hi = static_cast<uint64_t>((s_hi * PATCH_SLOT + ky * 2048) >> 4);
                 const uint64_t a_lo = static_cast<uint64_t>((s_lo * PATCH_SLOT + ky * 2048) >> 4);
                 const int s0 = stage;
                 mbar_wait(&full_bar[s0], phase);
-                tc_fence_after();
                 const uint64_t b0s = static_cast<uint64_t>((s0 * B_STAGE) >> 4);
-                if (elect_one()) {
 #pragma unroll
-                  for (int k4 = 0; k4 < BK / 16; ++k4)                               // A_hi W_hi (or the only product)
-                    umma_f16(d_tmem, a_d0[k4] + a_hi, b_d0 + b0s + 2 * k4, idesc, k4 == 0 ? accum : 1u);
-                  if (p_nh == 1) umma_commit(&empty_bar[s0]);
-                }
-                __syncwarp();
+                for (int k4 = 0; k4 < BK / 16; ++k4)                                 // A_hi W_hi (or the only product)
+                  mma(a_d0[k4] + a_hi, b_d0 + b0s + 2 * k4, k4 == 0 ? accum : 1u);
+                if (p_nh == 1) { done(); release(&empty_bar[s0]); }
                 accum = 1u;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 if (p_nh == 2) {
                   const int s1 = stage;
                   mbar_wait(&full_bar[s1], phase);
-                  tc_fence_after();
                   const uint64_t b1s = static_cast<uint64_t>((s1 * B_STAGE) >> 4);
-                  if (elect_one()) {
 #pragma unroll
-                    for (int k4 = 0; k4 < BK / 16; ++k4) umma_f16(d_tmem, a_d0[k4] + a_lo, b_d0 + b0s + 2 * k4, idesc, 1u);   // A_lo W_hi
+                  for (int k4 = 0; k4 < BK / 16; ++k4) mma(a_d0[k4] + a_lo, b_d0 + b0s + 2 * k4, 1u);   // A_lo W_hi
 #pragma unroll
-                    for (int k4 = 0; k4 < BK / 16; ++k4) umma_f16(d_tmem, a_d0[k4] + a_hi, b_d0 + b1s + 2 * k4, idesc, 1u);   // A_hi W_lo
-                    umma_commit(&empty_bar[s0]);
-                    umma_commit(&empty_bar[s1]);
-                  }
-                  __syncwarp();
+                  for (int k4 = 0; k4 < BK / 16; ++k4) mma(a_d0[k4] + a_hi, b_d0 + b1s + 2 * k4, 1u);   // A_hi W_lo
+                  done();
+                  release(&empty_bar[s0]);
+                  release(&empty_bar[s1]);
                   if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
               }
-              if ((!p_stat || inner == n_inner - 1) && elect_one()) {   // last reader of these slots
-                umma_commit(&a_empty[s_hi]);
-                if (p_nh == 2) umma_commit(&a_empty[s_lo]);
+              if (!p_stat || inner == n_inner - 1) {                // last reader of these slots
+                release(&a_empty[s_hi]);
+                if (p_nh == 2) release(&a_empty[s_lo]);
               }
-              __syncwarp();
             }
         } else
         if (p.pair) {
@@ -812,63 +827,49 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           for (int kb = 0; kb < nkb; kb += 2) {
             const int s0 = stage;
             mbar_wait(&full_bar[s0], phase);
-            tc_fence_after();
-            const uint64_t a0 = static_cast<uint64_t>((s0 * A_STAGE) >> 4), b0s = static_cast<uint64_t>((s0 * B_STAGE) >> 4);
-            if (elect_one()) {
+            const uint64_t a0s = static_cast<uint64_t>((s0 * A_STAGE) >> 4), b0s = static_cast<uint64_t>((s0 * B_STAGE) >> 4);
 #pragma unroll
-              for (int k4 = 0; k4 < BK / 16; ++k4)                                   // A_hi W_hi
-                umma_f16(d_tmem, a_d0[k4] + a0, b_d0 + b0s + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-            }
-            __syncwarp();
+            for (int k4 = 0; k4 < BK / 16; ++k4)                                     // A_hi W_hi
+              mma(a_d0[k4] + a0s, b_d0 + b0s + 2 * k4, (kb | k4) != 0 ? 1u : 0u);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
             const int s1 = stage;
             mbar_wait(&full_bar[s1], phase);
-            tc_fence_after();
             const uint64_t a1 = static_cast<uint64_t>((s1 * A_STAGE) >> 4), b1s = static_cast<uint64_t>((s1 * B_STAGE) >> 4);
-            if (elect_one()) {
 #pragma unroll
-              for (int k4 = 0; k4 < BK / 16; ++k4)                                   // A_lo W_hi
-                umma_f16(d_tmem, a_d0[k4] + a1, b_d0 + b0s + 2 * k4, idesc, 1u);
+            for (int k4 = 0; k4 < BK / 16; ++k4)                                     // A_lo W_hi
+              mma(a_d0[k4] + a1, b_d0 + b0s + 2 * k4, 1u);
 #pragma unroll
-              for (int k4 = 0; k4 < BK / 16; ++k4)                                   // A_hi W_lo
-                umma_f16(d_tmem, a_d0[k4] + a0, b_d0 + b1s + 2 * k4, idesc, 1u);
-              umma_commit(&empty_bar[s0]);
-              umma_commit(&empty_bar[s1]);
-            }
-            __syncwarp();
+            for (int k4 = 0; k4 < BK / 16; ++k4)                                     // A_hi W_lo
+              mma(a_d0[k4] + a0s, b_d0 + b1s + 2 * k4, 1u);
+            done();
+            release(&empty_bar[s0]);
+            release(&empty_bar[s1]);
             if (++stage == STAGES) { stage = 0; phase ^= 1; }
           }
         } else
         for (int kb = 0; kb < nkb; ++kb) {
-          if (A_STAT && inner == 0) mbar_wait(&a_full[kb], mi & 1);   // resident A block of this m-tile has landed
           mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t a_off = static_cast<uint64_t>(((A_STAT ? kb : stage) * A_STAGE) >> 4);
+          const uint64_t a_off = static_cast<uint64_t>((stage * A_STAGE) >> 4);
           const uint64_t b_off = static_cast<uint64_t>((stage * B_STAGE) >> 4);
-          if (elect_one()) {
 #pragma unroll
-            for (int k4 = 0; k4 < BK / 16; ++k4) {
-              umma_f16(d_tmem, a_d0[k4] + a_off, b_d0 + b_off + 2 * k4, idesc, (kb | k4) != 0 ? 1u : 0u);
-            }
-            umma_commit(&empty_bar[stage]);
-          }
-          __syncwarp();
+          for (int k4 = 0; k4 < BK / 16; ++k4) mma(a_d0[k4] + a_off, b_d0 + b_off + 2 * k4, (kb | k4) != 0 ? 1u : 0u);
+          done();
+          release(&empty_bar[stage]);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        if (elect_one()) {
-          umma_commit(&acc_full[acc]);
-          if (A_STAT && inner == n_inner - 1) umma_commit(a_empty);   // every MMA reading the resident A tile is done
-        }
-        __syncwarp();
+        // hand-over: one chunk slot, chunk parity selects the full barrier (with two epilogue groups each waits on its own)
+        ChunkDump<BLOCK_N, C::CHUNK, 0>::run(d, [&](int ch, auto store) {
+          mbar_wait(acc_empty, (fills & 1) ^ 1);
+          store(acc_u + wg * 64 * C::ACC_LD * 4, C::ACC_LD);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&acc_full[ch & 1]);
+          ++fills;
+        });
       }
     }
   } else {
-    run_epilogue(0, (warp - (NPW + 2)) * 32 + lane);      // first epilogue group (even chunks, or all of them)
+    run_epilogue(0, (warp - W_EPI) * 32 + lane);          // first epilogue group (even chunks, or all of them)
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == NPW + 1) tmem_dealloc(tmem_base, C::TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -917,7 +918,7 @@ static int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -939,7 +940,7 @@ static int launch2_cfg(const CUtensorMap& tw, const CUtensorMap& ty, const CUten
   int grid = num_sms() * C::CTAS_PER_SM;
   if (grid > ntn * ntm) grid = ntn * ntm;
   if (MODE == MODE_CONV_PATCH && grid > ntm) grid = ntm;       // m-tiles are strided over CTAs, n-tiles run inside
-  return check_cuda(launch_k(kern, dim3(grid), dim3((NPW + (MODE == MODE_CONV_PATCH ? 7 : 6)) * 32), smem, st, tw, ty, tx, p,
+  return check_cuda(launch_k(kern, dim3(grid), dim3(igemm2_warps(MODE, NPW) * 32), smem, st, tw, ty, tx, p,
                              use_tma_store),
                     "igemm2 launch");
 }
@@ -985,8 +986,8 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
   const bool patch_geom = mode == MODE_CONV && p.split_in && p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1 &&
                           p.Cin % 64 == 0 && p.H % 8 == 0 && p.W % 16 == 0 && g_tunable[13] == 1 && g_tunable[4] == 0 &&
                           (reinterpret_cast<uintptr_t>(p.x) & 15) == 0 && p.x_ld % 8 == 0;
-  // HEAD2 tiles: 128 columns (1.39 ms at B = 8); 256-column tiles (tunable 12) measured 1.56 ms once the MMA issue was fixed
-  const int bn = p.h2_w != nullptr ? ((patch_geom || g_tunable[12] == 0) ? 128 : 256) : igemm_block_n(p.Cout);
+  // HEAD2 tiles: 128 columns (a 256-column tile would need 128 accumulator registers per consumer thread)
+  const int bn = p.h2_w != nullptr ? 128 : igemm_block_n(p.Cout);
   const bool store_ok = p.out_mode == OUT_F16_NHWC && bn >= 64 && g_tunable[3] == 0 &&
                         (reinterpret_cast<uintptr_t>(p.y) & 15) == 0 && p.y_ld % 8 == 0;
   const bool patch = patch_geom && (p.h2_w != nullptr || (p.split_out && store_ok && (bn == 64 || bn == 128)) ||
@@ -1101,18 +1102,16 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
     pp.pair = 1;                                                   // see IgemmParams::pair
     pp.nkb = 2 * p.kh * p.kw * (p.Cin / 64);
   }
-  const int ntn_host = (p.Cout + bn - 1) / bn;
   if (p.h2_w != nullptr) {                     // HEAD2 epilogue: the strict-precision predictor GEMM (see IgemmParams)
-    if (!(a_tma && (bn == 128 || bn == 256) && pp.pair && p.Cout % 256 == 0 && p.h2_part != nullptr && p.Cout / 256 <= 12)) {
-      set_error("igemm2 HEAD2: needs the pair-schedule TMA path with 128/256-column tiles and Cout a multiple of 256");
+    if (!(a_tma && pp.pair && p.Cout % 256 == 0 && p.h2_part != nullptr && p.Cout / 256 <= 12)) {
+      set_error("igemm2 HEAD2: needs the pair-schedule TMA path and Cout a multiple of 256");
       return -1;
     }
-    if (bn == 256) return launch2_cfg<256, MODE_CONV_TMA, 4, 2>(tw, ty, tx, pp, 0, st);
     return launch2_cfg<128, MODE_CONV_TMA, 4, 2>(tw, ty, tx, pp, 0, st);
   }
   if (p.split_out && use_tma_store) {          // staged hi/lo tiles: the SPLIT instantiations (N tiles of 64 / 128 only)
-    if (mode == MODE_DCN && bn == 64) return launch2_cfg<64, MODE_DCN, 16, 1>(tw, ty, tx, pp, use_tma_store, st);
-    if (mode == MODE_DCN && bn == 128) return launch2_cfg<128, MODE_DCN, 16, 1>(tw, ty, tx, pp, use_tma_store, st);
+    if (mode == MODE_DCN && bn == 64) return launch2_cfg<64, MODE_DCN, 8, 1>(tw, ty, tx, pp, use_tma_store, st);
+    if (mode == MODE_DCN && bn == 128) return launch2_cfg<128, MODE_DCN, 8, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (a_tma && bn == 64) return launch2_cfg<64, MODE_CONV_TMA, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (a_tma && bn == 128) return launch2_cfg<128, MODE_CONV_TMA, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (bn == 64) return launch2_cfg<64, MODE_CONV, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
@@ -1122,13 +1121,9 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
 #define MF_DISPATCH2(BN)                                                                          \
   if (bn == BN) {                                                                                 \
     if (mode == MODE_DCN) return launch2_cfg<BN, MODE_DCN, 8>(tw, ty, tx, pp, use_tma_store, st);  \
-    if (a_tma && BN == 128 && pp.kc == 64 && pp.nkb <= AS_MAX_KB && ntn_host >= 4 && g_tunable[6] == 1)      \
-      return launch2_cfg<128, MODE_CONV_TMA_AS, 4>(tw, ty, tx, pp, use_tma_store, st);             \
     if (a_tma) return launch2_cfg<BN, MODE_CONV_TMA, 4>(tw, ty, tx, pp, use_tma_store, st);        \
     return launch2_cfg<BN, MODE_CONV, 4>(tw, ty, tx, pp, use_tma_store, st);                       \
   }
-  if (mode == MODE_DCN && g_tunable[7] != 2 && bn == 64) return launch2_cfg<64, MODE_DCN, 16>(tw, ty, tx, pp, use_tma_store, st);
-  if (mode == MODE_DCN && g_tunable[7] != 2 && bn == 128) return launch2_cfg<128, MODE_DCN, 16>(tw, ty, tx, pp, use_tma_store, st);
   MF_DISPATCH2(16)
   MF_DISPATCH2(32)
   MF_DISPATCH2(64)

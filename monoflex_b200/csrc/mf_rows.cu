@@ -5,15 +5,17 @@
 //   * per output tile (128 consecutive pixels of one output row) the TMA warp loads each needed input row segment ONCE
 //     (144 pixels x 16 B, two tiled cp.async.bulk.tensor boxes of 8-byte elements per (row, plane, parity), zero fill outside
 //     the image);
-//   * the MMA warp reads the im2col matrix *through descriptors*: with the no-swizzle K-major layout a core matrix is
+//   * the consumer warpgroup reads the im2col matrix *through descriptors* (wgmma, two 64-pixel halves per tile): with the no-swizzle K-major layout a core matrix is
 //     8 rows x 16 B with rows 16 B apart, which is exactly "8 consecutive pixels" of a segment, so
 //       A[r, tap kx] = segment[(r + kx) * 16 B]      -> start address + kx*16, SBO = 128 (8 pixels)
 //     and the second 16-byte K chunk of an MMA (the next tap for Cin = 8, the second channel plane for Cin = 16) is
 //     reached through LBO. A 7x7 conv is 28 MMAs per tile, a 3x3 one 9 - no 49x / 9x copies through L1/L2 (the
 //     cp.async gather this replaces ran at 0.57 ms for the 7x7 layer; its unique HBM traffic is 0.03 ms);
 //   * stride 2 works on column-parity planes (pixel 2*ox + kx - 1 = parity (kx+1)&1, index ox + (kx-1)>>1);
-//   * the whole packed weight matrix stays resident in smem (<= 14 KB), accumulators are double-buffered in TMEM, the
-//     epilogue (scale/shift + ReLU) writes either the planar layout of the next stem layer or plain NHWC rows.
+//   * the whole packed weight matrix stays resident in smem (<= 14 KB), the accumulators live in the consumer warpgroup's
+//     registers, whose epilogue (scale/shift + ReLU) writes either the planar layout of the next stem layer or plain NHWC
+//     rows while the TMA warp already fetches the next tiles' segments (two CTAs per SM overlap one's epilogue with the
+//     other's MMAs).
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 #include <cstring>
@@ -47,7 +49,7 @@ struct RowsParams {
 };
 
 template <int BLOCK_N>
-__global__ void __launch_bounds__(192, 2)
+__global__ void __launch_bounds__(160, 2)
 rows_conv_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                  const __grid_constant__ RowsParams p) {
   pdl_launch_dependents();
@@ -60,33 +62,24 @@ rows_conv_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
   const int NST = p.nstages;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(a_smem + NST * stage_stride);
   uint64_t* empty_bar = full_bar + R_STAGES;
-  uint64_t* acc_full = empty_bar + R_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* w_bar = acc_empty + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(w_bar + 1);
+  uint64_t* w_bar = empty_bar + R_STAGES;
   uint64_t* desc_tab = w_bar + 2;                              // [2 * MAX_MMA]
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;      // warp-uniform for the compiler
   const int tiles_x = (p.Wo + RBM - 1) / RBM;
   const int ntiles = p.B * p.Ho * tiles_x;
-  constexpr int ACC_COLS = 32;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tmap_x);
     tma_prefetch_desc(&tmap_w);
-    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(&acc_full[a], 1); mbar_init(&acc_empty[a], 128); }
+    for (int s = 0; s < NST; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 4); }
     mbar_init(w_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 2 * ACC_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   pdl_wait();
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ================================================================ TMA: resident weights, then row segments per tile
     // (all lanes walk the loop, one elected lane issues)
     {
@@ -116,100 +109,90 @@ rows_conv_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_consta
         if (++stage == NST) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ================================================================ MMA issuer (all lanes walk the loop, one issues)
-    {
-      constexpr uint32_t idesc = umma_idesc_f16(RBM, BLOCK_N);
-      mbar_wait(w_bar, 0);
-      tc_fence_after();
-      const uint32_t a0 = smem_u32(a_smem), b0 = smem_u32(b_smem);
-      // descriptor tables in smem (stage 0 addresses): the issue loop is ld.shared + 64-bit add per MMA
-      for (int i = lane; i < p.nmma; i += 32) {
-        desc_tab[2 * i] = umma_desc_kmajor(a0 + p.mma_a[i], p.mma_lbo[i], 128, 0);
-        desc_tab[2 * i + 1] = umma_desc_sw128(b0 + p.mma_b[i]);
-      }
-      __syncwarp();
-      const int nmma = p.nmma;
-      int stage = 0, ti = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++ti) {
-        const int acc = ti & 1;
-        mbar_wait(&acc_empty[acc], ((ti >> 1) & 1) ^ 1);
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * ACC_COLS;
-        const uint64_t a_off = static_cast<uint64_t>((stage * stage_stride) >> 4);
-        if (elect_one()) {
-#pragma unroll 7
-          for (int i = 0; i < nmma; ++i)
-            umma_f16(d_tmem, desc_tab[2 * i] + a_off, desc_tab[2 * i + 1], idesc, i != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          umma_commit(&acc_full[acc]);
-        }
-        __syncwarp();
-        if (++stage == NST) { stage = 0; phase ^= 1; }
-      }
-    }
   } else {
-    // ================================================================ epilogue (warps 2..5)
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    float sc[BLOCK_N], sh[BLOCK_N];                     // tile-invariant affine: registers, not per-tile loads
+    // ================================================================ consumer warpgroup (warps 0-3): MMAs, then epilogue
+    const int t = threadIdx.x, w = t >> 5;
+    const uint32_t a0 = smem_u32(a_smem), b0 = smem_u32(b_smem);
+    // descriptor tables in smem (stage 0 addresses): the issue loop is ld.shared + 64-bit add per MMA
+    for (int i = t; i < p.nmma; i += 128) {
+      desc_tab[2 * i] = gmma_desc(a0 + p.mma_a[i], p.mma_lbo[i], 128, 0);
+      desc_tab[2 * i + 1] = gmma_desc_sw128(b0 + p.mma_b[i]);
+    }
+    bar_sync_named(1, 128);
+    float sc[BLOCK_N / 4], sh[BLOCK_N / 4];             // tile-invariant affine of this thread's columns 8 j + 2 (lane % 4) + e
 #pragma unroll
-    for (int i = 0; i < BLOCK_N; ++i) { sc[i] = __ldg(p.scale + i); sh[i] = __ldg(p.shift + i); }
-    const bool relu = p.act == ACT_RELU;
-    int ti = 0;
-    for (int t = blockIdx.x; t < ntiles; t += gridDim.x, ++ti) {
-      const int acc = ti & 1;
-      const int tx = t % tiles_x, row = t / tiles_x;
-      const int oy = row % p.Ho, b = row / p.Ho;
-      const int ox = tx * RBM + r;
-      mbar_wait(&acc_full[acc], (ti >> 1) & 1);
-      tc_fence_after();
-      uint32_t v[BLOCK_N];
-      const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * ACC_COLS;
-      if constexpr (BLOCK_N == 32) tmem_ld32(taddr, v); else tmem_ld16(taddr, v);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(&acc_empty[acc]);
-      if (ox >= p.Wo) continue;
-      __half2 o[BLOCK_N / 2], ol[BLOCK_N / 2];
+    for (int j = 0; j < BLOCK_N / 8; ++j)
 #pragma unroll
-      for (int i = 0; i < BLOCK_N; i += 2) {
-        float f0 = __uint_as_float(v[i]) * sc[i] + sh[i];
-        float f1 = __uint_as_float(v[i + 1]) * sc[i + 1] + sh[i + 1];
-        if (relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
-        o[i / 2] = __floats2half2_rn(f0, f1);
-        const float2 hf = __half22float2(o[i / 2]);
-        ol[i / 2] = __floats2half2_rn(f0 - hf.x, f1 - hf.y);          // lo half of the pair (dead code unless split_out)
+      for (int e = 0; e < 2; ++e) {
+        sc[2 * j + e] = __ldg(p.scale + 8 * j + 2 * (lane & 3) + e);
+        sh[2 * j + e] = __ldg(p.shift + 8 * j + 2 * (lane & 3) + e);
       }
-      if (p.out_planar) {
-        const int npar = p.out_npar, Wg = p.Wo / npar;
-        const int par = npar == 2 ? (ox & 1) : 0, xi = npar == 2 ? (ox >> 1) : ox;
-        const int Ghalf = (p.Cout / 8) * npar, G = p.split_out ? 2 * Ghalf : Ghalf;
+    const bool relu = p.act == ACT_RELU;
+    mbar_wait(w_bar, 0);
+    const int nmma = p.nmma;
+    int stage = 0;
+    uint32_t phase = 0;
+    float d[2][BLOCK_N / 2];
+    for (int tt = blockIdx.x; tt < ntiles; tt += gridDim.x) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint64_t a_off = static_cast<uint64_t>((stage * stage_stride) >> 4);
+      gmma_fence();
+#pragma unroll 7
+      for (int i = 0; i < nmma; ++i) {
+        const uint64_t ad = desc_tab[2 * i] + a_off, bd = desc_tab[2 * i + 1];
+        Gmma<BLOCK_N>::template mma<0, 0>(d[0], ad, bd, i != 0 ? 1u : 0u);
+        Gmma<BLOCK_N>::template mma<0, 0>(d[1], ad + (1024 >> 4), bd, i != 0 ? 1u : 0u);     // pixels 64..127: +64 x 16 B
+      }
+      gmma_commit();
+      gmma_wait<0>();
+      gmma_hold(d[0]);
+      gmma_hold(d[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[stage]);
+      if (++stage == NST) { stage = 0; phase ^= 1; }
+      const int tx = tt % tiles_x, row = tt / tiles_x;
+      const int oy = row % p.Ho, b = row / p.Ho;
 #pragma unroll
-        for (int pl = 0; pl < BLOCK_N / 8; ++pl) {
-          if (pl * 8 < p.Cout) {
-            __half* dst = p.y + ((static_cast<long long>(b * p.Ho + oy) * G + (pl * npar + par)) * Wg + xi) * 8;
-            *reinterpret_cast<uint4*>(dst) = *reinterpret_cast<const uint4*>(&o[pl * 4]);
-            if (p.split_out)
-              *reinterpret_cast<uint4*>(dst + static_cast<long long>(Ghalf) * Wg * 8) = *reinterpret_cast<const uint4*>(&ol[pl * 4]);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int ox = tx * RBM + 64 * h + 16 * w + (lane >> 2) + 8 * hh;
+          if (ox >= p.Wo) continue;
+          __half2 o[BLOCK_N / 8], ol[BLOCK_N / 8];
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            float f0 = d[h][4 * j + 2 * hh] * sc[2 * j] + sh[2 * j];
+            float f1 = d[h][4 * j + 2 * hh + 1] * sc[2 * j + 1] + sh[2 * j + 1];
+            if (relu) { f0 = fmaxf(f0, 0.f); f1 = fmaxf(f1, 0.f); }
+            o[j] = __floats2half2_rn(f0, f1);
+            const float2 hf = __half22float2(o[j]);
+            ol[j] = __floats2half2_rn(f0 - hf.x, f1 - hf.y);          // lo half of the pair (dead code unless split_out)
+          }
+          const int c2 = 2 * (lane & 3);                 // this thread's channel pair inside each 8-channel plane
+          if (p.out_planar) {
+            const int npar = p.out_npar, Wg = p.Wo / npar;
+            const int par = npar == 2 ? (ox & 1) : 0, xi = npar == 2 ? (ox >> 1) : ox;
+            const int Ghalf = (p.Cout / 8) * npar, G = p.split_out ? 2 * Ghalf : Ghalf;
+#pragma unroll
+            for (int pl = 0; pl < BLOCK_N / 8; ++pl) {
+              if (pl * 8 < p.Cout) {
+                __half* dst = p.y + ((static_cast<long long>(b * p.Ho + oy) * G + (pl * npar + par)) * Wg + xi) * 8 + c2;
+                *reinterpret_cast<__half2*>(dst) = o[pl];
+                if (p.split_out) *reinterpret_cast<__half2*>(dst + static_cast<long long>(Ghalf) * Wg * 8) = ol[pl];
+              }
+            }
+          } else {
+            __half* dst = p.y + (static_cast<long long>(b * p.Ho + oy) * p.Wo + ox) * p.y_ld + c2;
+#pragma unroll
+            for (int pl = 0; pl < BLOCK_N / 8; ++pl)
+              if (pl * 8 < p.Cout) {
+                *reinterpret_cast<__half2*>(dst + pl * 8) = o[pl];
+                if (p.split_out) *reinterpret_cast<__half2*>(dst + p.y_lo + pl * 8) = ol[pl];
+              }
           }
         }
-      } else {
-        __half* dst = p.y + (static_cast<long long>(b * p.Ho + oy) * p.Wo + ox) * p.y_ld;
-#pragma unroll
-        for (int pl = 0; pl < BLOCK_N / 8; ++pl)
-          if (pl * 8 < p.Cout) {
-            *reinterpret_cast<uint4*>(dst + pl * 8) = *reinterpret_cast<const uint4*>(&o[pl * 4]);
-            if (p.split_out) *reinterpret_cast<uint4*>(dst + p.y_lo + pl * 8) = *reinterpret_cast<const uint4*>(&ol[pl * 4]);
-          }
-      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, 2 * ACC_COLS);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -350,7 +333,7 @@ int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar,
   p.nstages = nst;
   const int smem = w_bytes + nst * stage_stride + 1024 + 2048;
   const int tiles = B * p.Ho * ((p.Wo + RBM - 1) / RBM);
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < 2 * nsm ? tiles : 2 * nsm;    // two CTAs per SM (<= 110 KB of smem each)
@@ -360,14 +343,14 @@ int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar,
       if (check_cuda(cudaFuncSetAttribute(rows_conv_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "rows smem")) return -1;
       attr = smem;
     }
-    if (check_cuda(launch_k(rows_conv_kernel<16>, dim3(grid), dim3(192), smem, st, tx, tw, p), "rows_conv launch")) return -1;
+    if (check_cuda(launch_k(rows_conv_kernel<16>, dim3(grid), dim3(160), smem, st, tx, tw, p), "rows_conv launch")) return -1;
   } else {
     static int attr = 0;
     if (smem > attr) {
       if (check_cuda(cudaFuncSetAttribute(rows_conv_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem), "rows smem")) return -1;
       attr = smem;
     }
-    if (check_cuda(launch_k(rows_conv_kernel<32>, dim3(grid), dim3(192), smem, st, tx, tw, p), "rows_conv launch")) return -1;
+    if (check_cuda(launch_k(rows_conv_kernel<32>, dim3(grid), dim3(160), smem, st, tx, tw, p), "rows_conv launch")) return -1;
   }
   return check_cuda(cudaGetLastError(), "rows_conv launch");
 }

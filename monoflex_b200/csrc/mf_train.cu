@@ -154,7 +154,7 @@ int launch_adamw_p2p(const unsigned long long* param_ptrs, const unsigned long l
   if (hi <= lo) return 0;
   const long long n_vec = (hi - lo) * (MF_ADAMW_CHUNK / 4);
   long long blocks = (n_vec + 255) / 256;
-  const long long cap = 148LL * 8 * 4;
+  const long long cap = 132LL * 8 * 4;
   if (blocks > cap) blocks = cap;
   const AdamwConsts k = adamw_consts(beta1, beta2, eps, wd, step, 1.f / static_cast<float>(world), lr_scale);
   adamw_p2p_kernel<<<dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st>>>(
@@ -170,7 +170,7 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
   if (step < 1) { set_error("adamw: step must be >= 1 (1-based count of the update being applied)"); return -1; }
   const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
   long long blocks = (n_vec + 255) / 256;
-  const long long cap = 148LL * 8 * 4;                          // a few waves; grid-stride for the rest
+  const long long cap = 132LL * 8 * 4;                          // a few waves; grid-stride for the rest
   if (blocks > cap) blocks = cap;
   (void)launch_k(adamw_arena_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, p, g, m, v, chunk_lr,
                  n_chunks, adamw_consts(beta1, beta2, eps, wd, step, grad_scale, lr_scale));
@@ -244,7 +244,7 @@ int launch_adamw_arena_dyn(float* p, const float* g, float* m, float* v, const f
   if (n_chunks <= 0) return 0;
   const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
   long long blocks = (n_vec + 255) / 256;
-  const long long cap = 148LL * 8 * 4;
+  const long long cap = 132LL * 8 * 4;
   if (blocks > cap) blocks = cap;
   if (check_finite)
     (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
@@ -284,7 +284,7 @@ int launch_focal_loss_backward(const float* pred, const float* tgt, long long n,
                                cudaStream_t st) {
   if (n <= 0) return 0;
   long long blocks = (n + 1023) / 1024;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   (void)launch_k(focal_loss_backward_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, pred, tgt, n, scale,
                  grad);
   return check_cuda(cudaGetLastError(), "focal_loss_backward");

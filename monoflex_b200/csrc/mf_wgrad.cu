@@ -2,12 +2,13 @@
 //   dW[co, ci, ky, kx] = sum over (b, oy, ox) of  dY[b, oy, ox, co] * X[b, oy*s - p + ky, ox*s - p + kx, ci]
 // As a GEMM per tap: D[(tap, ci), co] = A^T B with A = im2col(X; tap) [pixels x ci] and B = dY [pixels x co]: the
 // reduction index (output pixels) is the ROW index of both NHWC operands in memory, so both are consumed as MN-major
-// tcgen05 operands (instruction-descriptor bits 15/16; smem descriptor LBO = stride between 64-channel blocks, SBO = 1024 B
-// between 8-pixel groups - validated by mf_selftest.cu) straight from SWIZZLE_128B TMA boxes:
+// wgmma operands (transpose immediates; smem descriptor LBO = stride between 64-channel blocks, SBO = 1024 B between 8-pixel
+// groups - validated by mf_selftest.cu) straight from SWIZZLE_128B TMA boxes:
 //   A stage = two 64-channel "slots" (slot = (tap, 64-channel block)), each ONE im2col-mode TMA box of 64 output pixels
 //             (zero padding / stride / row and image wrap-around done by the TMA unit, as in the forward kernel);
 //   B stage = BLOCK_N/64 tiled-TMA boxes [64 pixels x 64 output channels] of dY.
-// Persistent, warp specialised (TMA warp, MMA thread, 4 epilogue warps); the long reduction (B*Ho*Wo pixels) is split over
+// Persistent, warp specialised (TMA warp; two consumer warpgroups, one per 64-row half of the 128-row M tile, that issue the
+// wgmmas and then add their accumulator fragments into dW); the long reduction (B*Ho*Wo pixels) is split over
 // the CTAs (split-K work items), each finishing with fp32 atomic adds (RED) into the OIHW fp32 gradient - the summation
 // order across splits is therefore not fixed (like cuDNN's non-deterministic wgrad algorithms).
 #include "mf_common.cuh"
@@ -21,7 +22,7 @@ static constexpr int WG_STAGES = 6;
 // Narrow layers (Cin or Cout = 16 / 32: level0 / level1 of DLA-34) use narrower boxes: an A slot is AW = min(Cin, 64)
 // channels wide (128 / AW slots per M tile), a B box BW = min(Cout, 64); the TMA swizzle and the descriptor layout type
 // follow the box width (128B / 64B / 32B), LBO = box bytes, SBO = 8 rows of the box.
-MF_DEVINL constexpr uint32_t wg_layout(int width) { return width == 64 ? 2u : (width == 32 ? 4u : 6u); }
+MF_DEVINL constexpr int wg_swizzle(int width) { return width * 2; }     // box row bytes = swizzle span
 
 struct WgradParams {
   int B, H, W, Cin, Ho, Wo, Cout, kh, kw, stride, pad_h, pad_w;
@@ -33,38 +34,29 @@ struct WgradParams {
 };
 
 template <int BLOCK_N, int AW, int BW>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(288, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_dy, const WgradParams p) {
   constexpr int SPT = 128 / AW;                            // A slots per M tile
   constexpr int A_BOX = WG_BK * AW * 2, B_BOX = WG_BK * BW * 2;
   constexpr int A_STAGE = SPT * A_BOX;                     // = 16 KB
   constexpr int NB = BLOCK_N / BW;
   constexpr int B_STAGE = NB * B_BOX < 1024 ? 1024 : NB * B_BOX;
-  constexpr int TCOLS = BLOCK_N < 32 ? 32 : BLOCK_N;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_smem = smem;
   uint8_t* b_smem = a_smem + WG_STAGES * A_STAGE;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(b_smem + WG_STAGES * B_STAGE);
   uint64_t* empty_bar = full_bar + WG_STAGES;
-  uint64_t* acc_full = empty_bar + WG_STAGES;
-  uint64_t* acc_empty = acc_full + 1;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(acc_empty + 1);
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   const int nitems = p.ntm * p.ntn * p.splits;
   const int HoWo = p.Ho * p.Wo, cblocks = p.Cin / AW;
 
-  if (warp == 4 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_dy);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(acc_full, 1); mbar_init(acc_empty, 128);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     fence_mbar_init();
   }
-  if (warp == 5) tmem_alloc(tmem_ptr_smem, TCOLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   // item -> (m tile, n tile, k range)
   auto decode = [&](int item, int& mt, int& nt, int& kb_lo, int& kb_hi) {
@@ -77,7 +69,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
     kb_hi = kb_lo + base + (sp < extra ? 1 : 0);
   };
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================================================================ TMA producer (all lanes walk the loops, one issues)
     {
       int stage = 0;
@@ -116,76 +108,56 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__
         }
       }
     }
-  } else if (warp == 5) {
-    // ================================================================ MMA issuer (all lanes walk the loops, one issues)
-    {
-      constexpr uint32_t idesc = umma_idesc_f16(128, BLOCK_N) | (1u << 15) | (1u << 16);      // A and B MN-major
-      const uint64_t a_d0 = umma_desc_kmajor(smem_u32(a_smem), A_BOX, 16 * AW, wg_layout(AW));
-      const uint64_t b_d0 = umma_desc_kmajor(smem_u32(b_smem), B_BOX, 16 * BW, wg_layout(BW));
-      int stage = 0, it = 0;
-      uint32_t phase = 0;
-      for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
-        int mt, nt, kb_lo, kb_hi;
-        decode(item, mt, nt, kb_lo, kb_hi);
-        mbar_wait(acc_empty, (it & 1) ^ 1);
-        tc_fence_after();
-        for (int kb = kb_lo; kb < kb_hi; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t a_off = static_cast<uint64_t>((stage * A_STAGE) >> 4), b_off = static_cast<uint64_t>((stage * B_STAGE) >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int k4 = 0; k4 < WG_BK / 16; ++k4)               // 16 pixels = two 8-row groups (2 * SBO) per MMA
-              umma_f16(tmem_base, a_d0 + a_off + static_cast<uint64_t>(k4 * ((2 * 16 * AW) >> 4)),
-                       b_d0 + b_off + static_cast<uint64_t>(k4 * ((2 * 16 * BW) >> 4)), idesc, (kb > kb_lo || k4 != 0) ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-            if (kb == kb_hi - 1) umma_commit(acc_full);
-          }
-          __syncwarp();
-          if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-        }
-        if (kb_hi <= kb_lo) {                                     // empty K range (host never asks for more splits than blocks)
-          if (elect_one()) umma_commit(acc_full);
-          __syncwarp();
-        }
-      }
-    }
   } else {
-    // ================================================================ epilogue: TMEM -> fp32 atomics into OIHW dW
-    const int row = warp * 32 + lane;                              // M index inside the tile
+    // ================================================================ consumers: warpgroup wg owns M rows [64 wg, 64 wg + 64)
+    const int wg = warp >> 2;
+    const uint64_t a_d0 = gmma_desc(smem_u32(a_smem) + wg * (64 / AW) * A_BOX, A_BOX, 16 * AW, wg_swizzle(AW));
+    const uint64_t b_d0 = gmma_desc(smem_u32(b_smem), B_BOX, 16 * BW, wg_swizzle(BW));
     const int taps = p.kh * p.kw;
-    int it = 0;
-    for (int item = blockIdx.x; item < nitems; item += gridDim.x, ++it) {
+    const int t = threadIdx.x & 127, w = t >> 5;
+    int stage = 0;
+    uint32_t phase = 0;
+    float d[BLOCK_N / 2];
+    for (int item = blockIdx.x; item < nitems; item += gridDim.x) {
       int mt, nt, kb_lo, kb_hi;
       decode(item, mt, nt, kb_lo, kb_hi);
-      const int slot = SPT * mt + row / AW;
-      const bool valid = slot < p.nslots && kb_hi > kb_lo;
-      const int tap = valid ? slot / cblocks : 0;
-      const int ci = valid ? (slot - tap * cblocks) * AW + (row % AW) : 0;
-      mbar_wait(acc_full, it & 1);
-      tc_fence_after();
-      constexpr int CH = BLOCK_N >= 32 ? 32 : 16;
 #pragma unroll
-      for (int c = 0; c < BLOCK_N; c += CH) {
-        uint32_t r[CH];
-        if constexpr (CH == 32) tmem_ld32(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c, r);
-        else tmem_ld16(tmem_base + (static_cast<uint32_t>(warp * 32) << 16) + c, r);
-        tmem_ld_wait();
-        if (valid) {
+      for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
+      for (int kb = kb_lo; kb < kb_hi; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint64_t a_off = static_cast<uint64_t>((stage * A_STAGE) >> 4), b_off = static_cast<uint64_t>((stage * B_STAGE) >> 4);
+        gmma_fence();
 #pragma unroll
-          for (int j = 0; j < CH; ++j) {
-            const int co = nt * BLOCK_N + c + j;
-            if (co < p.Cout) atomicAdd(p.dw + (static_cast<long long>(co) * p.Cin + ci) * taps + tap, __uint_as_float(r[j]));
-          }
-        }
+        for (int k4 = 0; k4 < WG_BK / 16; ++k4)                   // 16 pixels = two 8-row groups (2 * SBO) per MMA
+          Gmma<BLOCK_N>::template mma<1, 1>(d, a_d0 + a_off + static_cast<uint64_t>(k4 * ((2 * 16 * AW) >> 4)),
+                                            b_d0 + b_off + static_cast<uint64_t>(k4 * ((2 * 16 * BW) >> 4)), 1u);
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_hold(d);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
       }
-      tc_fence_before();
-      mbar_arrive(acc_empty);
+      if (kb_hi <= kb_lo) continue;                               // empty K range (host never asks for more splits than blocks)
+      // fp32 atomics into OIHW dW straight from the accumulator fragment
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = wg * 64 + 16 * w + (lane >> 2) + 8 * hh;  // M index inside the tile
+        const int slot = SPT * mt + row / AW;
+        if (slot >= p.nslots) continue;
+        const int tap = slot / cblocks;
+        const int ci = (slot - tap * cblocks) * AW + (row % AW);
+        float* dst = p.dw + static_cast<long long>(ci) * taps + tap;
+#pragma unroll
+        for (int j = 0; j < BLOCK_N / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int co = nt * BLOCK_N + 8 * j + 2 * (lane & 3) + e;
+            if (co < p.Cout) atomicAdd(dst + static_cast<long long>(co) * p.Cin * taps, d[4 * j + 2 * hh + e]);
+          }
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc(tmem_base, TCOLS);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -212,7 +184,7 @@ static int launch_wgrad_cfg(const CUtensorMap& tx, const CUtensorMap& tdy, const
     if (check_cuda(cudaFuncSetAttribute(wgrad_kernel<BLOCK_N, AW, BW>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM), "wgrad smem")) return -1;
     attr = true;
   }
-  wgrad_kernel<BLOCK_N, AW, BW><<<grid, 192, SMEM, st>>>(tx, tdy, p);
+  wgrad_kernel<BLOCK_N, AW, BW><<<grid, 288, SMEM, st>>>(tx, tdy, p);
   return check_cuda(cudaGetLastError(), "conv wgrad launch");
 }
 template <int AW>
@@ -255,7 +227,7 @@ int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, c
   p.ntn = Cout / bn;
   p.nkb = static_cast<int>((Mout + WG_BK - 1) / WG_BK);
   p.dw = dw;
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int tiles = p.ntm * p.ntn;

@@ -1,6 +1,6 @@
 // Weight gradient of the two full-resolution 16 -> 16 channel convolutions of the stem (level0 3x3 and the 7x7 base layer on the
 // zero-padded 16-channel image rows; stride 1, "same" padding). These layers are all reduction and no tile: dW is 16 x 16 x k x k
-// numbers summed over B*H*W = 3.9 M pixels. The general tcgen05 wgrad (mf_wgrad.cu) feeds them through 2 KB im2col TMA boxes
+// numbers summed over B*H*W = 3.9 M pixels. The general wgmma wgrad (mf_wgrad.cu) feeds them through 2 KB im2col TMA boxes
 // (64 pixels x 16 channels, request-bound inside the TMA unit: 2.15 ms per layer at B = 8, 8 % of the train step); here a
 // warp owns one kernel ROW (ky) of taps and walks 16-pixel blocks of an output row:
 //     dW[co, ci, ky, kx] += sum_p X[p + (ky - pad, kx - pad), ci] * dY[p, co]
@@ -118,7 +118,7 @@ int launch_conv_wgrad_narrow(const __half* x, int x_ld, int B, int H, int W, con
   }
   if (static_cast<long long>(B) * H * ((W + 15) / 16) >= (1ll << 31)) { set_error("conv wgrad (narrow): too many pixel blocks"); return -1; }
   if (check_cuda(cudaMemsetAsync(dw, 0, sizeof(float) * 16 * 16 * k * k, st), "conv wgrad narrow memset")) return -1;
-  int dev = 0, nsm = 148;
+  int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int grid = nsm * 4;

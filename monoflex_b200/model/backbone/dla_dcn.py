@@ -2,10 +2,10 @@
 
 The module tree only *holds parameters* under the reference's names so that `state_dict()` keys, checkpoint loading,
 optimizer param groups and DDP see exactly what they see in the reference (SURVEY §8b). Execution is not per-module:
-`DLASeg.forward` builds (once per input shape) a static plan of fused sm_100a kernels over NHWC fp16 buffers
+`DLASeg.forward` builds (once per input shape) a static plan of fused sm_90a kernels over NHWC fp16 buffers
 (monoflex_b200/engine.py) and replays it:
 
-  conv+BN(+residual)+ReLU      -> one tcgen05 implicit GEMM with affine epilogue      (BasicBlock :84-98, Root :195-203)
+  conv+BN(+residual)+ReLU      -> one wgmma implicit GEMM with affine epilogue        (BasicBlock :84-98, Root :195-203)
   torch.cat for Root           -> producers write channel slices of one buffer         (:197)
   MaxPool2d(2)                 -> vectorised NHWC kernel writing its concat slice      (:238)
   DCN (+BN+ReLU)               -> offset/mask conv + fused gather-contract kernel      (DeformConv :384-396)
@@ -297,7 +297,7 @@ class DLASeg(nn.Module):
             # KeypointDetector's tape bridge (model/detector.py), the training entry point
             return self.train_forward(x)
         if not x.is_cuda:
-            raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only (input is on %s); no CPU fallback" % x.device)
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only (input is on %s); no CPU fallback" % x.device)
         x = x.float().contiguous()
         plan = self._plan_for(x)
         self.run_plan(plan, x)
@@ -309,7 +309,7 @@ class DLASeg(nn.Module):
         if not self.training:
             raise RuntimeError("train_forward needs module.train()")
         if not x.is_cuda:
-            raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only (input is on %s); no CPU fallback" % x.device)
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only (input is on %s); no CPU fallback" % x.device)
         x = x.float().contiguous()
         plan = self._plan_for(x)
         self.run_plan(plan, x)

@@ -79,7 +79,7 @@ class KeypointDetector(nn.Module):
     def _forward_train(self, x, targets, prepared=None, sync_log=True):
         """model/detector.py:32-34 + detector_head.py:17-25 in training mode -> (loss_dict, log_loss_dict)."""
         if not x.is_cuda:
-            raise RuntimeError("monoflex_b200 trains on sm_100a GPUs only; no CPU fallback")
+            raise RuntimeError("monoflex_b200 trains on sm_90a GPUs only; no CPU fallback")
         features = self.backbone.train_forward(x)
         pred = self.heads.predictor.train_forward(features, targets)
         engine.bump_buffers(self)               # running statistics were updated by the bn_train kernels
@@ -142,7 +142,7 @@ class KeypointDetector(nn.Module):
             raise RuntimeError("forward_async is an inference API")
         x = to_image_list(images).tensors
         if not x.is_cuda:
-            raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only; no CPU fallback")
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
         g = self._enqueue_graph(x, targets)
         return PendingDetections(self.heads.post_processor, g['ws'], g['plan_h'].cls)
 

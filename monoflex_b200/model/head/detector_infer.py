@@ -106,7 +106,7 @@ class PostProcessor(nn.Module):
         self.check_config()
         heat, reg = predictions['cls'], predictions['reg']
         if not heat.is_cuda:
-            raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only; no CPU fallback")
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
         heat, reg = heat.float().contiguous(), reg.float().contiguous()
         ws = self.launch(heat, reg, self.prepare_targets(targets, test, heat.device))
         return self.finish(ws, heat)

@@ -131,7 +131,7 @@ class Loss_Computation(object):
         when the caller wants the numbers (a CUDA-graph capture cannot contain it)."""
         cls, reg = predictions['cls'], predictions['reg']
         if not (cls.is_cuda and reg.is_cuda):
-            raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only; no CPU fallback")
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
         cls, reg = cls.float().contiguous(), reg.float().contiguous()
         if len(targets) != reg.shape[0]:
             raise ValueError("Loss_Computation: %d target lists for a batch of %d" % (len(targets), reg.shape[0]))

@@ -314,7 +314,7 @@ def _as_rows(features):
         r.B, r.H, r.W, r.C, r.ch_off, r.buf, r.split = act.B, act.H, act.W, act.C, act.ch_off, act.buf, act.split
         return r
     if not features.is_cuda:
-        raise RuntimeError("monoflex_b200 runs on sm_100a GPUs only; no CPU fallback")
+        raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
     B, C, H, W = features.shape
     r = _Rows()
     r.B, r.H, r.W, r.C, r.ch_off, r.split = B, H, W, C, 0, False

@@ -29,7 +29,7 @@ class Trainer(object):
     def __init__(self, model, cfg, loss_scale=None, symmetric_group=None, process_group=None, bucket_bytes=32 << 20,
                  use_cuda_graph=False, graph_warmup=2):
         if not next(model.parameters()).is_cuda:
-            raise RuntimeError("monoflex_b200 trains on sm_100a GPUs only; no CPU fallback")
+            raise RuntimeError("monoflex_b200 trains on sm_90a GPUs only; no CPU fallback")
         self.model = model.train()
         if loss_scale is not None:
             model.loss_scale = float(loss_scale)

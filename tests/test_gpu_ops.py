@@ -275,7 +275,7 @@ def test_stem_7x7_from_image():
 @pytest.mark.parametrize("shape", [(2, 10, 144), (1, 7, 256), (1, 5, 40)])
 def test_stem_rows_chain(shape):
     """base_layer 7x7 -> level0 3x3 -> level1 3x3/2 on 16-byte-pixel planes (csrc/mf_rows.cu): taps are read through
-    shifted no-swizzle UMMA descriptors; every layer is compared on the GPU's own (fp16) input of that layer."""
+    shifted no-swizzle wgmma descriptors; every layer is compared on the GPU's own (fp16) input of that layer."""
     from monoflex_b200._lib import call, stream
     B, H, W = shape
     gen = np.random.Generator(np.random.PCG64(17))
@@ -605,9 +605,9 @@ def test_focal_loss_kernel():
     assert abs(out[0].item() - loss.item()) < 1e-4 * abs(loss.item()) and out[1].item() == npos.item()
 
 
-def test_tcgen05_mn_major_operands():
-    """MN-major (transposed) tcgen05 operand descriptors (csrc/mf_selftest.cu): D = A^T B with the reduction index as the
-    memory row index of both operands - the form the weight-gradient GEMM of the training rows will use. Exact in fp32
+def test_wgmma_mn_major_operands():
+    """MN-major (transposed) wgmma operand descriptors (csrc/mf_selftest.cu): D = A^T B with the reduction index as the
+    memory row index of both operands - the form the weight-gradient GEMM of the training rows uses. Exact in fp32
     accumulation order up to re-association."""
     from monoflex_b200._lib import call, stream
     gen = np.random.Generator(np.random.PCG64(77))

@@ -255,7 +255,7 @@ def test_sync_batchnorm_two_ranks_match_two_image_batch():
     (1, 10, 22, 32, 64, 1, 1, 0),        # project 1x1 after max-pool
 ])
 def test_conv_wgrad_tensor_core(case):
-    """dW of a convolution from NHWC fp16 activations / output gradients (MN-major tcgen05 operands, split-K) vs
+    """dW of a convolution from NHWC fp16 activations / output gradients (MN-major wgmma operands, split-K) vs
     torch.nn.grad.conv2d_weight on the same fp16-representable operands in fp32 (CPU)."""
     from monoflex_b200._lib import call, stream
     B, H, W, Cin, Cout, k, s, pad = case
@@ -712,10 +712,10 @@ def test_full_backward_tape_vs_reference_gradients():
     print("worst:", devs[:5], "median dev:", devs[len(devs) // 2][0], "n:", len(devs), "missing:", missing)
     assert missing == ["base.base_layer.0.weight"]
     assert len(devs) >= 150
-    # measured on B200 (loss scale 64): median 3.4 % .. 6.3 %, worst 30 % on the two earliest full-resolution BN layers, where
-    # the fp16 rounding of ~60 layers of gradient flow and of the forward activations has accumulated the most. The spread of
-    # the median is the summation ORDER of the batch statistics (3.4 % with 1024-row partials, 6.3 % with the 8-CTAs-per-SM
-    # grid; the BN operators themselves pass test_batchnorm_train_forward_backward unchanged): this synthetic network amplifies last-bit
+    # the worst deviations sit on the two earliest full-resolution BN layers, where the fp16 rounding of ~60 layers of
+    # gradient flow and of the forward activations has accumulated the most. The median moves with the summation ORDER of the
+    # batch statistics (partial-sum grid of the statistics kernels; the BN operators themselves pass
+    # test_batchnorm_train_forward_backward unchanged): this synthetic network amplifies last-bit
     # differences of the forward, which is what the fp16-forward emulation yardstick of
     # test_reference_training_loop_unchanged quantifies.
     assert devs[0][0] < 0.40, devs[:5]
@@ -775,9 +775,8 @@ def test_reference_training_loop_unchanged():
     # backward (torch autograd) evaluated on the oracle forward with only the kernels' fp16 rounding points emulated
     # (tools/grad_emulation_cpu.py). On this synthetic network (random weights + batch-statistics BN: the chaotic regime) that
     # alone moves the gradients to cos 0.87-0.98 in the backbone - the derivative is ill-conditioned in the point it is taken
-    # at, whatever computes it. The tape has to stay within 0.08 of that yardstick (measured gap 0.02-0.065, independent of
-    # the loss scale from 32 to 2048 - profiles/grad_fidelity_gpu_r02.txt: a different realisation of the forward rounding plus its own fp16
-    # gradient rounding), and the head, whose forward is two layers deep, has to be right outright.
+    # at, whatever computes it. The tape has to stay within 0.08 of that yardstick (a different realisation of the forward
+    # rounding plus its own fp16 gradient rounding), and the head, whose forward is two layers deep, has to be right outright.
     import json
     from conftest import GOLDEN
     yard = json.load(open(os.path.join(GOLDEN, "grad_cos_f16_forward_emulation.json")))["cos"]

@@ -1,4 +1,4 @@
-"""Timing of the conv backward building blocks (wgrad on MN-major tcgen05 operands, dgrad via the forward kernel) at the
+"""Timing of the conv backward building blocks (wgrad on MN-major wgmma operands, dgrad via the forward kernel) at the
 detector's 3x3 layer shapes, B = 8. One JSON line per shape (CUDA events, median of 7 after 3 warm-ups)."""
 import json
 import os

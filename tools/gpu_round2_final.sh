@@ -1,5 +1,5 @@
 #!/bin/bash
-# end-of-round measurement set on one B200: tests, smoke, both bench arms, B = 32, train step, ncu launch lists
+# end-of-round measurement set on one GPU: tests, smoke, both bench arms, B = 32, train step, ncu launch lists
 mkdir -p gpurun_out
 timeout 900 python -m pytest tests -q -m gpu --no-header 2>&1 | tail -15 > gpurun_out/fin_gputests.log
 python -c "import __graft_entry__ as g; g.smoke()" > gpurun_out/fin_smoke.log 2>&1
