@@ -25,14 +25,6 @@ const char* mf_last_error(void);
 int mf_version(void);
 /* 0 = wgmma tensor-core implicit GEMM (default, the product), 1 = CUDA-core cross-check kernels (diagnostics). */
 int mf_set_conv_impl(int impl);
-/* performance tunables (experiments; results never depend on them): id 0/1 = extra dynamic shared memory (bytes) for
- * DCN / conv CTAs (fewer resident CTAs, larger L1); id 2 = unused (was the first-generation non-persistent GEMM kernel, removed);
- * id 3 = 1 disables the TMA-store epilogue; id 4 = 1 disables the im2col-TMA A operand (cp.async gather instead); id 5 = 1 also uses
- * im2col TMA for Cin 8/16/32 (request-bound, slower); ids 6, 7 and 12 = unused (the A-stationary schedule, the DCN producer-warp
- * count and 256-column predictor tiles do not fit the sm_90a register / shared-memory budget); id 8 = 1 launches with programmatic
- * dependent launch (no measured gain under graph replay);
- * id 9 = 1 runs the fused head as 2-CTA clusters that TMA-multicast the 3x3 weight boxes (halves their L2->SM traffic). */
-int mf_set_tunable(int id, int value);
 /* N tile (16/32/64/128) the conv kernels use for `cout`; packed weights / scale / shift are padded to a multiple. */
 int mf_conv_block_n(int cout);
 
@@ -137,8 +129,9 @@ int mf_split_to_nchw_f32(const void* x, int x_ld, int x_lo, float* y, int B, int
  * w3_packed [nbranch*256, 9*Cin] fp16 (k = tap*Cin + c); w2_packed [nbranch*32, 256] fp16 (rows >= out_nch[i] zero);
  * bias2 [nbranch*32]; out_ptrs[i] = fp32 NCHW base pointer of branch i's first output channel (host array of device
  * pointers), out_ctot[i] = channel count of the tensor it points into, out_nch[i] <= 32 real channels.
- * hid_mask (nullable) [B*H*W] bytes: when given only pixels with a non-zero flag are stored to `hid` (mf_edge_mask marks the
- * border pixels the edge fusion gathers: ~830 of 30 720 per image, 245 MB less DRAM traffic per B = 8 forward). */
+ * hid_mask [B*H*W] bytes: only pixels with a non-zero flag are stored to `hid` (mf_edge_mask marks the border pixels the edge
+ * fusion gathers: ~830 of 30 720 per image, 245 MB less DRAM traffic per B = 8 forward). It may be NULL only when no branch
+ * has hid_col[i] >= 0; a branch with hid_col[i] >= 0 and a NULL mask is rejected. */
 int mf_head_fused(const void* x, int x_ld, int B, int H, int W, int Cin, const void* w3_packed, const void* w2_packed,
                   const float* scale, const float* shift, const float* bias2, int nbranch, void* const* out_ptrs,
                   const int* out_ctot, const int* out_nch, const int* hid_col, void* hid, int hid_ld,

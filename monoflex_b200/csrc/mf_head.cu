@@ -38,20 +38,12 @@ struct HeadParams {
   int hid_col[H_MAXBR];          // >= 0: hidden activations of this branch are stored at this column of `hid`
   __half* hid;                   // [M, hid_ld]
   int hid_ld;
-  const unsigned char* hid_mask; // [M] or null. Non-null: only flagged pixels are stored (the ~830 border pixels per image
-};                               // the edge fusion gathers), by per-thread stores instead of a TMA store of every tile
+  const unsigned char* hid_mask; // [M]: only flagged pixels are stored (the ~830 border pixels per image the edge fusion
+};                               // gathers); null only when no branch has hid_col >= 0
 
-// CL = true: launched as clusters of 2 CTAs that work on two consecutive m-tiles in lock-step. Every 3x3-weight (B) box is
-// then fetched from L2 ONCE per cluster - each CTA loads 64 of its 128 rows and TMA-multicasts them into both CTAs' stage -
-// which halves the B-operand L2->SM traffic. A stage is recycled only when the consumers of BOTH CTAs have released it
-// (each consumer warp arrives on the empty barrier of both CTAs).
-template <bool CL>
 __global__ void __launch_bounds__(H_THREADS, 1)
 head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-                  const __grid_constant__ CUtensorMap tmap_w2, const __grid_constant__ CUtensorMap tmap_hid,
-                  const __grid_constant__ HeadParams p) {
-  pdl_launch_dependents();
-  const int crank = CL ? static_cast<int>(cluster_ctarank()) : 0;
+                  const __grid_constant__ CUtensorMap tmap_w2, const __grid_constant__ HeadParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_smem = smem;
@@ -70,22 +62,20 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
   const int nkb = p.nkb;
 
   if (warp == 8 && lane == 0) {
-    tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_w2); tma_prefetch_desc(&tmap_hid);
-    for (int s = 0; s < H_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], CL ? 16 : 8); }
+    tma_prefetch_desc(&tmap_x); tma_prefetch_desc(&tmap_w); tma_prefetch_desc(&tmap_w2);
+    for (int s = 0; s < H_STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
     for (int a = 0; a < 2; ++a) { mbar_init(&w2_full[a], 1); mbar_init(&w2_empty[a], 8); }
     fence_mbar_init();
   }
   __syncthreads();
-  if (CL) cluster_sync_all();          // the peer's mbarriers are initialised before anything is multicast to them
-  pdl_wait();
 
   if (warp == 8) {
     // ================================================================ TMA producer (all lanes walk the loops, one issues)
     {
       int stage = 0, bc = 0;
       uint32_t phase = 0;
-      for (int mt = blockIdx.x; mt - crank < ntm; mt += gridDim.x) {   // CL: the pair runs the same trip count
-        const int m0 = (mt < ntm ? mt : 0) * HBM;                  // CL: an out-of-range partner tile re-reads tile 0 (discarded)
+      for (int mt = blockIdx.x; mt < ntm; mt += gridDim.x) {
+        const int m0 = mt * HBM;
         const int cn = m0 / HW, rem = m0 - cn * HW;
         const int cw = rem % p.W - 1, chh = rem / p.W - 1;          // 3x3, stride 1, pad 1
         for (int nt = 0; nt < ntn; ++nt) {
@@ -107,11 +97,7 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
               mbar_arrive_expect_tx(&full_bar[stage], H_ASTAGE + H_BSTAGE);
               tma_load_im2col_4d(smem_u32(a_smem + stage * H_ASTAGE), &tmap_x, &full_bar[stage], c0, cw, chh, cn,
                                  static_cast<uint16_t>(kx), static_cast<uint16_t>(ky));
-              if (CL)
-                tma_load_2d_mc(smem_u32(b_smem + stage * H_BSTAGE + crank * (HBN / 2) * 128), &tmap_w, &full_bar[stage],
-                               kb * HBK, nt * HBN + crank * (HBN / 2), static_cast<uint16_t>(3));
-              else
-                tma_load_2d(smem_u32(b_smem + stage * H_BSTAGE), &tmap_w, &full_bar[stage], kb * HBK, nt * HBN);
+              tma_load_2d(smem_u32(b_smem + stage * H_BSTAGE), &tmap_w, &full_bar[stage], kb * HBK, nt * HBN);
             }
             __syncwarp();
             c0 += HBK;
@@ -130,8 +116,7 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
     float d[HBN / 2], d2[16];
     int stage = 0, ti = 0;
     uint32_t phase = 0;
-    bool store_pending = false;
-    for (int mt = blockIdx.x; mt - crank < ntm; mt += gridDim.x) {   // CL: the pair runs the same trip count
+    for (int mt = blockIdx.x; mt < ntm; mt += gridDim.x) {
       for (int nt = 0; nt < ntn; ++nt, ++ti) {
         const int br = nt >> 1, h = nt & 1, n0 = nt * HBN, bcj = ti >> 1, buf = bcj & 1;   // ntn is even: tile parity == half
         gmma_fence();
@@ -146,20 +131,16 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
           gmma_wait<0>();
           gmma_hold(d);
           __syncwarp();
-          if (lane == 0) {
-            if (CL) { mbar_arrive_cluster(&empty_bar[stage], 0); mbar_arrive_cluster(&empty_bar[stage], 1); }
-            else mbar_arrive(&empty_bar[stage]);
-          }
+          if (lane == 0) mbar_arrive(&empty_bar[stage]);
           if (++stage == H_STAGES) { stage = 0; phase ^= 1; }
         }
         // ---- epilogue: affine + leaky -> fp16 staging (and the hidden rows the edge fusion gathers)
-        if (store_pending && threadIdx.x == 0) bulk_wait_read0();  // previous tile's TMA store has read the staging
         bar_sync_named(1, 256);
 #pragma unroll
         for (int hh = 0; hh < 2; ++hh) {
           const int row = wg * 64 + 16 * w + (lane >> 2) + 8 * hh;
           __half* hid_row = nullptr;                           // this thread's pixel is one the edge fusion will gather
-          if (p.hid_mask != nullptr && p.hid_col[br] >= 0) {
+          if (p.hid_col[br] >= 0) {
             const int m = mt * HBM + row;
             if (m < p.M && __ldg(p.hid_mask + m)) hid_row = p.hid + static_cast<long long>(m) * p.hid_ld + p.hid_col[br] + h * HBN;
           }
@@ -177,16 +158,6 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         }
         fence_proxy_async();
         bar_sync_named(1, 256);
-        if (threadIdx.x == 0) {
-          store_pending = false;
-          if (p.hid_col[br] >= 0 && p.hid_mask == nullptr) {   // unmasked: store the whole tile of hidden activations
-            const int col = p.hid_col[br] + h * HBN;
-            tma_store_2d(&tmap_hid, o_u, col, mt * HBM);
-            tma_store_2d(&tmap_hid, o_u + H_ASTAGE, col + 64, mt * HBM);
-            bulk_commit();
-            store_pending = true;
-          }
-        }
         // ---- stage 2: this warpgroup's 64 staged rows x the branch's 1x1 weights (K = 128 hidden channels of this half)
         if (h == 0) mbar_wait(&w2_full[buf], (bcj >> 1) & 1);
         gmma_fence();
@@ -221,10 +192,7 @@ head_fused_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_const
         }
       }
     }
-    if (store_pending && threadIdx.x == 0) bulk_wait0();
   }
-  __syncthreads();
-  if (CL) cluster_sync_all();          // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -244,7 +212,8 @@ static void* driver_fn(const char* name) {
 }
 
 // x: features [B*H*W, x_ld] fp16 (Cin channels used); w3: packed 3x3 weights [nbranch*256, 9*Cin]; w2: packed 1x1 weights
-// [nbranch*32, 256]; hid: [M, hid_ld] fp16 buffer receiving the hidden activations of the branches with hid_col >= 0.
+// [nbranch*32, 256]; hid: [M, hid_ld] fp16 buffer receiving the hidden activations of the branches with hid_col >= 0 at the
+// pixels hid_mask flags.
 int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* w3, const __half* w2,
                       const float* scale, const float* shift, const float* bias2, int nbranch, float* const* out,
                       const int* out_ctot, const int* out_nch, const int* hid_col, __half* hid, int hid_ld,
@@ -256,6 +225,9 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     set_error("head_fused: unsupported shape Cin=%d nbranch=%d", Cin, nbranch);
     return -1;
   }
+  for (int i = 0; i < nbranch; ++i) {
+    if (hid_col[i] >= 0 && hid_mask == nullptr) { set_error("head_fused: branch %d stores hidden rows but hid_mask is null", i); return -1; }
+  }
   HeadParams p;
   memset(&p, 0, sizeof(p));
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.M = B * H * W; p.nkb = 9 * Cin / 64; p.nbranch = nbranch;
@@ -265,7 +237,7 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     p.out[i] = out[i]; p.out_ctot[i] = out_ctot[i]; p.out_nch[i] = out_nch[i]; p.hid_col[i] = hid_col[i];
     if (out_nch[i] > 32) { set_error("head_fused: branch %d has %d > 32 output channels", i, out_nch[i]); return -1; }
   }
-  CUtensorMap tx, tw, tw2, th;
+  CUtensorMap tx, tw, tw2;
   {
     cuuint64_t gdim[4] = {static_cast<cuuint64_t>(Cin), static_cast<cuuint64_t>(W), static_cast<cuuint64_t>(H), static_cast<cuuint64_t>(B)};
     cuuint64_t gstr[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * W, static_cast<cuuint64_t>(x_ld) * 2 * W * H};
@@ -284,33 +256,21 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
   };
   const int K3 = 9 * Cin;
-  const bool cl = g_tunable[9] != 0;                       // 2-CTA clusters with multicast weight loads
-  if (!tiled2d(&tw, w3, K3, nbranch * 256, K3, 64, cl ? HBN / 2 : HBN) || !tiled2d(&tw2, w2, 256, nbranch * 32, 256, 64, 32) ||
-      !tiled2d(&th, hid, hid_ld, p.M, hid_ld, 64, HBM)) { set_error("head_fused: tiled tensor map failed"); return -1; }
+  if (!tiled2d(&tw, w3, K3, nbranch * 256, K3, 64, HBN) || !tiled2d(&tw2, w2, 256, nbranch * 32, 256, 64, 32)) {
+    set_error("head_fused: tiled tensor map failed");
+    return -1;
+  }
   static bool attr = false;
   if (!attr) {
-    if (check_cuda(cudaFuncSetAttribute(head_fused_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, H_SMEM), "head smem")) return -1;
-    if (check_cuda(cudaFuncSetAttribute(head_fused_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, H_SMEM), "head smem")) return -1;
+    if (check_cuda(cudaFuncSetAttribute(head_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, H_SMEM), "head smem")) return -1;
     attr = true;
   }
   int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int ntm = (p.M + HBM - 1) / HBM;
-  if (!cl) {
-    const int grid = ntm < nsm ? ntm : nsm;
-    return check_cuda(launch_k(head_fused_kernel<false>, dim3(grid), dim3(H_THREADS), H_SMEM, st, tx, tw, tw2, th, p), "head_fused launch");
-  }
-  int grid = (ntm + 1) & ~1;                               // whole pairs; an odd last tile gets an all-out-of-range partner
-  if (grid > (nsm & ~1)) grid = nsm & ~1;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(H_THREADS); cfg.dynamicSmemBytes = H_SMEM; cfg.stream = st;
-  cudaLaunchAttribute la[1];
-  la[0].id = cudaLaunchAttributeClusterDimension;
-  la[0].val.clusterDim.x = 2; la[0].val.clusterDim.y = 1; la[0].val.clusterDim.z = 1;
-  cfg.attrs = la; cfg.numAttrs = 1;
-  return check_cuda(cudaLaunchKernelEx(&cfg, head_fused_kernel<true>, tx, tw, tw2, th, p), "head_fused cluster launch");
+  const int grid = ntm < nsm ? ntm : nsm;
+  return check_cuda(launch_k(head_fused_kernel, dim3(grid), dim3(H_THREADS), H_SMEM, st, tx, tw, tw2, p), "head_fused launch");
 }
 
 }  // namespace mf

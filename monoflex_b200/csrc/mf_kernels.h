@@ -6,7 +6,7 @@
 
 namespace mf {
 
-enum { MODE_CONV = 0, MODE_DCN = 1, MODE_CONV_TMA = 2, MODE_CONV_PATCH = 4 };
+enum { MODE_CONV = 0, MODE_DCN = 1, MODE_CONV_TMA = 2 };
 enum { ACT_NONE = 0, ACT_RELU = 1, ACT_LEAKY = 2, ACT_OFFMASK = 3 };
 enum { OUT_F16_NHWC = 0, OUT_F32_NHWC = 1, OUT_F32_NCHW = 2 };
 
@@ -19,7 +19,6 @@ struct IgemmParams {
   int M;        // B*Ho*Wo
   int K_real;   // kh*kw*Cin
   int nkb;      // ceil(K_real / 64)
-  int kc;       // MODE_CONV_TMA: channels per im2col box (8/16/32/64), 64/kc taps per K block; 0 otherwise
   // DCN: per output pixel 18 offsets (dy,dx per tap) + 9 masks (already sigmoid-ed), fp32, row stride om_ld
   const float* offmask;
   int om_ld;

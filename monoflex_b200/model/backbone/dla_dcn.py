@@ -125,11 +125,14 @@ class DLA(nn.Module):
             inplanes = planes
         return nn.Sequential(*mods)
 
-    def plan(self, P, x8):
-        """DLA.forward (:324-331). x8: image already packed to NHWC fp16 with 8 channels (3 real + 5 zero)."""
-        import os
-        rows_ok = (len(self.level0) == 3 and len(self.level1) == 3 and self.channels[0] == 16 and x8.W % 2 == 0 and
-                   self.level1[0].stride[0] == 2 and os.environ.get("MF_NO_ROWS_STEM", "0") != "1" and not P.train)
+    def rows_stem(self, W, train):
+        """whether the stem (7x7, level0, stride-2 level1) runs on the row-segment kernel (csrc/mf_rows.cu): the DLA-34 stem
+        geometry at an even image width, inference only. The image packer depends on it too (see DLASeg.build_plan)."""
+        return (len(self.level0) == 3 and len(self.level1) == 3 and self.channels[0] == 16 and W % 2 == 0 and
+                self.level1[0].stride[0] == 2 and not train)
+
+    def plan(self, P, x8, rows_ok):
+        """DLA.forward (:324-331). x8: the packed image (see DLASeg.build_plan); rows_ok: self.rows_stem(x8.W, P.train)."""
         y = []
         if P.strict and rows_ok:
             # strict precision on the row-segment kernel: x8 is the image pair plane [hi3 | lo3 | 0 0] (mf_pack_image_pair8);
@@ -263,11 +266,11 @@ class DLASeg(nn.Module):
     def build_plan(self, B, H, W, device):
         strict = (not self.training) and self._precision() == "strict"
         P = engine.Plan(device, train=self.training, strict=strict)
-        import os
-        self._strict_rows = strict and os.environ.get("MF_NO_ROWS_STEM", "0") != "1" and W % 2 == 0
-        x8 = P.act(B, H, W, 8 if (self._strict_rows or not strict) else 16, split=False)
-        P.image_pack = "mf_pack_image_pair8" if self._strict_rows else ("mf_pack_image_split" if strict else "mf_pack_image")
-        levels = self.base.plan(P, x8)
+        rows = self.base.rows_stem(W, P.train)
+        # strict: the row-segment stem takes the 8-channel image pair plane, the generic stem the 16-channel split image
+        x8 = P.act(B, H, W, 8 if (rows or not strict) else 16, split=False)
+        P.image_pack = ("mf_pack_image_pair8" if rows else "mf_pack_image_split") if strict else "mf_pack_image"
+        levels = self.base.plan(P, x8, rows)
         ups = self.dla_up.plan(P, levels)
         y = [ups[i] for i in range(self.last_level - self.first_level)]   # the reference's .clone()s are not needed
         self.ida_up.plan(P, y, 0, len(y))
