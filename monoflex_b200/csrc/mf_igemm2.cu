@@ -43,8 +43,9 @@ struct Cfg2 {
   static constexpr int CHUNK = BLOCK_N >= 32 ? 32 : 16;         // accumulator hand-over unit (columns)
   static constexpr int ACC_LD = CHUNK + 4;                      // fp32 row stride of the chunk slot (conflict-free, see gmma_store_cols)
   static constexpr int ACC_BYTES = BM * ACC_LD * 4;
+  static constexpr int H2W_BYTES = EPI == 2 ? 32 * BLOCK_N * 4 : 0;   // HEAD2: the tile's 1x1 weights [32 outputs][BLOCK_N] fp32
   static constexpr int BUDGET = (CTAS_PER_SM == 2 ? 113 : 227) * 1024;
-  static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + 1024;
+  static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + H2W_BYTES + 1024;
   // ring depth: the shallower of the preferred depth and what the shared-memory budget leaves
   static constexpr int STAGES0 = (MODE == MODE_DCN ? 4 : (BLOCK_N >= 128 ? 5 : (BLOCK_N >= 64 ? 6 : (BLOCK_N >= 32 ? 5 : 6))));
   static constexpr int STAGES1 = (SPLIT && BLOCK_N >= 64) ? ((MODE == MODE_DCN && BLOCK_N < 128) ? STAGES0 : STAGES0 - 1) : STAGES0;
@@ -130,6 +131,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   float* sh_s = sc_s + BLOCK_N;
   uint8_t* prm_smem = reinterpret_cast<uint8_t*>(sh_s + BLOCK_N);      // MODE_DCN only: 9*128 sampling records (36 KB)
   const uint32_t acc_u = smem_u32(prm_smem + C::PRM_BYTES);           // chunk slot [128][ACC_LD] fp32
+  const uint32_t h2w_u = acc_u + C::ACC_BYTES;                         // HEAD2 only: [32][BLOCK_N] fp32 1x1 weights
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);      // warp-uniform for the compiler as well
   const int lane = threadIdx.x & 31;
@@ -184,6 +186,18 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
       if (et < BLOCK_N) {
         sts32f(sc_u + et * 4, __ldg(p.scale + n0 + et));
         sts32f(sh_u + et * 4, __ldg(p.shift + n0 + et));
+      }
+      if constexpr (HEAD2) {
+        // the 1x1 weights of this tile's BLOCK_N hidden channels, for every output of the branch: fetched once per tile while
+        // the consumers still run the tile's main loop, so the contraction below reads shared memory only. Read from global
+        // memory inside the output loop, they put a memory round trip on every pair of outputs while the consumers wait on
+        // the accumulator hand-over (the weights do not stay in the small L1 this kernel's shared memory leaves).
+        const int branch = n0 >> 8, nout = p.h2_nch[branch];
+        const float4* ws = reinterpret_cast<const float4*>(p.h2_w + static_cast<long long>(branch) * 32 * 256 + (n0 & 255));
+        for (int i = et; i < nout * (BLOCK_N / 4); i += EPI_THREADS) {
+          const int o = i / (BLOCK_N / 4), c4 = i - o * (BLOCK_N / 4);
+          sts128f(h2w_u + i * 16, __ldg(ws + o * 64 + c4));
+        }
       }
       bar_sync_named(1, EPI_THREADS);
 #pragma unroll
@@ -244,18 +258,18 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           if (mvalid) {
             const int bimg = m / HoWo, pix = m - bimg * HoWo;
             float* dst = p.h2_part + ((static_cast<long long>(plane) * p.B + bimg) * p.h2_ntot + p.h2_ch0[branch]) * HoWo + pix;
-            const float* wb = p.h2_w + static_cast<long long>(branch) * 32 * 256 + cin0;
+            const uint32_t wb = h2w_u + ch * CHUNK * 4;                                // staged at the tile's start
             // two outputs per pass (the second row of an odd tail re-reads the first and is not stored): 16 independent
-            // 16-byte weight loads in flight and four independent FMA chains per thread - the epilogue, not the tensor pipe,
+            // 16-byte shared-memory weight loads and four independent FMA chains per thread - the epilogue, not the tensor pipe,
             // is what the accumulator hand-over waits on once the MMA issue is tight
             for (int o = 0; o < nout; o += 2) {
-              const float* wr0 = wb + o * 256;
-              const float* wr1 = (o + 1 < nout) ? wr0 + 256 : wr0;
+              const uint32_t wr0 = wb + o * BLOCK_N * 4;
+              const uint32_t wr1 = (o + 1 < nout) ? wr0 + BLOCK_N * 4 : wr0;
               float4 wa[CHUNK / 4], wc[CHUNK / 4];
 #pragma unroll
               for (int i = 0; i < CHUNK / 4; ++i) {
-                wa[i] = __ldg(reinterpret_cast<const float4*>(wr0) + i);
-                wc[i] = __ldg(reinterpret_cast<const float4*>(wr1) + i);
+                wa[i] = lds128f(wr0 + i * 16);
+                wc[i] = lds128f(wr1 + i * 16);
               }
               float a0 = 0.f, a1 = 0.f, c0 = 0.f, c1 = 0.f;
 #pragma unroll
