@@ -110,6 +110,7 @@ class _predictor(nn.Module):
         head2 = not P.train and strict and hc == 256 and feat.C % 64 == 0 and \
             (H * W) % 4 == 0 and len(branches) <= 12 and self.num_classes <= 32 and \
             all(sum(h.weight.shape[0] for h in heads) <= 32 for heads in self.reg_heads)
+        ea = eb = hid_mask = None
         if head2:
             # ---- strict precision: the N = 2304 pair GEMM contracts the 1x1 heads in its epilogue from the fp32 accumulators
             # (csrc/mf_igemm2.cu EPI == 2); the 2.3 GB hidden map never reaches HBM, only its border pixels for the edge fusion
@@ -260,8 +261,10 @@ class _predictor(nn.Module):
         P.add("mf_sigmoid_clamp", lambda: (cls.data_ptr(), n_cls))
         P.finalize()
         P.cls, P.reg, P.hidden = cls, reg, hid
+        # the edge fusion's gathered rows [B,1,K+2,256] and the border-pixel mask of the hidden rows (None where not built)
+        P.ea, P.eb, P.hid_mask = ea, eb, hid_mask
         if P.train:       # what head_backward.predictor_backward needs: activations kept by the train-mode forward
-            P.ctx = dict(x=x, hid=hid, ea=ea if self.enable_edge_fusion else None, eb=eb if self.enable_edge_fusion else None,
+            P.ctx = dict(x=x, hid=hid, ea=ea, eb=eb,
                          bn={id(m): (raw, y, st, c0, cc) for (m, raw, y, st, c0, cc) in P.bn_saved}, K_edge=K_edge,
                          off_ch0=off_ch0, ch0s=ch0s)
         return P

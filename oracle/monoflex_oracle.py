@@ -211,25 +211,29 @@ def iabn(sd, p, x):
     return F.leaky_relu(bn_eval(sd, p, x, abs_weight=True), 0.01)
 
 
-def predictor(sd, features, edge_indices, edge_lens, p='heads.predictor', out_w=None, out_h=None, taps=None):
+def predictor(sd, features, edge_indices, edge_lens, p='heads.predictor', out_w=None, out_h=None, taps=None, stored=None):
     """_predictor.forward detector_predictor.py:121-165.
-    edge_indices int64 [B,K,2] (x,y); edge_lens int [B]."""
+    edge_indices int64 [B,K,2] (x,y); edge_lens int [B]. Runs in the dtype of `features` (float64 with a float64 `sd`).
+    stored: optional function applied to every intermediate an implementation keeps in memory between its stages (the
+    hidden activations of the nine branches, the gathered edge features, the edge Conv1d + BN output), e.g. an fp16 round
+    trip to model a reduced-precision implementation; identity by default."""
+    st = (lambda t: t) if stored is None else stored
     b, c, h, w = features.shape
     out_w = w if out_w is None else out_w
     out_h = h if out_h is None else out_h
-    feature_cls = iabn(sd, p + '.class_head.1', F.conv2d(features, sd[p + '.class_head.0.weight'], None, 1, 1))
+    feature_cls = st(iabn(sd, p + '.class_head.1', F.conv2d(features, sd[p + '.class_head.0.weight'], None, 1, 1)))
     output_cls = F.conv2d(feature_cls, sd[p + '.class_head.2.weight'], sd[p + '.class_head.2.bias'])
     regs = []
     for i, branch in enumerate(REG_BRANCHES):
-        rf = iabn(sd, '%s.reg_features.%d.1' % (p, i),
-                  F.conv2d(features, sd['%s.reg_features.%d.0.weight' % (p, i)], None, 1, 1))
+        rf = st(iabn(sd, '%s.reg_features.%d.1' % (p, i),
+                     F.conv2d(features, sd['%s.reg_features.%d.0.weight' % (p, i)], None, 1, 1)))
         for j, (ki, ch) in enumerate(branch):
             o = F.conv2d(rf, sd['%s.reg_heads.%d.%d.weight' % (p, i, j)], sd['%s.reg_heads.%d.%d.bias' % (p, i, j)])
             if REG_KEYS[ki] == '3d_offset':                                      # edge fusion :137-158
-                g = edge_indices.view(b, -1, 1, 2).float().clone()
+                g = edge_indices.view(b, -1, 1, 2).to(features.dtype).clone()
                 g[..., 0] = g[..., 0] / (out_w - 1) * 2 - 1
                 g[..., 1] = g[..., 1] / (out_h - 1) * 2 - 1
-                ef = F.grid_sample(torch.cat((feature_cls, rf), 1), g, align_corners=True).squeeze(-1)
+                ef = st(F.grid_sample(torch.cat((feature_cls, rf), 1), g, align_corners=True).squeeze(-1))
                 if taps is not None:
                     taps['edge_features'] = ef
 
@@ -240,10 +244,12 @@ def predictor(sd, features, edge_indices, edge_lens, p='heads.predictor', out_w=
                     else:
                         e = F.batch_norm(e, sd[q + '.1.running_mean'], sd[q + '.1.running_var'], sd[q + '.1.weight'],
                                          sd[q + '.1.bias'], False, 0.0, BN_EPS)
-                    return F.conv1d(e, sd[q + '.3.weight'], sd[q + '.3.bias'])
+                    return F.conv1d(st(e), sd[q + '.3.weight'], sd[q + '.3.bias'])
 
                 e_cls = trunc(p + '.trunc_heatmap_conv', ef[:, :256])
                 e_off = trunc(p + '.trunc_offset_conv', ef[:, 256:])
+                if taps is not None:
+                    taps['e_cls'], taps['e_off'] = e_cls, e_off
                 for k in range(b):
                     n = int(edge_lens[k])
                     ek = edge_indices[k, :n]
