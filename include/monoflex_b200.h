@@ -88,14 +88,16 @@ int mf_dcn_nhwc_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W, in
                       const void* w_packed, int n_pad, int k_pad, int Cout, const float* scale, const float* shift, int act,
                       void* y, int y_ld, int y_lo, void* stream);
 /* Strict-precision predictor (detector_predictor.py:62-132 class head + regression heads): the nbranch 3x3 convs (Cin -> 256 each,
- * IABN + leaky folded into scale / shift / act) run as ONE pair GEMM with N = nbranch*256, and the 1x1 heads are contracted in
- * its epilogue from the fp32 accumulators (w2 [nbranch][32][256] fp32, branch b owns out_nch[b] <= 32 channels starting at
- * out_ch0[b] of the ntot = num_classes + num_reg combined maps). The epilogue writes partial sums to part [8][B][ntot][H*W] fp32
- * (8 = 256 hidden channels / 32 per epilogue thread); mf_head2_reduce adds the planes in a fixed order plus the bias into the
- * NCHW cls / reg maps, so results are run-to-run identical. Hidden pair rows reach HBM only for branches with hid_col[b] >= 0
- * (hi block at that column of `hid`, lo block hid_lo further) and only at pixels flagged in hid_mask (mf_edge_mask). */
+ * IABN + leaky folded into scale / shift / act, act must be leaky) run as ONE pair GEMM with N = nbranch*256, and the 1x1 heads
+ * are contracted on the tensor cores straight from its accumulators, as fp16 pairs like every strict layer (w2: the 1x1 weights
+ * [nbranch*32, 256, 1, 1] packed by mf_pack_conv_weight_split with k_pad = 768; branch b owns rows 32 b .. 32 b + out_nch[b] - 1,
+ * out_nch[b] <= 32 channels starting at out_ch0[b] of the ntot = num_classes + num_reg combined maps). The kernel writes partial
+ * sums to part [2][B][ntot][H*W] fp32 (one plane per 128-channel half of a branch's 256 hidden channels); mf_head2_reduce adds
+ * the two planes in a fixed order plus the bias into the NCHW cls / reg maps, so results are run-to-run identical. Hidden pair
+ * rows reach HBM only for branches with hid_col[b] >= 0 (hi block at that column of `hid`, lo block hid_lo further) and only
+ * at pixels flagged in hid_mask (mf_edge_mask). */
 int mf_head_conv_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W, int Cin, const void* w_packed, int n_pad, int k_pad,
-                       int nbranch, const float* scale, const float* shift, int act, const float* w2, float* part, int ntot,
+                       int nbranch, const float* scale, const float* shift, int act, const void* w2, float* part, int ntot,
                        const int* out_nch, const int* out_ch0, const int* hid_col, void* hid, int hid_ld, int hid_lo,
                        const unsigned char* hid_mask, void* stream);
 int mf_head2_reduce(const float* part, const float* bias, float* cls, float* reg, int B, int ncls, int nreg, int HW, void* stream);

@@ -187,7 +187,7 @@ int mf_conv2d_nhwc_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W,
   return launch_igemm2(p, static_cast<const __half*>(w_packed), n_pad, k_pad, MODE_CONV, MF_STREAM(stream));
 }
 int mf_head_conv_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W, int Cin, const void* w_packed, int n_pad, int k_pad,
-                       int nbranch, const float* scale, const float* shift, int act, const float* w2, float* part, int ntot,
+                       int nbranch, const float* scale, const float* shift, int act, const void* w2, float* part, int ntot,
                        const int* out_nch, const int* out_ch0, const int* hid_col, void* hid, int hid_ld, int hid_lo,
                        const unsigned char* hid_mask, void* stream) {
   IgemmParams p;
@@ -198,9 +198,9 @@ int mf_head_conv_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W, i
   p.split_in = 1; p.split_out = 0; p.x_lo = x_lo; p.cw = 64;
   p.K_real = 27 * Cin; p.nkb = (p.K_real + 63) / 64;
   p.Cout = nbranch * 256; p.scale = scale; p.shift = shift; p.act = act;
-  p.out_mode = OUT_F32_NCHW;                     // no output tensor map: the epilogue writes partial planes + masked hidden rows
+  p.out_mode = OUT_F32_NCHW;                     // no output tensor map: the consumers write partial planes + masked hidden rows
   p.y = hid; p.y_ld = hid_ld; p.y_lo = hid_lo;
-  p.h2_w = w2; p.h2_part = part; p.h2_ntot = ntot; p.h2_mask = hid_mask;
+  p.h2_w = static_cast<const __half*>(w2); p.h2_part = part; p.h2_ntot = ntot; p.h2_mask = hid_mask;
   bool need_hid = false;
   for (int i = 0; i < nbranch; ++i) {
     if (out_nch[i] < 0 || out_nch[i] > 32 || out_ch0[i] < 0 || out_ch0[i] + out_nch[i] > ntot) {

@@ -192,6 +192,17 @@ template <> struct Gmma<32> {
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
         : "l"(a), "l"(b), "r"(acc), "n"(TA), "n"(TB));
   }
+  // A from registers: a[0..3] = fp16 pairs (row 16 w + l / 4 + 8 (i & 1), columns 8 (i >> 1) + 2 (l % 4) + {0, 1}). That is
+  // the accumulator fragment layout above: columns [16 s, 16 s + 16) of an m64nN accumulator d are A = {d[8 s], d[8 s + 1]},
+  // {d[8 s + 2], d[8 s + 3]}, {d[8 s + 4], d[8 s + 5]}, {d[8 s + 6], d[8 s + 7]}, with no data movement between threads.
+  template <int TB>
+  MF_DEVINL static void mma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t acc) {
+    asm volatile(
+        "{\n.reg .pred p;\nsetp.ne.b32 p, %21, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(acc), "n"(TB));
+  }
 };
 template <> struct Gmma<64> {
   template <int TA, int TB>

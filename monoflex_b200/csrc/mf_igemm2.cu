@@ -18,6 +18,8 @@
 //                         -> one TMA store per 64-channel sub-tile (fp32 NHWC / NCHW outputs: direct stores)
 // Registers + the chunk slot act as a double buffer: the epilogue of tile i overlaps the main loop of tile i+1; the smem ring
 // and the barriers persist across tiles, so the per-tile cost is the MMA time, not a pipeline fill + drain.
+// HEAD2 (strict predictor, EPI == 2) has neither producer nor epilogue warps: the consumers contract the 1x1 heads from their
+// own accumulators on the tensor cores and store the results (see IgemmParams).
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 
@@ -29,7 +31,9 @@ static constexpr int A_STAGE = BM * BK * 2;   // 16 KB
 
 // SPLIT: the fp16 NHWC output is a hi/lo pair (strict-precision mode): two staging tiles per 64-channel sub-tile, paid for
 // with one pipeline stage (the K loop of a split layer is 3x longer, so the shallower ring costs nothing measurable).
-// EPI (see igemm2_kernel): 1 = SPLIT doubles the staging, 2 = HEAD2 has no output staging at all (256-column tiles fit).
+// EPI (see igemm2_kernel): 1 = SPLIT doubles the staging; 2 = HEAD2 has no output staging and no chunk slot, its staging area
+// holds the two slots of 1x1 head weights instead. HEAD2 at BLOCK_N = 128: FIXED = 32768 + 384 + 1024 + 1024 = 35200 B, and
+// (232448 - 35200) / (16384 + 16384) = 6.02, so a sixth ring stage fits (SMEM = 6 x 32768 + 35200 = 231808 B).
 template <int BLOCK_N, int MODE, int EPI = 0>
 struct Cfg2 {
   static constexpr bool SPLIT = EPI == 1;
@@ -37,17 +41,20 @@ struct Cfg2 {
   static constexpr int LAG = BLOCK_N >= 64 ? 3 : (BLOCK_N >= 32 ? 3 : 4);   // cp.async groups in flight per producer thread
   static constexpr int B_STAGE = BLOCK_N * BK * 2;
   static constexpr int OUT_HALF = BLOCK_N >= 64 ? (BLOCK_N / 64) * A_STAGE : 0;     // staging of one fp16 tile
-  static constexpr int OUT_STAGE = EPI == 2 ? 0 : (SPLIT ? 2 * OUT_HALF : OUT_HALF);
+  // HEAD2: one slot of split 1x1 head weights = 4 boxes [32 outputs][64 hidden channels] fp16, 128B-swizzled:
+  // W_hi of the tile's two 64-channel chunks, then W_lo of both
+  static constexpr int W1_BOX = 32 * BK * 2;
+  static constexpr int W1_STAGE = 4 * W1_BOX;
+  static constexpr int OUT_STAGE = EPI == 2 ? 2 * W1_STAGE : (SPLIT ? 2 * OUT_HALF : OUT_HALF);
   static constexpr int BAR_BYTES = 384;                         // barriers
   static constexpr int PRM_BYTES = MODE == MODE_DCN ? 9 * BM * 32 : 0;   // DCN sampling records
   static constexpr int CHUNK = BLOCK_N >= 32 ? 32 : 16;         // accumulator hand-over unit (columns)
   static constexpr int ACC_LD = CHUNK + 4;                      // fp32 row stride of the chunk slot (conflict-free, see gmma_store_cols)
-  static constexpr int ACC_BYTES = BM * ACC_LD * 4;
-  static constexpr int H2W_BYTES = EPI == 2 ? 32 * BLOCK_N * 4 : 0;   // HEAD2: the tile's 1x1 weights [32 outputs][BLOCK_N] fp32
+  static constexpr int ACC_BYTES = EPI == 2 ? 0 : BM * ACC_LD * 4;
   static constexpr int BUDGET = (CTAS_PER_SM == 2 ? 113 : 227) * 1024;
-  static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + H2W_BYTES + 1024;
+  static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + 1024;
   // ring depth: the shallower of the preferred depth and what the shared-memory budget leaves
-  static constexpr int STAGES0 = (MODE == MODE_DCN ? 4 : (BLOCK_N >= 128 ? 5 : (BLOCK_N >= 64 ? 6 : (BLOCK_N >= 32 ? 5 : 6))));
+  static constexpr int STAGES0 = (MODE == MODE_DCN ? 4 : (EPI == 2 ? 6 : (BLOCK_N >= 128 ? 5 : (BLOCK_N >= 64 ? 6 : (BLOCK_N >= 32 ? 5 : 6)))));
   static constexpr int STAGES1 = (SPLIT && BLOCK_N >= 64) ? ((MODE == MODE_DCN && BLOCK_N < 128) ? STAGES0 : STAGES0 - 1) : STAGES0;
   static constexpr int FIT = (BUDGET - FIXED) / (A_STAGE + B_STAGE);
   static constexpr int STAGES = STAGES1 < FIT ? STAGES1 : FIT;
@@ -80,8 +87,11 @@ struct ChunkDump {                         // compile-time walk over the chunks 
 };
 
 // warps of a CTA: NPW producers, 8 consumers, the weight-TMA warp (MODE_DCN: the producers issue the weight loads, which
-// keeps 640 threads and 96 registers for the consumers' 64 accumulators), 4 epilogue warps
-__host__ __device__ constexpr int igemm2_warps(int mode, int npw) { return npw + 8 + (mode == MODE_DCN ? 0 : 1) + 4; }
+// keeps 640 threads and 96 registers for the consumers' 64 accumulators), 4 epilogue warps (none for HEAD2, whose consumers
+// finish their own tiles)
+__host__ __device__ constexpr int igemm2_warps(int mode, int npw, int epi) {
+  return npw + 8 + (mode == MODE_DCN ? 0 : 1) + (epi == 2 ? 0 : 4);
+}
 
 template <int N>
 MF_DEVINL void act_chunk(float (&v)[N], int act, int nb) {
@@ -97,9 +107,10 @@ MF_DEVINL void act_chunk(float (&v)[N], int act, int nb) {
   }
 }
 
-// EPI: 0 = plain epilogue, 1 = SPLIT (staged hi/lo output tiles), 2 = HEAD2 (1x1 head contraction in the epilogue, see IgemmParams)
+// EPI: 0 = plain epilogue, 1 = SPLIT (staged hi/lo output tiles), 2 = HEAD2 (the consumers contract the 1x1 heads on the
+// tensor cores, see IgemmParams; no epilogue warps, NPW = 0). tmap_y: the output tiles, or for HEAD2 the split 1x1 weights.
 template <int BLOCK_N, int MODE, int NPW, int EPI>
-__global__ void __launch_bounds__(igemm2_warps(MODE, NPW) * 32, Cfg2<BLOCK_N, MODE, EPI>::CTAS_PER_SM)
+__global__ void __launch_bounds__(igemm2_warps(MODE, NPW, EPI) * 32, Cfg2<BLOCK_N, MODE, EPI>::CTAS_PER_SM)
 igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_y,
               const __grid_constant__ CUtensorMap tmap_x, const IgemmParams p, const int use_tma_store) {
   constexpr bool PTILE = MODE == MODE_DCN;               // m-tile = 16 x 8 patch of one image
@@ -107,13 +118,14 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   constexpr int EPI_THREADS = A_TMA ? 128 + NPW * 32 : 128;
   constexpr bool SPLIT = EPI == 1;
   constexpr bool HEAD2 = EPI == 2;
+  static_assert(!HEAD2 || (A_TMA && NPW == 0 && BLOCK_N == 128), "HEAD2: TMA-only warps, 128-column tiles");
   using C = Cfg2<BLOCK_N, MODE, EPI>;
   constexpr int STAGES = C::STAGES;
   constexpr int LAG = C::LAG;
   const bool split_out = SPLIT || p.split_out != 0;      // SPLIT == staged hi/lo tiles; narrow tiles store both halves directly
   constexpr int B_STAGE = C::B_STAGE;
   constexpr int NPT = NPW * 32;
-  constexpr int RPP = NPT / 8;
+  constexpr int RPP = NPT > 0 ? NPT / 8 : 1;
   constexpr int PASSES = BM / RPP;
   constexpr int W_TMA = NPW + 8;                                   // weight-TMA warp (not in MODE_DCN)
   constexpr int W_EPI = NPW + 8 + (MODE == MODE_DCN ? 0 : 1);      // first warp of epilogue group 0
@@ -127,11 +139,13 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* acc_full = empty_bar + STAGES;     // [2] chunk slot written (chunk parity)
   uint64_t* acc_empty = acc_full + 2;          // [1] chunk slot read
+  uint64_t* w1_full = acc_empty + 1;           // HEAD2: [2] 1x1 weight slot loaded
+  uint64_t* w1_empty = w1_full + 2;            // HEAD2: [2] 1x1 weight slot read by both consumer warpgroups
   float* sc_s = reinterpret_cast<float*>(o_smem + C::OUT_STAGE + C::BAR_BYTES);
   float* sh_s = sc_s + BLOCK_N;
   uint8_t* prm_smem = reinterpret_cast<uint8_t*>(sh_s + BLOCK_N);      // MODE_DCN only: 9*128 sampling records (36 KB)
   const uint32_t acc_u = smem_u32(prm_smem + C::PRM_BYTES);           // chunk slot [128][ACC_LD] fp32
-  const uint32_t h2w_u = acc_u + C::ACC_BYTES;                         // HEAD2 only: [32][BLOCK_N] fp32 1x1 weights
+  const uint32_t w1_u = smem_u32(o_smem);                              // HEAD2: two 1x1 weight slots (Cfg2::W1_STAGE)
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);      // warp-uniform for the compiler as well
   const int lane = threadIdx.x & 31;
@@ -144,7 +158,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
 
   if (warp == NPW && lane == 0) {
     tma_prefetch_desc(&tmap_w);
-    if (use_tma_store) tma_prefetch_desc(&tmap_y);
+    if (use_tma_store || HEAD2) tma_prefetch_desc(&tmap_y);
     if (A_TMA) tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], A_TMA ? 1 : NPT + 1);
@@ -153,6 +167,10 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
     mbar_init(&acc_full[0], 8);
     mbar_init(&acc_full[1], 8);
     mbar_init(&acc_empty[0], 128);                                 // a chunk is read by one epilogue group
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(&w1_full[s], 1);
+      mbar_init(&w1_empty[s], 8);
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -186,18 +204,6 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
       if (et < BLOCK_N) {
         sts32f(sc_u + et * 4, __ldg(p.scale + n0 + et));
         sts32f(sh_u + et * 4, __ldg(p.shift + n0 + et));
-      }
-      if constexpr (HEAD2) {
-        // the 1x1 weights of this tile's BLOCK_N hidden channels, for every output of the branch: fetched once per tile while
-        // the consumers still run the tile's main loop, so the contraction below reads shared memory only. Read from global
-        // memory inside the output loop, they put a memory round trip on every pair of outputs while the consumers wait on
-        // the accumulator hand-over (the weights do not stay in the small L1 this kernel's shared memory leaves).
-        const int branch = n0 >> 8, nout = p.h2_nch[branch];
-        const float4* ws = reinterpret_cast<const float4*>(p.h2_w + static_cast<long long>(branch) * 32 * 256 + (n0 & 255));
-        for (int i = et; i < nout * (BLOCK_N / 4); i += EPI_THREADS) {
-          const int o = i / (BLOCK_N / 4), c4 = i - o * (BLOCK_N / 4);
-          sts128f(h2w_u + i * 16, __ldg(ws + o * 64 + c4));
-        }
       }
       bar_sync_named(1, EPI_THREADS);
 #pragma unroll
@@ -250,57 +256,6 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           }
         }
         act_chunk<CHUNK>(v, p.act, nb);
-        if constexpr (HEAD2) {
-          // ---- 1x1 heads of this branch on the fp32 hidden values of this thread's pixel (32 of the branch's 256 channels)
-          const int branch = n0 >> 8, cin0 = (n0 & 255) + ch * CHUNK;            // 256 hidden channels per branch
-          const int nout = p.h2_nch[branch];
-          const int plane = cin0 >> 5;
-          if (mvalid) {
-            const int bimg = m / HoWo, pix = m - bimg * HoWo;
-            float* dst = p.h2_part + ((static_cast<long long>(plane) * p.B + bimg) * p.h2_ntot + p.h2_ch0[branch]) * HoWo + pix;
-            const uint32_t wb = h2w_u + ch * CHUNK * 4;                                // staged at the tile's start
-            // two outputs per pass (the second row of an odd tail re-reads the first and is not stored): 16 independent
-            // 16-byte shared-memory weight loads and four independent FMA chains per thread - the epilogue, not the tensor pipe,
-            // is what the accumulator hand-over waits on once the MMA issue is tight
-            for (int o = 0; o < nout; o += 2) {
-              const uint32_t wr0 = wb + o * BLOCK_N * 4;
-              const uint32_t wr1 = (o + 1 < nout) ? wr0 + BLOCK_N * 4 : wr0;
-              float4 wa[CHUNK / 4], wc[CHUNK / 4];
-#pragma unroll
-              for (int i = 0; i < CHUNK / 4; ++i) {
-                wa[i] = lds128f(wr0 + i * 16);
-                wc[i] = lds128f(wr1 + i * 16);
-              }
-              float a0 = 0.f, a1 = 0.f, c0 = 0.f, c1 = 0.f;
-#pragma unroll
-              for (int i = 0; i < CHUNK / 4; i += 2) {
-                a0 += v[4 * i] * wa[i].x + v[4 * i + 1] * wa[i].y + v[4 * i + 2] * wa[i].z + v[4 * i + 3] * wa[i].w;
-                a1 += v[4 * i + 4] * wa[i + 1].x + v[4 * i + 5] * wa[i + 1].y + v[4 * i + 6] * wa[i + 1].z + v[4 * i + 7] * wa[i + 1].w;
-                c0 += v[4 * i] * wc[i].x + v[4 * i + 1] * wc[i].y + v[4 * i + 2] * wc[i].z + v[4 * i + 3] * wc[i].w;
-                c1 += v[4 * i + 4] * wc[i + 1].x + v[4 * i + 5] * wc[i + 1].y + v[4 * i + 6] * wc[i + 1].z + v[4 * i + 7] * wc[i + 1].w;
-              }
-              dst[static_cast<long long>(o) * HoWo] = a0 + a1;
-              if (o + 1 < nout) dst[static_cast<long long>(o + 1) * HoWo] = c0 + c1;
-            }
-            // hidden pair rows for the edge fusion: two branches only, border pixels only
-            const int hc = p.h2_hid_col[branch];
-            if (hc >= 0 && p.h2_mask[m] != 0) {
-              __half* yp = reinterpret_cast<__half*>(p.y) + static_cast<long long>(m) * p.y_ld + hc + cin0;
-#pragma unroll
-              for (int i = 0; i < CHUNK; i += 8) {
-                __half2 o[4], l[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  o[e] = __floats2half2_rn(v[i + 2 * e], v[i + 2 * e + 1]);
-                  const float2 h = __half22float2(o[e]);
-                  l[e] = __floats2half2_rn(v[i + 2 * e] - h.x, v[i + 2 * e + 1] - h.y);
-                }
-                *reinterpret_cast<uint4*>(yp + i) = *reinterpret_cast<uint4*>(o);
-                *reinterpret_cast<uint4*>(yp + p.y_lo + i) = *reinterpret_cast<uint4*>(l);
-              }
-            }
-          }
-        } else
         if (p.out_mode == OUT_F16_NHWC) {
           if (staged) {
             if constexpr (BLOCK_N >= 64) {
@@ -627,8 +582,25 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
     {
       int stage = 0;
       uint32_t phase = 0;
+      int tl = 0;                                       // HEAD2: tiles of this CTA so far (1x1 weight slot = tl & 1)
       for (int t = blockIdx.x; t < ntiles; t += gridDim.x) {
         const int n0 = (t % ntn) * BLOCK_N;
+        if constexpr (HEAD2) {
+          // the branch's split 1x1 weights for the tile's 128 hidden channels (K blocks 3c = W_hi and 3c + 2 = W_lo of the
+          // two 64-channel chunks c, rows = the branch's 32 outputs), before the tile's first K block
+          const int slot = tl & 1;
+          mbar_wait(&w1_empty[slot], ((tl >> 1) & 1) ^ 1);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&w1_full[slot], C::W1_STAGE);
+            const int kc = 3 * ((n0 & 255) >> 6), row = (n0 >> 8) * 32;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)                  // q = 2 lo + chunk
+              tma_load_2d(w1_u + slot * C::W1_STAGE + q * C::W1_BOX, &tmap_y, &w1_full[slot],
+                          (kc + 3 * (q & 1) + 2 * (q >> 1)) * BK, row);
+          }
+          __syncwarp();
+          ++tl;
+        }
         int cw = 0, chh = 0, cn = 0;
         if (A_TMA) {                              // coordinates of the tile's first output pixel in input space (incl. -pad)
           const int m0 = (t / ntn) * BM;
@@ -723,17 +695,99 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           release(&empty_bar[stage]);
           if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
-        // hand-over: one chunk slot, chunk parity selects the full barrier (with two epilogue groups each waits on its own)
-        ChunkDump<BLOCK_N, C::CHUNK, 0>::run(d, [&](int ch, auto store) {
-          mbar_wait(acc_empty, (fills & 1) ^ 1);
-          store(acc_u + wg * 64 * C::ACC_LD * 4, C::ACC_LD);
+        if constexpr (HEAD2) {
+          // ---- 1x1 heads on the tensor cores, straight from the accumulators: IABN affine + leaky ReLU, split into fp16
+          // pairs (the same expressions the hi/lo output of every strict layer uses), then per 16-channel k slice
+          // A_hi W_hi + A_lo W_hi + A_hi W_lo as m64n32k16 with A in registers (Gmma<32>::mma_rs), over the slot the
+          // weight-TMA warp filled at the tile's start
+          const int n0 = (t % ntn) * BLOCK_N, m_tile = t / ntn;
+          const int branch = n0 >> 8, nout = p.h2_nch[branch];
+          const int tq = lane & 3;
+          const int row0 = m_tile * BM + wg * 64 + ((warp - NPW) & 3) * 16 + (lane >> 2);   // rows row0 and row0 + 8
+          uint32_t ahi[BLOCK_N / 16][4], alo[BLOCK_N / 16][4];
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            const float2 s2 = __ldg(reinterpret_cast<const float2*>(p.scale + n0 + 8 * j + 2 * tq));
+            const float2 h2 = __ldg(reinterpret_cast<const float2*>(p.shift + n0 + 8 * j + 2 * tq));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float v0 = d[4 * j + 2 * h] * s2.x + h2.x, v1 = d[4 * j + 2 * h + 1] * s2.y + h2.y;
+              v0 = fmaxf(v0, 0.01f * v0);
+              v1 = fmaxf(v1, 0.01f * v1);
+              const __half2 hi = __floats2half2_rn(v0, v1);
+              const float2 hf = __half22float2(hi);
+              const __half2 lo = __floats2half2_rn(v0 - hf.x, v1 - hf.y);
+              ahi[j >> 1][2 * (j & 1) + h] = *reinterpret_cast<const uint32_t*>(&hi);
+              alo[j >> 1][2 * (j & 1) + h] = *reinterpret_cast<const uint32_t*>(&lo);
+            }
+          }
+          // the next tile's first MMA does not read d (scale-d = 0), but its asm operands do: without this the old
+          // accumulators stay live through the tail, and ptxas spills and serializes every wgmma of the kernel
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 2; ++i) d[i] = 0.f;
+          const int slot = fills & 1;
+          mbar_wait(&w1_full[slot], (fills >> 1) & 1);
+          const uint32_t wb = w1_u + slot * C::W1_STAGE;
+          float o[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) o[i] = 0.f;
+          gmma_fence();
+#pragma unroll
+          for (int s = 0; s < BLOCK_N / 16; ++s) {
+            const uint32_t bw = wb + (s >> 2) * C::W1_BOX + (s & 3) * 32;
+            const uint64_t bhi = gmma_desc_sw128(bw), blo = gmma_desc_sw128(bw + 2 * C::W1_BOX);
+            Gmma<32>::mma_rs<0>(o, ahi[s], bhi, s != 0 ? 1u : 0u);
+            Gmma<32>::mma_rs<0>(o, alo[s], bhi, 1u);
+            Gmma<32>::mma_rs<0>(o, ahi[s], blo, 1u);
+          }
+          gmma_commit();
+          gmma_wait<0>();
+          gmma_hold(o);
           __syncwarp();
-          if (lane == 0) mbar_arrive(&acc_full[ch & 1]);
+          if (lane == 0) mbar_arrive(&w1_empty[slot]);
           ++fills;
-        });
+          // partial sums of the tile's 128 hidden channels -> plane (n0 & 255) >> 7; o[4 j + 2 h + e] is output 8 j + 2 tq + e
+          // of row row0 + 8 h, so a quad's 8 rows fill one 32-byte sector of each output's plane
+          float* part = p.h2_part + (static_cast<long long>((n0 & 255) >> 7) * p.B * p.h2_ntot + p.h2_ch0[branch]) * HoWo;
+          const int hc = p.h2_hid_col[branch];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = row0 + 8 * h;
+            if (m < p.M) {
+              const int bimg = m / HoWo, pix = m - bimg * HoWo;
+              float* dst = part + static_cast<long long>(bimg) * p.h2_ntot * HoWo + pix;
+#pragma unroll
+              for (int j = 0; j < 4; ++j) {
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int oc = 8 * j + 2 * tq + e;
+                  if (oc < nout) dst[static_cast<long long>(oc) * HoWo] = o[4 * j + 2 * h + e];
+                }
+              }
+              // hidden pair rows for the edge fusion: two branches only, border pixels only
+              if (hc >= 0 && p.h2_mask[m] != 0) {
+                __half* yp = reinterpret_cast<__half*>(p.y) + static_cast<long long>(m) * p.y_ld + hc + (n0 & 255) + 2 * tq;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                  *reinterpret_cast<uint32_t*>(yp + 8 * j) = ahi[j >> 1][2 * (j & 1) + h];
+                  *reinterpret_cast<uint32_t*>(yp + p.y_lo + 8 * j) = alo[j >> 1][2 * (j & 1) + h];
+                }
+              }
+            }
+          }
+        } else {
+          // hand-over: one chunk slot, chunk parity selects the full barrier (with two epilogue groups each waits on its own)
+          ChunkDump<BLOCK_N, C::CHUNK, 0>::run(d, [&](int ch, auto store) {
+            mbar_wait(acc_empty, (fills & 1) ^ 1);
+            store(acc_u + wg * 64 * C::ACC_LD * 4, C::ACC_LD);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&acc_full[ch & 1]);
+            ++fills;
+          });
+        }
       }
     }
-  } else {
+  } else if constexpr (!HEAD2) {
     run_epilogue(0, (warp - W_EPI) * 32 + lane);          // first epilogue group (even chunks, or all of them)
   }
 }
@@ -803,12 +857,12 @@ static int launch2_cfg(const CUtensorMap& tw, const CUtensorMap& ty, const CUten
   const int ntm = MODE == MODE_DCN ? p.B * ((p.H + 7) / 8) * ((p.W + 15) / 16) : (p.M + BM - 1) / BM;
   int grid = num_sms() * C::CTAS_PER_SM;
   if (grid > ntn * ntm) grid = ntn * ntm;
-  return check_cuda(launch_k(kern, dim3(grid), dim3(igemm2_warps(MODE, NPW) * 32), C::SMEM, st, tw, ty, tx, p,
+  return check_cuda(launch_k(kern, dim3(grid), dim3(igemm2_warps(MODE, NPW, EPI) * 32), C::SMEM, st, tw, ty, tx, p,
                              use_tma_store),
                     "igemm2 launch");
 }
 
-// out[b, ch, pix] = bias[ch] + sum over the eight partial planes (fixed order: deterministic), ch < ncls -> cls, else reg
+// out[b, ch, pix] = bias[ch] + plane 0 + plane 1 (fixed order: deterministic), ch < ncls -> cls, else reg
 __global__ void head2_reduce_kernel(const float* __restrict__ part, const float* __restrict__ bias, float* __restrict__ cls,
                                     float* __restrict__ reg, int B, int ncls, int nreg, int HW) {
   const int ntot = ncls + nreg;
@@ -816,11 +870,8 @@ __global__ void head2_reduce_kernel(const float* __restrict__ part, const float*
   const long long i = (static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x) * 4;
   if (i >= plane) return;
   float4 s = __ldg(reinterpret_cast<const float4*>(part + i));
-#pragma unroll
-  for (int q = 1; q < 8; ++q) {
-    const float4 t = __ldg(reinterpret_cast<const float4*>(part + q * plane + i));
-    s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
-  }
+  const float4 t = __ldg(reinterpret_cast<const float4*>(part + plane + i));
+  s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
   const long long row = i / HW;                       // HW % 4 == 0 is checked by the launcher: 4 elements share (b, ch)
   const int ch = static_cast<int>(row % ntot), b = static_cast<int>(row / ntot);
   const int pix = static_cast<int>(i - row * HW);
@@ -931,12 +982,21 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
     pp.pair = 1;                                                   // see IgemmParams::pair
     pp.nkb = 2 * p.kh * p.kw * (p.Cin / 64);
   }
-  if (p.h2_w != nullptr) {                     // HEAD2 epilogue: the strict-precision predictor GEMM (see IgemmParams)
-    if (!(a_tma && pp.pair && p.Cout % 256 == 0 && p.h2_part != nullptr && p.Cout / 256 <= 12)) {
-      set_error("igemm2 HEAD2: needs the pair-schedule TMA path and Cout a multiple of 256");
+  if (p.h2_w != nullptr) {                     // HEAD2: the strict-precision predictor GEMM (see IgemmParams)
+    if (!(a_tma && pp.pair && p.Cout % 256 == 0 && p.h2_part != nullptr && p.Cout / 256 <= 12 && p.act == ACT_LEAKY)) {
+      set_error("igemm2 HEAD2: needs the pair-schedule TMA path, Cout a multiple of 256 and the leaky activation");
       return -1;
     }
-    return launch2_cfg<128, MODE_CONV_TMA, 4, 2>(tw, ty, tx, pp, 0, st);
+    // the split 1x1 head weights [nbranch * 32][768]: boxes of 64 K x 32 outputs, 128B-swizzled like the B operand
+    cuuint64_t gdim[2] = {3 * 256, static_cast<cuuint64_t>(p.Cout / 256 * 32)};
+    cuuint64_t gstr[1] = {3 * 256 * 2};
+    cuuint32_t box[2] = {BK, 32};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(&ty, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(p.h2_w), gdim, gstr, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(1x1 head weights) failed (%d)", static_cast<int>(r)); return -1; }
+    return launch2_cfg<128, MODE_CONV_TMA, 0, 2>(tw, ty, tx, pp, 0, st);
   }
   if (p.split_out && use_tma_store) {          // staged hi/lo tiles: the SPLIT instantiations (N tiles of 64 / 128 only)
     if (mode == MODE_DCN && bn == 64) return launch2_cfg<64, MODE_DCN, 8, 1>(tw, ty, tx, pp, use_tma_store, st);

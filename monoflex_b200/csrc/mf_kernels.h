@@ -44,13 +44,15 @@ struct IgemmParams {
   // one third less operand traffic into shared memory than the K-concatenation (which loads A_hi and W_hi twice).
   // nkb then counts stage fills = 2 * taps * Cin / 64.
   int pair;
-  // HEAD2 epilogue (strict-precision predictor, EPI == 2 instantiation): this GEMM is the nine 3x3 head branches (N = nbranch x 256,
-  // 128-column tiles, IABN + leaky folded into scale / shift / act). Instead of storing the hidden tile, every epilogue thread
-  // contracts its 32 fp32 hidden values with the branch's 1x1 head weights (fp32, <= 32 outputs) and writes the partial dot
-  // products to plane (n_tile_in_branch * 4 + chunk) of `h2_part` [8][B][h2_ntot][Ho*Wo]; mf_head2_reduce sums the eight planes
-  // in a fixed order (+ bias) into the fp32 NCHW cls / reg maps. The hidden pair rows are stored only for the branches the edge
+  // HEAD2 (strict-precision predictor, EPI == 2 instantiation): this GEMM is the nine 3x3 head branches (N = nbranch x 256,
+  // 128-column tiles, IABN + leaky folded into scale / shift / act). Instead of storing the hidden tile, each consumer warpgroup
+  // turns its 64 x 128 accumulator into fp16 hi/lo pairs and contracts them with the branch's split 1x1 head weights (<= 32
+  // outputs) on the tensor cores, three products per k slice like every strict GEMM. The partial sums over the tile's 128
+  // hidden channels go to plane (n0 & 255) >> 7 of `h2_part` [2][B][h2_ntot][Ho*Wo]; mf_head2_reduce adds the two planes in a
+  // fixed order (+ bias) into the fp32 NCHW cls / reg maps. The hidden pair rows are stored only for the branches the edge
   // fusion gathers (h2_hid_col >= 0) and only at the pixels flagged in h2_mask.
-  const float* h2_w;             // [nbranch][32][256] fp32, rows >= h2_nch[b] unused
+  const __half* h2_w;            // [nbranch * 32][768] fp16 pairs (mf_pack_conv_weight_split of [nbranch * 32, 256, 1, 1]),
+                                 // rows >= h2_nch[b] of a branch zero
   float* h2_part;
   int h2_ntot;                   // channels of the combined output (cls + reg = 53)
   int h2_nch[12], h2_ch0[12], h2_hid_col[12];

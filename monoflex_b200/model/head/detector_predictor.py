@@ -112,14 +112,14 @@ class _predictor(nn.Module):
             all(sum(h.weight.shape[0] for h in heads) <= 32 for heads in self.reg_heads)
         ea = eb = hid_mask = None
         if head2:
-            # ---- strict precision: the N = 2304 pair GEMM contracts the 1x1 heads in its epilogue from the fp32 accumulators
+            # ---- strict precision: the N = 2304 pair GEMM contracts the 1x1 heads on the tensor cores from its accumulators
             # (csrc/mf_igemm2.cu EPI == 2); the 2.3 GB hidden map never reaches HBM, only its border pixels for the edge fusion
             import ctypes
             nb = len(branches)
             w3, n_pad, k_pad = P.pack_weight(w_all, split=True)
             scale, shift = P.affine(nb * hc, n_pad, abn, None, abs_weight=True)
             ntot = self.num_classes + self.num_reg
-            head_w = torch.zeros(nb, 32, hc, dtype=torch.float32, device=dev)
+            head_w = torch.zeros(nb, 32, hc, dtype=torch.float32, device=dev)     # 32 output rows per branch, zero-padded
             head_bias = torch.zeros(ntot, dtype=torch.float32, device=dev)
             out_nch, out_ch0, hid_col = [], [], []
             head_lists = [[self.class_head[2]]] + [list(h) for h in self.reg_heads]
@@ -129,7 +129,9 @@ class _predictor(nn.Module):
                 head_w[i, :wcat.shape[0]] = wcat
                 head_bias[c0:c0 + wcat.shape[0]] = torch.cat([h.bias.detach().float() for h in heads])
                 out_nch.append(wcat.shape[0]); out_ch0.append(c0); hid_col.append(-1)
-            part = torch.empty(8, B, ntot, H * W, dtype=torch.float32, device=dev)
+            w1, _, k1_pad = P.pack_weight(head_w.reshape(nb * 32, hc, 1, 1), split=True)     # [W_hi | W_hi | W_lo] per 64 channels
+            assert k1_pad == 3 * hc
+            part = torch.empty(2, B, ntot, H * W, dtype=torch.float32, device=dev)
             P.edge_idx = torch.zeros(B, K_edge, 2, dtype=torch.long, device=dev)
             hid_buf = hid_mask = None
             if self.enable_edge_fusion:
@@ -139,11 +141,11 @@ class _predictor(nn.Module):
                 ow_, oh_ = self.output_width, self.output_height
                 P.add("mf_edge_mask", lambda: (P.edge_idx.data_ptr(), hid_mask.data_ptr(), B, K_edge, H, W, ow_, oh_))
             arr_nc, arr_c0, arr_hc = (ctypes.c_int * nb)(*out_nch), (ctypes.c_int * nb)(*out_ch0), (ctypes.c_int * nb)(*hid_col)
-            P.keep.extend([head_w, head_bias, part, hid_buf, hid_mask, arr_nc, arr_c0, arr_hc, cls, reg])
+            P.keep.extend([w1, head_bias, part, hid_buf, hid_mask, arr_nc, arr_c0, arr_hc, cls, reg])
             cin = feat.C
             P.add("mf_head_conv_f16x2", lambda: (
                 x.ptr(), x.ld, x.lo, B, H, W, cin, w3.data_ptr(), n_pad, k_pad, nb, scale.data_ptr(), shift.data_ptr(),
-                engine.ACT_LEAKY, head_w.data_ptr(), part.data_ptr(), ntot, ctypes.cast(arr_nc, ctypes.c_void_p),
+                engine.ACT_LEAKY, w1.data_ptr(), part.data_ptr(), ntot, ctypes.cast(arr_nc, ctypes.c_void_p),
                 ctypes.cast(arr_c0, ctypes.c_void_p), ctypes.cast(arr_hc, ctypes.c_void_p),
                 hid_buf.data_ptr() if hid_buf is not None else None, 4 * hc, 2 * hc,
                 hid_mask.data_ptr() if hid_mask is not None else None))
