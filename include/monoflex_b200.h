@@ -339,11 +339,17 @@ int mf_nms_hm(const float* heat, float* out, int planes, int H, int W, void* str
  * heat [B,C,H,W] fp32 (apply_sigmoid=1: raw logits), reg [B,R=50,H,W] fp32, calib [B,6] = f_u,f_v,c_u,c_v,b_x,b_y,
  * pad [B,2], size [B,2] = (W,H) of the padded image, dim_mean [C,3]. Workspaces ws_score/ws_idx: [B*C*K*8]
  * (stage 1 runs 8 CTAs per (image, class) plane; stage 2 merges their candidates).
- * Outputs: scores/clses/ys/xs [B,K] fp32, inds [B,K] int64, pois [B,K,R], result [B,K,14], count [B] = #(score>=thresh). */
+ * depth_mode selects the OUTPUT_DEPTH estimator (detector_infer.py:148-209): 0 soft, 1 hard, 2 mean, 3 oracle, 4 direct,
+ * 5 keypoints_avg, 6 keypoints_center, 7 keypoints_02, 8 keypoints_13. The oracle matches every detection against its
+ * own image's ground truth gt [B,G,7] = (valid, class, x1, y1, x2, y2, z); gt may be NULL for the other modes.
+ * Outputs: scores/clses/ys/xs [B,K] fp32, inds [B,K] int64, pois [B,K,R], result [B,K,14], count [B] = #(score>=thresh),
+ * depth_err [B,K] (estimated depth error), proj [B,K,2] (projected 3D centre on the map), min_unc [B,K] int32
+ * (argmax of 1/uncertainty over the four estimators in modes 0-3, -1 otherwise). */
 int mf_decode_detections(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
                          const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                         float* ws_score, int* ws_idx, float* scores, long long* inds, float* clses, float* ys, float* xs,
-                         float* pois, float* result, int* count, void* stream);
+                         int depth_mode, const float* gt, int G, float* ws_score, int* ws_idx, float* scores,
+                         long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
+                         float* depth_err, float* proj, int* min_unc, void* stream);
 
 /* ---- boundary B: the reference's native operator ABI (_ext, src/vision.cpp:4-9, src/dcn_v2.h:9-59) ------------ */
 /* at::Tensor dcn_v2_forward(input, weight, bias, offset, mask, kh,kw,sh,sw,ph,pw,dh,dw,deformable_group): fp32 NCHW,

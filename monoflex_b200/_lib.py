@@ -80,8 +80,8 @@ SIGNATURES = {
     "mf_preprocess_images_u8": [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P],
     "mf_draw_heatmaps": [_P, _I, _I, _I, _I, _I, _P, _P],
     "mf_nms_hm": [_P, _P, _I, _I, _I, _P],
-    "mf_decode_detections": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _P, _P, _P, _P, _P, _P, _P, _P, _P,
-                             _P, _P],
+    "mf_decode_detections": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _I, _P, _P, _P, _P, _P,
+                             _P, _P, _P, _P, _P, _P, _P, _P, _P],
     "mf_dcn_v2_forward": [_P, _P, _P, _P, _P, _P] + [_I] * 14 + [_P, _SZ, _P],
     "mf_dcn_v2_backward": [_P] * 11 + [_I] * 14 + [_P, _SZ, _P],
     "mf_dcn_v2_backward_workspace": [_I] * 14,

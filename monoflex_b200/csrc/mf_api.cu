@@ -496,10 +496,12 @@ int mf_nms_hm(const float* heat, float* out, int planes, int H, int W, void* str
 }
 int mf_decode_detections(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
                          const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                         float* ws_score, int* ws_idx, float* scores, long long* inds, float* clses, float* ys, float* xs,
-                         float* pois, float* result, int* count, void* stream) {
-  return launch_decode(heat, reg, calib, pad, size, dim_mean, B, C, H, W, R, K, thresh, apply_sigmoid, ws_score, ws_idx,
-                       scores, inds, clses, ys, xs, pois, result, count, MF_STREAM(stream));
+                         int depth_mode, const float* gt, int G, float* ws_score, int* ws_idx, float* scores,
+                         long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
+                         float* depth_err, float* proj, int* min_unc, void* stream) {
+  return launch_decode(heat, reg, calib, pad, size, dim_mean, B, C, H, W, R, K, thresh, apply_sigmoid, depth_mode, gt, G,
+                       ws_score, ws_idx, scores, inds, clses, ys, xs, pois, result, count, depth_err, proj, min_unc,
+                       MF_STREAM(stream));
 }
 
 int mf_dcn_v2_forward(const float* x, const float* w, const float* bias, const float* offset, const float* mask, float* y,

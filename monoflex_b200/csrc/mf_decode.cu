@@ -260,7 +260,53 @@ struct DecodeParams {
   float* pois;            // [B, K, R]
   float* result;          // [B, K, 14]
   int* count;             // [B]
+  // OUTPUT_DEPTH estimator (MF_DEPTH_* in mf_launch.h) and, for the oracle, the ground truth of every image:
+  // gt [B, G, 7] = (valid, class, x1, y1, x2, y2, z)
+  int depth_mode;
+  const float* gt;
+  int G;
+  float* depth_err;       // [B, K] estimated depth error of the chosen depth
+  float* proj;            // [B, K, 2] projected 3D centre on the output map (xs + off_x, ys + off_y)
+  int* min_unc;           // [B, K] argmax(1 / sigma) of the four estimators (ensemble modes), else -1
 };
+
+// The oracle of detector_infer.py:239-278 for one detection: start from the mean of the four estimators, match the
+// nearest GT centre of the same class (other classes count as distance 9999, first minimum), and if the 2D IoU
+// (engine/visualize_infer.py:23-27) is not below 0.5 take the estimator closest to the GT depth (first minimum).
+// A zero-area union gives a NaN IoU, which is not < 0.5, so the match is accepted as in the reference. An image without
+// valid GT keeps the mean (the reference calls argmin on an empty tensor there). The explicit _rn intrinsics keep the
+// compiler from contracting the distance and IoU arithmetic into FMAs, so it rounds like the reference's fp32 numpy.
+__device__ __forceinline__ void oracle_depth(const float* __restrict__ gt, int G, int cls, float x1, float y1, float x2,
+                                             float y2, const float* dep, const float* sig, float& depth, float& err) {
+  const float cx = __fmul_rn(__fadd_rn(x1, x2), 0.5f), cy = __fmul_rn(__fadd_rn(y1, y2), 0.5f);
+  int near = -1;
+  float best = 0.f;
+  for (int g = 0; g < G; ++g) {
+    const float* t = gt + g * 7;
+    if (t[0] == 0.f) continue;
+    const float dx = __fsub_rn(cx, __fmul_rn(__fadd_rn(t[2], t[4]), 0.5f));
+    const float dy = __fsub_rn(cy, __fmul_rn(__fadd_rn(t[3], t[5]), 0.5f));
+    const float dist = t[1] == static_cast<float>(cls) ? __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)) : 9999.f;
+    if (near < 0 || dist < best) { best = dist; near = g; }
+  }
+  if (near < 0) return;
+  const float* t = gt + near * 7;
+  const float iw = fmaxf(__fsub_rn(fminf(x2, t[4]), fmaxf(x1, t[2])), 0.f);
+  const float ih = fmaxf(__fsub_rn(fminf(y2, t[5]), fmaxf(y1, t[3])), 0.f);
+  const float inter = __fmul_rn(iw, ih);
+  const float uni = __fsub_rn(__fadd_rn(__fmul_rn(__fsub_rn(x2, x1), __fsub_rn(y2, y1)),
+                                        __fmul_rn(__fsub_rn(t[4], t[2]), __fsub_rn(t[5], t[3]))), inter);
+  const float iou = __fdiv_rn(inter, uni);
+  if (iou < 0.5f) return;
+  float de = fabsf(dep[0] - t[6]), bd = dep[0], bs = sig[0];
+#pragma unroll
+  for (int i = 1; i < 4; ++i) {
+    const float di = fabsf(dep[i] - t[6]);
+    if (di < de) { de = di; bd = dep[i]; bs = sig[i]; }
+  }
+  depth = bd;
+  err = bs;
+}
 
 // channel map runs/monoflex.yaml:27-28: 2d_dim 0:4 | 3d_offset 4:6 | corner_offset 6:26 | corner_uncertainty 26:29 |
 // 3d_dim 29:32 | ori_cls 32:40 | ori_offset 40:48 | depth 48 | depth_uncertainty 49
@@ -379,15 +425,50 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
     dep[i] = fminf(fmaxf(dep[i], 0.1f), 100.f);
     sig[i] = expf(q[26 + i - 1]);
   }
-  // soft ensemble detector_infer.py:176-198
-  float wsum = 0.f, wts[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) { wts[i] = 1.f / sig[i]; wsum += wts[i]; }
+  // OUTPUT_DEPTH selection detector_infer.py:148-209. The four ensemble modes report the estimator of largest weight
+  // 1 / sigma (first maximum, :185); `hard` takes its depth.
   float depth = 0.f, err = 0.f;
+  int min_unc = -1;
+  float dbest = dep[0], smin = sig[0];
+  if (p.depth_mode <= MF_DEPTH_ORACLE) {
+    float wbest = 1.f / sig[0];
+    min_unc = 0;
 #pragma unroll
-  for (int i = 0; i < 4; ++i) { const float wn = wts[i] / wsum; depth += dep[i] * wn; err += wn * sig[i]; }
-  // location :142-155 + kitti_utils.py:350-369
-  const float u = (xf + q[4]) * dr - padx, v = (yf + q[5]) * dr - pady;
+    for (int i = 1; i < 4; ++i) {
+      const float w = 1.f / sig[i];
+      if (w > wbest) { wbest = w; dbest = dep[i]; min_unc = i; }
+      smin = fminf(smin, sig[i]);
+    }
+  }
+  if (p.depth_mode == MF_DEPTH_SOFT) {
+    // soft ensemble :193-198
+    float wsum = 0.f, wts[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { wts[i] = 1.f / sig[i]; wsum += wts[i]; }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) { const float wn = wts[i] / wsum; depth += dep[i] * wn; err += wn * sig[i]; }
+  } else if (p.depth_mode == MF_DEPTH_HARD) {                   // :187-191
+    depth = dbest; err = smin;
+  } else if (p.depth_mode == MF_DEPTH_MEAN || p.depth_mode == MF_DEPTH_ORACLE) {   // :200-209
+    depth = (dep[0] + dep[1] + dep[2] + dep[3]) / 4.f; err = (sig[0] + sig[1] + sig[2] + sig[3]) / 4.f;
+    if (p.depth_mode == MF_DEPTH_ORACLE)
+      oracle_depth(p.gt + static_cast<long long>(b) * p.G * 7, p.G, cls, x1, y1, x2, y2, dep, sig, depth, err);
+  } else if (p.depth_mode == MF_DEPTH_DIRECT) {                 // :150-153
+    depth = dep[0]; err = sig[0];
+  } else if (p.depth_mode == MF_DEPTH_KEYPOINTS_AVG) {          // :156-158: mean over the three key-point depths
+    depth = (dep[1] + dep[2] + dep[3]) / 3.f; err = (sig[1] + sig[2] + sig[3]) / 3.f;
+  } else {                                                      // :160-170: keypoints_center / _02 / _13
+    const int i = p.depth_mode - MF_DEPTH_KEYPOINTS_CENTER + 1;
+    depth = i == 1 ? dep[1] : i == 2 ? dep[2] : dep[3];
+    err = i == 1 ? sig[1] : i == 2 ? sig[2] : sig[3];
+  }
+  p.depth_err[o] = err;
+  p.min_unc[o] = min_unc;
+  // projected 3D centre on the map (:125), then location :142-155 + kitti_utils.py:350-369
+  const float px = xf + q[4], py = yf + q[5];
+  p.proj[o * 2] = px;
+  p.proj[o * 2 + 1] = py;
+  const float u = px * dr - padx, v = py * dr - pady;
   const float lx = ((u - c_u) * depth) / f_u + b_x;
   float ly = ((v - c_v) * depth) / f_v + b_y;
   // multi-bin orientation :245-295: argmax over softmax(bin logits)[..., 1] (first max wins)
@@ -418,8 +499,17 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
 
 int launch_decode(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
                   const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                  float* s1_score, int* s1_idx, float* scores, long long* inds, float* clses, float* ys, float* xs,
-                  float* pois, float* result, int* count, cudaStream_t st) {
+                  int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores, long long* inds,
+                  float* clses, float* ys, float* xs, float* pois, float* result, int* count, float* depth_err,
+                  float* proj, int* min_unc, cudaStream_t st) {
+  if (depth_mode < 0 || depth_mode >= MF_DEPTH_MODES) {
+    set_error("decode: depth_mode %d is not one of the %d OUTPUT_DEPTH estimators", depth_mode, MF_DEPTH_MODES);
+    return -1;
+  }
+  if (depth_mode == MF_DEPTH_ORACLE && (gt == nullptr || G < 0)) {
+    set_error("decode: the oracle depth needs the ground-truth table gt [B, G, 7] (gt=%p, G=%d)", static_cast<const void*>(gt), G);
+    return -1;
+  }
   // score bits of the slab's pixels + the staged slab with its one-row halo
   auto smem_for = [&](int s) {
     const int items = ((H * W + s - 1) / s + S1_THREADS - 1) / S1_THREADS;
@@ -463,6 +553,7 @@ int launch_decode(const float* heat, const float* reg, const float* calib, const
   p.dim_mean = dim_mean; p.B = B; p.C = C; p.K = K; p.R = R; p.H = H; p.W = W; p.S = S; p.thresh = thresh; p.down_ratio = 4;
   p.scores = scores; p.inds = inds; p.clses = clses; p.ys = ys; p.xs = xs; p.pois = pois; p.result = result;
   p.count = count;
+  p.depth_mode = depth_mode; p.gt = gt; p.G = G; p.depth_err = depth_err; p.proj = proj; p.min_unc = min_unc;
   (void)launch_k(topk_decode_stage2_kernel, dim3(B), dim3(S2_THREADS), 0, st, p);
   return check_cuda(cudaGetLastError(), "topk_decode_stage2");
 }

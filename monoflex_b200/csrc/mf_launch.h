@@ -70,10 +70,17 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
 int launch_adamw_arena_dyn(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
                            void* dyn16, int check_finite, cudaStream_t st);
+// OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
+enum {
+  MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,
+  MF_DEPTH_KEYPOINTS_AVG = 5, MF_DEPTH_KEYPOINTS_CENTER = 6, MF_DEPTH_KEYPOINTS_02 = 7, MF_DEPTH_KEYPOINTS_13 = 8,
+  MF_DEPTH_MODES = 9
+};
 int launch_decode(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
                   const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                  float* s1_score, int* s1_idx, float* scores, long long* inds, float* clses, float* ys, float* xs,
-                  float* pois, float* result, int* count, cudaStream_t st);
+                  int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores, long long* inds,
+                  float* clses, float* ys, float* xs, float* pois, float* result, int* count, float* depth_err,
+                  float* proj, int* min_unc, cudaStream_t st);
 int launch_nms_hm(const float* hm, float* out, int planes, int H, int W, cudaStream_t st);
 int launch_pack_conv_weight_dgrad(const float* w, int Cout, int Cin, int kh, int kw, int cout_pad, int n_pad, int k_pad,
                                   __half* out, cudaStream_t st);

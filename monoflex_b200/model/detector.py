@@ -149,33 +149,35 @@ class KeypointDetector(nn.Module):
     # ------------------------------------------------------------------ CUDA-graph path
     def _forward_graph(self, x, targets):
         g = self._enqueue_graph(x, targets)
-        return self.heads.post_processor.finish(g['ws'], g['plan_h'].cls)
+        return self.heads.post_processor.finish(g['ws'], g['plan_h'].cls, g['plan_h'].reg)
 
     def _enqueue_graph(self, x, targets):
         pred, post = self.heads.predictor, self.heads.post_processor
         post.check_config()
         x = x.float().contiguous()
         k_edge = targets[0].get_field("edge_indices").shape[0]
-        key = (tuple(x.shape), x.device, k_edge, engine.fingerprint(self), post.det_threshold, post.max_detection, self.precision)
+        # per-call target fields of the decode: calib / pad / size and, for the oracle depth, the ground-truth table
+        meta = post.prepare_targets(targets, self.test, x.device)
+        key = (tuple(x.shape), x.device, k_edge, engine.fingerprint(self), post.det_threshold, post.max_detection, self.precision,
+               post.output_depth, tuple(tuple(m.shape) for m in meta))
         g = self._graph
         if g is None or g['key'] != key:
-            g = self._capture(x, targets, key)
+            g = self._capture(x, targets, key, meta)
         g['x'].copy_(x, non_blocking=True)
         pred.load_targets(g['plan_h'], targets)
-        meta = post.prepare_targets(targets, self.test, x.device)
         for dst, src in zip(g['meta'], meta):
             if dst.data_ptr() != src.data_ptr():
                 dst.copy_(src, non_blocking=True)
         g['graph'].replay()
         return g
 
-    def _capture(self, x, targets, key):
+    def _capture(self, x, targets, key, meta):
         pred, post = self.heads.predictor, self.heads.post_processor
         xs = x.clone()
         plan_b = self.backbone._plan_for(xs)
         plan_h = pred.plan_for(plan_b.output, key[2])
         pred.load_targets(plan_h, targets)
-        meta = tuple(t.clone() for t in post.prepare_targets(targets, self.test, x.device))
+        meta = tuple(t.clone() for t in meta)
 
         def body():
             self.backbone.run_plan(plan_b, xs)

@@ -38,18 +38,38 @@ class DecodeWorkspace(object):
         self.pois = torch.empty(B, K, R, **f)
         self.result = torch.empty(B, K, 14, **f)
         self.count = torch.empty(B, dtype=torch.int32, device=device)
+        self.depth_err = torch.empty(B, K, **f)
+        self.proj = torch.empty(B, K, 2, **f)
+        self.min_unc = torch.empty(B, K, dtype=torch.int32, device=device)
 
 
-def decode_detections(heat, reg, calib, pad, size, dim_mean, K, thresh, apply_sigmoid=False, ws=None):
-    """nms_hm + select_topk + select_point_of_interest + 3D decode in two kernels. All arguments are CUDA tensors."""
+# OUTPUT_DEPTH estimators of the decode kernel (detector_infer.py:148-209), in the order of the C ABI's `depth_mode`
+DEPTH_MODES = ('soft', 'hard', 'mean', 'oracle', 'direct', 'keypoints_avg', 'keypoints_center', 'keypoints_02',
+               'keypoints_13')
+ENSEMBLE_DEPTH_MODES = DEPTH_MODES[:4]
+
+
+def decode_detections(heat, reg, calib, pad, size, dim_mean, K, thresh, apply_sigmoid=False, ws=None, depth_mode='soft',
+                      gt=None):
+    """nms_hm + select_topk + select_point_of_interest + 3D decode in two kernels. All arguments are CUDA tensors.
+    `depth_mode` is one of DEPTH_MODES; 'oracle' needs `gt` [B, G, 7] fp32 = (valid, class, x1, y1, x2, y2, z) per
+    ground-truth slot of every image."""
     B, C, H, W = heat.shape
     R = reg.shape[1]
+    if depth_mode not in DEPTH_MODES:
+        raise ValueError("depth_mode %r is not one of %s" % (depth_mode, DEPTH_MODES))
+    if depth_mode == 'oracle':
+        if gt is None or gt.dim() != 3 or tuple(gt.shape[::2]) != (B, 7) or gt.dtype != torch.float32 \
+                or not gt.is_contiguous():
+            raise ValueError("the oracle depth needs gt as a contiguous float32 [B, G, 7] tensor")
     if ws is None or (ws.B, ws.C, ws.K, ws.R) != (B, C, K, R):
         ws = DecodeWorkspace(B, C, K, R, heat.device)
+    gt_ptr, G = (gt.data_ptr(), gt.shape[1]) if gt is not None else (None, 0)
     call("mf_decode_detections", heat.data_ptr(), reg.data_ptr(), calib.data_ptr(), pad.data_ptr(), size.data_ptr(),
-         dim_mean.data_ptr(), B, C, H, W, R, K, float(thresh), 1 if apply_sigmoid else 0, ws.ws_score.data_ptr(),
-         ws.ws_idx.data_ptr(), ws.scores.data_ptr(), ws.inds.data_ptr(), ws.clses.data_ptr(), ws.ys.data_ptr(),
-         ws.xs.data_ptr(), ws.pois.data_ptr(), ws.result.data_ptr(), ws.count.data_ptr(), stream())
+         dim_mean.data_ptr(), B, C, H, W, R, K, float(thresh), 1 if apply_sigmoid else 0, DEPTH_MODES.index(depth_mode),
+         gt_ptr, G, ws.ws_score.data_ptr(), ws.ws_idx.data_ptr(), ws.scores.data_ptr(), ws.inds.data_ptr(),
+         ws.clses.data_ptr(), ws.ys.data_ptr(), ws.xs.data_ptr(), ws.pois.data_ptr(), ws.result.data_ptr(),
+         ws.count.data_ptr(), ws.depth_err.data_ptr(), ws.proj.data_ptr(), ws.min_unc.data_ptr(), stream())
     return ws
 
 
