@@ -351,6 +351,36 @@ int mf_decode_detections(const float* heat, const float* reg, const float* calib
                          long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
                          float* depth_err, float* proj, int* min_unc, void* stream);
 
+/* ---- KITTI official metric (data/datasets/evaluation/kitti_object_eval_python/eval.py:644-726, rotate_iou.py) ---------
+ * Objects: float64 rows of MF_KITTI_OBJ values, CSR-packed per image (gt_off / dt_off: DEVICE int32 [n_img + 1]):
+ *   class code (0 Car, 1 Pedestrian, 2 Cyclist, 3 Van, 4 Person_sitting, 5 Truck by lower-cased name, MF_KITTI_DONTCARE for
+ *   exactly "DontCare", -1 otherwise), truncated, occluded, alpha, x1, y1, x2, y2, l, h, w, x, y, z, rotation_y, score.
+ * pair_off: DEVICE int64 [n_img] start of each image's detection x ground-truth block, n_pair = sum of n_dt_i * n_gt_i.
+ * mf_kitti_eval_overlaps: overlaps [3][n_pair] float64 = eval_class's per-image blocks overlaps[i][d, g] of metric 0 (2D,
+ *   float64), 1 (BEV, float32 rotated IoU) and 2 (3D, float32 ratio), row-major per image.
+ * mf_kitti_eval_statistics: flags, both compute_statistics passes and get_thresholds for all 18 * ncls configurations
+ *   (metric, class, difficulty, overlap set) of the HOST class list classes[ncls] (0..5, at most 8 entries). max_dt: the
+ *   largest detection count of one image (HOST value); images are matched with at most MF_KITTI_MAX_DT detections, a larger
+ *   max_dt is rejected. An image over the limit that max_dt understates is not matched and is reported in out's last slot. workspace: caller-owned, at least mf_kitti_eval_workspace(n_gt, n_dt, ncls) bytes, and it carries
+ *   the state into mf_kitti_eval_ap.
+ * mf_kitti_eval_ap: out float64 = recall, precision, aos [3][3 metric][ncls][3 difficulty][2 overlap set][41], then
+ *   AP [2 (R40, R11)][4 (bbox, bev, 3d, aos)][ncls][3][2], then compute_aos (first detection's alpha != -10), then the
+ *   detection count of the largest image over MF_KITTI_MAX_DT (0: none; otherwise the tables are not valid).
+ * mf_kitti_pack_results: the decode's rows [n, 14] fp32 (class, alpha, x1, y1, x2, y2, h, w, l, x, y, z, ry, score) as
+ *   generate_kitti_3d_detection writes and get_label_anno parses them: np.round(x, 4) in float32, widened. */
+#define MF_KITTI_OBJ 16
+#define MF_KITTI_DONTCARE 6
+#define MF_KITTI_MAX_DT 128
+size_t mf_kitti_eval_workspace(int n_gt, int n_dt, int ncls);
+int mf_kitti_pack_results(const float* rows, int n, double* out, void* stream);
+int mf_kitti_eval_overlaps(const double* gt, const int* gt_off, const double* dt, const int* dt_off,
+                           const long long* pair_off, int n_img, long long n_pair, double* overlaps, void* stream);
+int mf_kitti_eval_statistics(const double* gt, const int* gt_off, const double* dt, const int* dt_off,
+                             const long long* pair_off, int n_img, int n_gt, int n_dt, int max_dt, const double* overlaps,
+                             long long n_pair, const int* classes, int ncls, void* workspace, size_t ws_bytes,
+                             void* stream);
+int mf_kitti_eval_ap(const void* workspace, int n_gt, int n_dt, int ncls, double* out, void* stream);
+
 /* ---- boundary B: the reference's native operator ABI (_ext, src/vision.cpp:4-9, src/dcn_v2.h:9-59) ------------ */
 /* at::Tensor dcn_v2_forward(input, weight, bias, offset, mask, kh,kw,sh,sw,ph,pw,dh,dw,deformable_group): fp32 NCHW,
  * exact fp32 arithmetic (passes testcuda.py:check_zero_offset at 1e-10). y is caller-allocated [B,Cout,Ho,Wo]. */

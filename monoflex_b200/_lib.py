@@ -82,6 +82,11 @@ SIGNATURES = {
     "mf_nms_hm": [_P, _P, _I, _I, _I, _P],
     "mf_decode_detections": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _I, _P, _P, _P, _P, _P,
                              _P, _P, _P, _P, _P, _P, _P, _P, _P],
+    "mf_kitti_eval_workspace": [_I, _I, _I],
+    "mf_kitti_pack_results": [_P, _I, _P, _P],
+    "mf_kitti_eval_overlaps": [_P, _P, _P, _P, _P, _I, _LL, _P, _P],
+    "mf_kitti_eval_statistics": [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P, _LL, _P, _I, _P, _SZ, _P],
+    "mf_kitti_eval_ap": [_P, _I, _I, _I, _P, _P],
     "mf_dcn_v2_forward": [_P, _P, _P, _P, _P, _P] + [_I] * 14 + [_P, _SZ, _P],
     "mf_dcn_v2_backward": [_P] * 11 + [_I] * 14 + [_P, _SZ, _P],
     "mf_dcn_v2_backward_workspace": [_I] * 14,
