@@ -331,6 +331,24 @@ int mf_preprocess_images_u8(const void* const* src_ptrs, const int* hw4, const i
                             const float* mean3, const float* std3, int to_bgr, float* out_nchw, void* stream);
 int mf_draw_heatmaps(const int* obj6, int B, int max_objs, int ncls, int H, int W, float* hm, void* stream);
 
+/* ---- training-target encoding (data/datasets/kitti.py:126-179, 335-521 + augmentations.py:28-77, runs/monoflex.yaml only).
+ * mf_encode_targets: labels DEVICE float64 [B][M][MF_TARGET_LABEL_COLS] = valid, class id (0 Car, 1 Pedestrian, 2 Cyclist),
+ *   truncation, occlusion, xmin, ymin, xmax, ymax, h, w, l, tx, ty, tz, ry, 0 (slot = index in the class-filtered label list);
+ *   P2 DEVICE float64 [B][3][4]; sizes DEVICE int32 [B][2] = original (w, h) <= (W, H); flips DEVICE int32 [B] or NULL.
+ *   Writes hm fp32 [B][3][H/4][W/4]; obj fp32 [B*M][mf_loss_obj_cols()] and img fp32 [B][8] as mf_loss_forward reads them
+ *   (img from the flipped P2); alphas, reg_weight fp32 [B][M]; gt_bboxes fp32 [B][M][4]; occlusions, truncations float64
+ *   [B][M]; obj6 int32 [B][M][6] (mf_draw_heatmaps' table); P2_out float64 [B][3][4] (flipped); edge_indices int64 [B][K][2]
+ *   with K = 2 (W/4 + H/4) and edge_len int64 [B] (count - 1). status int32 [1] = number of objects the reference would raise
+ *   on (an edge object with two non-zero radii, an outside object whose 2D box centre is outside the image) plus images
+ *   larger than W x H; they are left out of every output. No host synchronisation.
+ * mf_encode_edges: edge_indices / edge_len alone (the test split's fields) for sizes [B][2]. */
+#define MF_TARGET_LABEL_COLS 16
+int mf_encode_targets(const double* labels, const double* P2, const int* sizes, const int* flips, int B, int M, int H, int W,
+                      float* hm, float* obj, float* img, float* alphas, float* gt_bboxes, float* reg_weight,
+                      double* occlusions, double* truncations, int* obj6, double* P2_out, long long* edge_indices,
+                      long long* edge_len, int* status, void* stream);
+int mf_encode_edges(const int* sizes, int B, int H, int W, long long* edge_indices, long long* edge_len, void* stream);
+
 /* nms_hm alone (model/layers/utils.py:45-58): out = heat * (maxpool3x3(heat) == heat), planes = B*C */
 int mf_nms_hm(const float* heat, float* out, int planes, int H, int W, void* stream);
 

@@ -23,6 +23,7 @@ import torch
 import torch.distributed as dist
 
 from . import solver
+from .targets import EncodedTargets
 
 
 class Trainer(object):
@@ -55,12 +56,16 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ eager step (the reference loop, line by line)
     def step(self, images, targets, sync_log=True):
-        """one optimisation step on a batch -> (loss_dict, log_loss_dict) of the forward that produced the gradients"""
+        """one optimisation step on a batch -> (loss_dict, log_loss_dict) of the forward that produced the gradients.
+        targets: the per-image ParamsLists, or the EncodedTargets of GpuTargetEncoder.encode"""
         if self.use_cuda_graph and self.iteration >= self.graph_warmup:
             return self._step_graph(images, targets, sync_log)
         model, opt = self.model, self.optimizer
         model.train()
-        loss_dict, log = model._forward_train(images, targets, sync_log=sync_log)
+        if isinstance(targets, EncodedTargets):
+            loss_dict, log = model._forward_train(images, targets.edge_targets(), prepared=targets.prepared, sync_log=sync_log)
+        else:
+            loss_dict, log = model._forward_train(images, targets, sync_log=sync_log)
         losses = sum(loss_dict.values())
         opt.zero_grad()
         losses.backward()                                            # fused loss backward -> tape bridge -> p.grad (arena views)
@@ -88,8 +93,11 @@ class Trainer(object):
         model, opt = self.model, self.optimizer
         dev = images.device
         pred, lossev = model.heads.predictor, model.heads.loss_evaluator
-        g = {"x": images.clone(), "prep": tuple(t.clone() for t in lossev.prepare_targets(targets, dev)),
-             "update_inside": self.world == 1 and opt._symm is None}
+        if isinstance(targets, EncodedTargets):
+            prep, targets = targets.prepared, targets.edge_targets()
+        else:
+            prep = lossev.prepare_targets(targets, dev)
+        g = {"x": images.clone(), "prep": tuple(t.clone() for t in prep), "update_inside": self.world == 1 and opt._symm is None}
         opt._lr_table()
         pred._targets_preloaded = True
         graph = torch.cuda.CUDAGraph()
@@ -119,9 +127,12 @@ class Trainer(object):
         if tuple(images.shape) != tuple(g["x"].shape):
             raise RuntimeError("captured training step: batch shape changed from %s to %s" % (tuple(g["x"].shape), tuple(images.shape)))
         g["x"].copy_(images, non_blocking=True)
-        for dst, src in zip(g["prep"], model.heads.loss_evaluator.prepare_targets(targets, images.device)):
-            dst.copy_(src, non_blocking=True)
-        model.heads.predictor.load_targets(g["plan_h"], targets)
+        if isinstance(targets, EncodedTargets):               # encoded straight into the step's static buffers
+            targets.encode_into(g["prep"], (g["plan_h"].edge_idx, g["plan_h"].edge_len))
+        else:
+            for dst, src in zip(g["prep"], model.heads.loss_evaluator.prepare_targets(targets, images.device)):
+                dst.copy_(src, non_blocking=True)
+            model.heads.predictor.load_targets(g["plan_h"], targets)
         opt._lr_table()                                              # in-place refresh when the scheduler moved the lr
         g["graph"].replay()
         if g["update_inside"]:
