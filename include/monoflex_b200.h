@@ -275,8 +275,9 @@ int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* 
  *       26-28 keypoints_depth_mask | 29-58 keypoints 10 x (x, y, visible)        (data/datasets/kitti.py:496-521)
  *   img [B,8] (device): f_u f_v c_u c_v b_x b_y pad_x pad_y;  weights11 / dim_mean9: HOST arrays (INIT_LOSS_WEIGHT in
  *       LOSS_NAMES order runs/monoflex.yaml:45-47, DIMENSION_MEAN config/defaults.py:206-208)
- *   out48 (device): [0..10] the 11 losses in LOSS_NAMES order; [16..26] 2D_IoU, depth_loss(log), keypoint_depth_loss(log),
- *       depth_MAE, center_MAE, 02_MAE, 13_MAE, lower_MAE, hard_MAE, soft_MAE, mean_MAE; [32..38] counts
+ *   out48 (device): [0..10] the 11 losses in LOSS_NAMES order; [16..27] 2D_IoU, depth_loss(log), keypoint_depth_loss(log),
+ *       depth_MAE, center_MAE, 02_MAE, 13_MAE, lower_MAE, hard_MAE, soft_MAE, mean_MAE, 3D_IoU (mean over the labelled
+ *       objects of get_iou_3d of the predicted and the label corners, 0 without objects); [32..38] counts
  *   ws64 (device): normalisers kept for the backward call.  No host synchronisation in either call.
  * mf_loss_backward: grad_losses11 (device) = upstream gradient of each loss (ones for the trainer's plain sum,
  * engine/trainer.py:109-110); writes grad_reg [B,50,H,W] (zero except at object centres) and grad_cls [B,ncls,H,W];
@@ -288,6 +289,13 @@ int mf_loss_forward(const float* pred_cls, const float* hm, const float* pred_re
 int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                      const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
                      const float* ws64, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream);
+
+/* get_iou_3d (model/layers/iou_loss.py:99-136): out[i] = float32 3D IoU of the boxes pred[i] and target[i], each given by its
+ * 8 corners in Anno_Encoder.encode_box3d's order (model/anno_encoder.py:88-122); pred, target [N,8,3] float32, out [N] float32,
+ * all device. The BEV overlap is clipped in float64; a ring counts as valid when its four turns are non-zero with one sign
+ * (DESIGN.md §9: a simple non-convex quadrilateral is invalid here, valid in shapely). NaN corners give NaN. One thread per
+ * pair; N = 0 launches nothing. */
+int mf_iou3d_corners(const float* pred, const float* target, long long n, float* out, void* stream);
 
 /* torch.optim.AdamW as configured by solver/__init__.py:10-37 (one param group per tensor, lr x BIAS_LR_FACTOR for
  * "bias" tensors, betas (0.9, 0.99), weight decay 1e-5) over ONE flat fp32 arena: every tensor starts at a multiple of

@@ -73,6 +73,7 @@ SIGNATURES = {
     "mf_loss_obj_cols": [],
     "mf_loss_forward": [_P] * 7 + [_I] * 6 + [_P, _P, _P],
     "mf_loss_backward": [_P] * 7 + [_I] * 6 + [_P, _P, _P, _P, _P],
+    "mf_iou3d_corners": [_P, _P, _LL, _P, _P],
     "mf_adamw_chunk": [],
     "mf_adamw_step_p2p": [_P, _P, _I, _I, ctypes.c_ulonglong, ctypes.c_ulonglong, _P, _P, _P, _LL, _F, _F, _F, _F, _LL, _F, _P],
     "mf_adamw_step_dyn": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],

@@ -5,7 +5,8 @@
 //
 // The reference runs ~300 micro-kernels and 14+ .item() host syncs per step for O(objects) arithmetic. Here:
 //   loss_forward_kernel  (1 CTA):   counts/normalisers -> per-object terms (one thread per object slot) -> deterministic
-//                                   block reduction -> 11 losses + 12 logged metrics in one device buffer (no host sync);
+//                                   block reduction -> 11 losses + 12 logged metrics (3D_IoU included, mf_iou3d.cuh) in one
+//                                   device buffer (no host sync);
 //   loss_backward_kernel (1 thread per (object, regression channel)): the SAME templated per-object function evaluated on
 //                                   forward-mode dual numbers seeded on that channel -> d(sum_k g_k loss_k)/d reg at the
 //                                   object's centre pixel, atomically added into grad_reg (objects may share a pixel).
@@ -13,7 +14,10 @@
 // abs / detach carries torch's sub-gradient convention in one place (the Dual overloads below).
 //
 // The heat-map term is the focal-loss pair of mf_train.cu / mf_elementwise.cu; this file only scales it.
+#include <type_traits>
+
 #include "mf_common.cuh"
+#include "mf_iou3d.cuh"
 #include "mf_launch.h"
 
 namespace mf {
@@ -89,7 +93,8 @@ enum {
 enum { T_BBOX = 0, T_DEPTH, T_OFF, T_TRUNC, T_ORI_CLS, T_ORI_REG, T_DIMS, T_CORNER, T_KP, T_KD_VALID, T_KD_INVALID, T_WAD, NTERM };
 // loss index (LOSS_NAMES order of runs/monoflex.yaml:45) each internal term belongs to
 __constant__ int kTermLoss[NTERM] = {1, 2, 3, 9, 4, 4, 5, 6, 7, 8, 8, 10};
-enum { L_IOU = 0, L_DEPTH_L1, L_KD_VALID_L1, L_DEPTH_MAE, L_MAE_C, L_MAE_02, L_MAE_13, L_LOWER, L_HARD, L_SOFT, L_MEAN, NLOG };
+enum { L_IOU = 0, L_DEPTH_L1, L_KD_VALID_L1, L_DEPTH_MAE, L_MAE_C, L_MAE_02, L_MAE_13, L_LOWER, L_HARD, L_SOFT, L_MEAN, L_IOU3D,
+       NLOG };
 
 struct LossCfg {
   float w[11];            // INIT_LOSS_WEIGHT in LOSS_NAMES order
@@ -238,6 +243,22 @@ __device__ void object_terms(const T* p, const float* __restrict__ o, const floa
     logs[L_SOFT] = fabsf(val(soft) - td) / td;
     logs[L_MEAN] = fabsf((val(pd) + val(kd[0]) + val(kd[1]) + val(kd[2])) * 0.25f - td) / td;
   }
+  // ---- 3D IoU of the two boxes (:333, get_iou_3d layers/iou_loss.py:99-136), logged only: the dual-number backward does
+  //      not instantiate it. The corners are the corner-loss expressions above, restated here so that the loss terms' code
+  //      (and therefore their rounding) is left as it was
+  if constexpr (std::is_same<T, float>::value) {
+    if (logs) {
+      float pc[24], tc[24];
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const float X = dims[0] * (0.5f * sx[k]), Y = dims[1] * (0.5f * sy[k]), Z = dims[2] * (0.5f * sz[k]);
+        const float tX = o[O_DIMS] * 0.5f * sx[k], tY = o[O_DIMS + 1] * 0.5f * sy[k], tZ = o[O_DIMS + 2] * 0.5f * sz[k];
+        pc[3 * k] = pcs * X + psn * Z + lx; pc[3 * k + 1] = Y + ly; pc[3 * k + 2] = -psn * X + pcs * Z + lz;
+        tc[3 * k] = tcs * tX + tsn * tZ + tlx; tc[3 * k + 1] = tY + tly; tc[3 * k + 2] = -tsn * tX + tcs * tZ + td;
+      }
+      logs[L_IOU3D] = iou3d_corners(pc, tc);
+    }
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ kernels
@@ -354,6 +375,7 @@ __global__ void __launch_bounds__(256) loss_forward_kernel(const float* __restri
     out[16 + 3] = lg[L_DEPTH_MAE] * i3;
     out[16 + 4] = lg[L_MAE_C] * i3; out[16 + 5] = lg[L_MAE_02] * i3; out[16 + 6] = lg[L_MAE_13] * i3;
     out[16 + 7] = lg[L_LOWER] * i3; out[16 + 8] = lg[L_HARD] * i3; out[16 + 9] = lg[L_SOFT] * i3; out[16 + 10] = lg[L_MEAN] * i3;
+    out[16 + 11] = lg[L_IOU3D] * i3;                                        // 3D_IoU (mean over the labelled objects)
     out[32] = n3; out[33] = n2d; out[34] = ntr; out[35] = nkp; out[36] = nkv; out[37] = nor; out[38] = focal2[1];
   }
 }

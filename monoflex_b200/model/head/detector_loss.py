@@ -7,8 +7,12 @@ of runs/monoflex.yaml:45 (views of one device buffer; ``sum(loss_dict.values()).
 runs the fused backward kernel), ``log_loss_dict`` the reference's logged scalars.
 
 Differences, on purpose:
-  * ONE device->host copy per call for the logged scalars instead of the reference's 14+ ``.item()`` syncs; the shapely-based
-    '3D_IoU' metric (detector_loss.py:333, CPU polygon clipping for logging only) is not computed (SURVEY §8c iii);
+  * ONE device->host copy per call for the logged scalars instead of the reference's 14+ ``.item()`` syncs;
+  * '3D_IoU' (detector_loss.py:333: the mean over the labelled objects of get_iou_3d of the predicted and the label corners,
+    shapely polygons in a Python loop there) is computed inside the forward loss kernel from the corners it already builds
+    for corner_loss, with the clip of csrc/mf_iou3d.cuh (float64 bird's-eye-view clip, the reference's float32 steps); no
+    extra launch, no host read. A simple non-convex ring counts as invalid there, valid in shapely (DESIGN.md §9);
+    encode_box3d never builds one. Without any labelled object the value is 0, like the other logged means;
   * only the runs/monoflex.yaml loss configuration is built - anything else raises NotImplementedError (no fallback).
 """
 import ctypes
@@ -18,8 +22,9 @@ import torch
 from ..._lib import call, load
 from ..layers.utils import Converter_key2channel
 
-LOG_KEYS = ['2D_IoU', 'depth_loss', 'keypoint_depth_loss', 'depth_MAE', 'center_MAE', '02_MAE', '13_MAE', 'lower_MAE',
-            'hard_MAE', 'soft_MAE', 'mean_MAE']
+LOG_KEYS = ['2D_IoU', '3D_IoU', 'depth_loss', 'keypoint_depth_loss', 'depth_MAE', 'center_MAE', '02_MAE', '13_MAE',
+            'lower_MAE', 'hard_MAE', 'soft_MAE', 'mean_MAE']                  # the reference's log_loss_dict order
+LOG_SLOTS = [0, 11, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10]        # out[16 + slot] of each LOG_KEYS entry, include/monoflex_b200.h
 OBJ_FIELDS = [("cls_ids", 1), ("target_centers", 2), ("2d_bboxes", 4), ("reg_mask", 1), ("trunc_mask", 1), ("dimensions", 3),
               ("locations", 3), ("rotys", 1), ("offset_3D", 2), ("orientations", 8), ("keypoints_depth_mask", 3),
               ("keypoints", 30)]          # column order of the packed label table, include/monoflex_b200.h
@@ -171,7 +176,7 @@ class DeferredLog(object):
             host = self._host
         else:
             host = torch.cat([out[:11], out[16:16 + len(LOG_KEYS)]]).cpu()                # the step's single D2H read
-        log_loss_dict = {k: float(host[11 + i]) for i, k in enumerate(LOG_KEYS)}
+        log_loss_dict = {k: float(host[11 + j]) for k, j in zip(LOG_KEYS, LOG_SLOTS)}
         for i, k in enumerate(REF_LOSS_NAMES):                                            # detector_loss.py:478-480
             if k not in log_loss_dict:
                 log_loss_dict[k] = float(host[i])
