@@ -311,6 +311,20 @@ int mf_adamw_chunk(void);
 int mf_adamw_step_dyn(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
                       long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
                       float lr_scale, long long* state4, void* dyn16, int check_finite, void* stream);
+/* mf_adamw_step_dyn with torch.nn.utils.clip_grad_norm_(params, max_norm) in front of the update (the reference's
+ * SOLVER.GRAD_NORM_CLIP, engine/trainer.py:119). The scan launch computes the float64 sum of squares of the gradient arena
+ * per CTA into partials (device double[(n_chunks + 1) / 2], scratch); the prepare launch reduces them in a fixed order and
+ * writes *total_norm_out (device float) = the 2-norm of grad_scale * grads, the value clip_grad_norm_ returns, and
+ * clip_coef = min(reciprocal(total_norm + 1e-6) * max_norm, 1) in torch's float32 steps. The update multiplies the
+ * gradient by clip_coef and, when clip_coef != 1, writes it back to grads (the arena keeps its convention: with
+ * grad_scale = 1/world it holds the clipped SUM). With check_finite, a total norm that is not finite skips the step
+ * (state4[2] += 1; params, moments and grads untouched). Chunks with chunk_lr 0 are neither updated nor rewritten.
+ * Deterministic: the partials depend on n_chunks only. max_norm <= 0 is exactly mf_adamw_step_dyn (partials and
+ * total_norm_out unused). */
+int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
+                           long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+                           float lr_scale, long long* state4, void* dyn16, int check_finite, float max_norm, double* partials,
+                           float* total_norm_out, void* stream);
 
 /* DDP gradient all-reduce (tools/plain_train_net.py:100-104) FUSED with the AdamW step for world > 1: one kernel over
  * peer-mapped memory. param_ptrs / grad_ptrs: HOST arrays [world] of device addresses of every rank's parameter / gradient

@@ -77,6 +77,7 @@ SIGNATURES = {
     "mf_adamw_chunk": [],
     "mf_adamw_step_p2p": [_P, _P, _I, _I, ctypes.c_ulonglong, ctypes.c_ulonglong, _P, _P, _P, _LL, _F, _F, _F, _F, _LL, _F, _P],
     "mf_adamw_step_dyn": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
+    "mf_adamw_step_dyn_clip": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _P, _P, _I, _F, _P, _P, _P],
     "mf_adamw_step": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _LL, _F, _F, _P],
     "mf_preprocess_images_u8": [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P],
     "mf_draw_heatmaps": [_P, _I, _I, _I, _I, _I, _P, _P],

@@ -473,8 +473,18 @@ int mf_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_
 int mf_adamw_step_dyn(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
                       long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
                       float lr_scale, long long* state4, void* dyn16, int check_finite, void* stream) {
+  // without clipping the gradient arena is only read
+  return launch_adamw_arena_dyn(params, const_cast<float*>(grads), exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps,
+                                weight_decay, grad_scale, lr_scale, state4, dyn16, check_finite, 0.f, nullptr, nullptr,
+                                MF_STREAM(stream));
+}
+int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
+                           long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
+                           float lr_scale, long long* state4, void* dyn16, int check_finite, float max_norm, double* partials,
+                           float* total_norm_out, void* stream) {
   return launch_adamw_arena_dyn(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps, weight_decay,
-                                grad_scale, lr_scale, state4, dyn16, check_finite, MF_STREAM(stream));
+                                grad_scale, lr_scale, state4, dyn16, check_finite, max_norm, partials, total_norm_out,
+                                MF_STREAM(stream));
 }
 int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
                       unsigned long long mc_params, unsigned long long mc_grads, float* exp_avg, float* exp_avg_sq,

@@ -67,9 +67,10 @@ int launch_focal_loss_backward(const float* pred, const float* tgt, long long n,
 int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                        float beta1, float beta2, float eps, float wd, long long step, float grad_scale, float lr_scale,
                        cudaStream_t st);
-int launch_adamw_arena_dyn(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
+int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
-                           void* dyn16, int check_finite, cudaStream_t st);
+                           void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out,
+                           cudaStream_t st);
 // OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
 enum {
   MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,

@@ -186,7 +186,73 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
 //                           (state[2] += 1). Either way it publishes (bc1, rsqrt_bc2, skip) and clears the flag;
 //   3. adamw_arena_dyn_kernel: the arena update, reading those three values from device memory.
 // state = long long[4]: [0] step count, [1] found-non-finite flag of the current step, [2] skipped steps, [3] unused.
-struct AdamwDyn { float bc1, rsqrt_bc2; int skip, pad; };
+//
+// With gradient-norm clipping (max_norm > 0; torch.nn.utils.clip_grad_norm_ between backward and step, the reference's
+// SOLVER.GRAD_NORM_CLIP, engine/trainer.py:119) the same three launches become:
+//   1. grad_sumsq_kernel  : each CTA writes the float64 sum of squares of its fixed grid-stride share of the arena to
+//                           partials[blockIdx.x] (the grid depends on n_chunks only, so the norm is run-to-run identical);
+//   2. adamw_prepare_clip_kernel (1 CTA): reduces the partials in a fixed order, total_norm = float(sqrt(sum) * grad_scale)
+//                           (the norm of the gradient the update uses: with an NCCL SUM in the arena, of the rank mean) and
+//                           clip_coef = min(reciprocal(total_norm + 1e-6) * max_norm, 1) in torch's float32 steps
+//                           (_clip_grads_with_norm_; `scalar / tensor` is `reciprocal() * scalar`). A norm that is not
+//                           finite is the finite guard's skip; otherwise the step bookkeeping above;
+//   3. adamw_arena_dyn_kernel<true>: g <- g * clip_coef, written back to the arena when clip_coef != 1 (p.grad then holds what
+//                           clip_grad_norm_ leaves there; torch's multiply by exactly 1 is exact, so nothing is written),
+//                           then the update as above.
+struct AdamwDyn { float bc1, rsqrt_bc2; int skip; float clip_coef; };
+
+__device__ __forceinline__ void adamw_prepare_step(long long* state, AdamwDyn* dyn, float beta1, float beta2, bool skip) {
+  if (skip) state[2] += 1; else state[0] += 1;
+  state[1] = 0;
+  const double step = static_cast<double>(state[0] < 1 ? 1 : state[0]);
+  const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
+  const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
+  dyn->bc1 = static_cast<float>(bc1);
+  dyn->rsqrt_bc2 = static_cast<float>(1.0 / sqrt(bc2));
+  dyn->skip = skip ? 1 : 0;
+}
+
+// sum over a 256-thread CTA in a fixed order (butterfly within each warp, then the 8 warp sums in order); valid in thread 0
+__device__ __forceinline__ double block_sum_256(double s, double* red8) {
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) s += __shfl_xor_sync(0xffffffffu, s, d);
+  if ((threadIdx.x & 31) == 0) red8[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = red8[0];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) s += red8[w];
+  }
+  return s;
+}
+
+__global__ void __launch_bounds__(256) grad_sumsq_kernel(const float* __restrict__ g, long long n_vec, double* __restrict__ partials) {
+  __shared__ double red[8];
+  double s = 0.0;
+  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(g) + i);
+    const double x = v.x, y = v.y, z = v.z, w = v.w;
+    s += x * x + y * y + z * z + w * w;
+  }
+  s = block_sum_256(s, red);
+  if (threadIdx.x == 0) partials[blockIdx.x] = s;
+}
+
+__global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2,
+                                                                 int check, const double* __restrict__ partials, int n_partials,
+                                                                 float grad_scale, float max_norm, float* total_norm_out) {
+  __shared__ double red[8];
+  double s = 0.0;
+  for (int i = threadIdx.x; i < n_partials; i += 256) s += partials[i];
+  s = block_sum_256(s, red);
+  if (threadIdx.x != 0) return;
+  const float norm = static_cast<float>(sqrt(s) * static_cast<double>(grad_scale));
+  *total_norm_out = norm;
+  adamw_prepare_step(state, dyn, beta1, beta2, check != 0 && !isfinite(norm));
+  const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
+  dyn->clip_coef = c > 1.f ? 1.f : c;                          // torch.clamp(max=1.0) keeps a NaN
+}
 
 __global__ void __launch_bounds__(256) grad_finite_kernel(const float* __restrict__ g, long long n_vec, long long* state) {
   bool bad = false;
@@ -201,23 +267,18 @@ __global__ void __launch_bounds__(256) grad_finite_kernel(const float* __restric
 }
 __global__ void adamw_prepare_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2, int check) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  const bool skip = check != 0 && state[1] != 0;
-  if (skip) state[2] += 1; else state[0] += 1;
-  state[1] = 0;
-  const double step = static_cast<double>(state[0] < 1 ? 1 : state[0]);
-  const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
-  const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
-  dyn->bc1 = static_cast<float>(bc1);
-  dyn->rsqrt_bc2 = static_cast<float>(1.0 / sqrt(bc2));
-  dyn->skip = skip ? 1 : 0;
+  adamw_prepare_step(state, dyn, beta1, beta2, check != 0 && state[1] != 0);
 }
-__global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict__ p, const float* __restrict__ g,
+// CLIP = false never writes g; chunks with lr 0 (padding-only, mark_unused) are neither updated nor clipped
+template <bool CLIP>
+__global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict__ p, float* __restrict__ g,
                                                               float* __restrict__ m, float* __restrict__ v,
                                                               const float* __restrict__ chunk_lr, long long n_chunks,
                                                               AdamwConsts k, const AdamwDyn* __restrict__ dyn) {
   if (dyn->skip) return;
   k.bc1 = dyn->bc1;
   k.rsqrt_bc2 = dyn->rsqrt_bc2;
+  const float coef = CLIP ? dyn->clip_coef : 1.f;
   constexpr int VEC_PER_CHUNK = MF_ADAMW_CHUNK / 4;
   const long long n_vec = n_chunks * VEC_PER_CHUNK;
   for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec;
@@ -225,7 +286,11 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
     const float lr = __ldg(chunk_lr + i / VEC_PER_CHUNK) * k.lr_scale;
     if (lr == 0.f) continue;
     float4 pp = reinterpret_cast<float4*>(p)[i];
-    const float4 gg = __ldcs(reinterpret_cast<const float4*>(g) + i);
+    float4 gg = __ldcs(reinterpret_cast<const float4*>(g) + i);
+    if (CLIP && coef != 1.f) {
+      gg.x *= coef; gg.y *= coef; gg.z *= coef; gg.w *= coef;
+      __stcs(reinterpret_cast<float4*>(g) + i, gg);
+    }
     float4 mm = reinterpret_cast<float4*>(m)[i];
     float4 vv = reinterpret_cast<float4*>(v)[i];
     adamw_update4(pp, gg, mm, vv, lr, k);
@@ -234,23 +299,37 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
     reinterpret_cast<float4*>(v)[i] = vv;
   }
 }
-int launch_adamw_arena_dyn(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
+// max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL)
+int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
-                           void* dyn16, int check_finite, cudaStream_t st) {
+                           void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out,
+                           cudaStream_t st) {
   if (n_chunks <= 0) return 0;
+  const bool clip = max_norm > 0.f;
+  if (clip && (partials == nullptr || total_norm_out == nullptr)) {
+    set_error("adamw_step_dyn_clip: max_norm > 0 needs the partials buffer and total_norm_out");
+    return -1;
+  }
   const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
-  long long blocks = (n_vec + 255) / 256;
+  long long blocks = (n_vec + 255) / 256;                       // <= (n_chunks + 1) / 2: the partials the caller provides
   const long long cap = 132LL * 8 * 4;
   if (blocks > cap) blocks = cap;
-  if (check_finite)
-    (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
-  (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, static_cast<AdamwDyn*>(dyn16), beta1, beta2, check_finite);
+  AdamwDyn* dyn = static_cast<AdamwDyn*>(dyn16);
+  if (clip) {
+    (void)launch_k(grad_sumsq_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, partials);
+    (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta1, beta2, check_finite, partials,
+                   static_cast<int>(blocks), grad_scale, max_norm, total_norm_out);
+  } else {
+    if (check_finite)
+      (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
+    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta1, beta2, check_finite);
+  }
   AdamwConsts k;
   k.beta1 = beta1; k.beta2 = beta2; k.eps = eps; k.wd = wd; k.bc1 = 1.f; k.rsqrt_bc2 = 1.f;
   k.grad_scale = grad_scale; k.lr_scale = lr_scale;
-  (void)launch_k(adamw_arena_dyn_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k,
-                 static_cast<const AdamwDyn*>(dyn16));
-  return check_cuda(cudaGetLastError(), "adamw_arena_dyn");
+  (void)launch_k(clip ? adamw_arena_dyn_kernel<true> : adamw_arena_dyn_kernel<false>, dim3(static_cast<unsigned>(blocks)),
+                 dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
+  return check_cuda(cudaGetLastError(), clip ? "adamw_arena_dyn_clip" : "adamw_arena_dyn");
 }
 
 // ---------------------------------------------------------------- focal loss backward (layers/focal_loss.py:35-55)

@@ -157,6 +157,9 @@ class FusedAdamW(torch.optim.Optimizer):
         dev = self.arena.params.device
         self._state4 = torch.zeros(4, dtype=torch.int64, device=dev)      # [step, found-non-finite, skipped steps, -]
         self._dyn16 = torch.zeros(4, dtype=torch.float32, device=dev)
+        # per-CTA sums of squares of the clipping scan (mf_adamw_step_dyn_clip), allocated once so step() stays capturable
+        self._norm_partials = torch.empty((self.arena.n_chunks + 1) // 2, dtype=torch.float64, device=dev)
+        self.last_grad_norm = torch.full((), float("nan"), dtype=torch.float32, device=dev)
         self._bind_state()
 
     # -- torch.optim plumbing ---------------------------------------------------------------------------------------
@@ -217,11 +220,20 @@ class FusedAdamW(torch.optim.Optimizer):
         return int(self._state4[2].item())
 
     @torch.no_grad()
-    def step(self, closure=None, grad_scale=1.0):
+    def step(self, closure=None, grad_scale=1.0, max_grad_norm=None):
+        """One AdamW update of the whole arena on `grad_scale * grads`.
+        max_grad_norm > 0: `torch.nn.utils.clip_grad_norm_(params, max_grad_norm)` first, on the device and inside the same
+        three launches (capturable): the norm of `grad_scale * grads` goes to `last_grad_norm` (a 0-d device tensor, the
+        value clip_grad_norm_ returns; read it without a sync), the gradient arena is left clipped like p.grad after
+        clip_grad_norm_ (still the SUM when grad_scale = 1/world), and a non-finite norm skips the step like any non-finite
+        gradient. None or <= 0 (the reference's GRAD_NORM_CLIP = -1): no clipping, `last_grad_norm` is not written."""
         if closure is not None:
             raise NotImplementedError("FusedAdamW: closures are not used by the reference trainer")
         if not self.arena.params.is_cuda:
             raise RuntimeError("FusedAdamW.step: parameters are not on a CUDA device (there is no CPU path)")
+        clip = max_grad_norm is not None and float(max_grad_norm) > 0
+        if clip and not self.capturable:
+            raise NotImplementedError("FusedAdamW.step: max_grad_norm needs the device-side step (capturable=True)")
         from . import _lib
         lib = _lib.load()
         if lib.mf_adamw_chunk() != self.arena.chunk:
@@ -238,10 +250,15 @@ class FusedAdamW(torch.optim.Optimizer):
         if self.capturable:
             if self.step_count == 1 and int(self._state4[0].item()) != 0:
                 raise RuntimeError("FusedAdamW: device step counter out of sync")
-            _lib.call("mf_adamw_step_dyn", self.arena.params.data_ptr(), self.arena.grads.data_ptr(), self.exp_avg.data_ptr(),
-                      self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1, b2, self.defaults["eps"],
-                      self.defaults["weight_decay"], float(grad_scale), 1.0, self._state4.data_ptr(), self._dyn16.data_ptr(),
-                      1 if self.check_finite else 0, torch.cuda.current_stream().cuda_stream)
+            args = (self.arena.params.data_ptr(), self.arena.grads.data_ptr(), self.exp_avg.data_ptr(),
+                    self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1, b2, self.defaults["eps"],
+                    self.defaults["weight_decay"], float(grad_scale), 1.0, self._state4.data_ptr(), self._dyn16.data_ptr(),
+                    1 if self.check_finite else 0)
+            if clip:
+                _lib.call("mf_adamw_step_dyn_clip", *args, float(max_grad_norm), self._norm_partials.data_ptr(),
+                          self.last_grad_norm.data_ptr(), torch.cuda.current_stream().cuda_stream)
+            else:
+                _lib.call("mf_adamw_step_dyn", *args, torch.cuda.current_stream().cuda_stream)
             self._step_t += 1
             for p in self.arena.tensors:
                 torch.autograd.graph.increment_version(p)

@@ -18,6 +18,14 @@ every parameter from its live storage, and nothing between the image copy and th
 temporaries, zero_grad and (single GPU) the guarded AdamW update - is captured ONCE in a CUDA graph and replayed; per step
 the host copies the batch and its labels into static buffers and launches one graph (multi-GPU: graph, NCCL all-reduce,
 AdamW).
+
+`cfg.SOLVER.GRAD_NORM_CLIP > 0` (the reference's clip_grad_norm_ between backward and step, engine/trainer.py:119): the eager
+step calls torch's `clip_grad_norm_` over the parameters, line for line like the reference. The captured step clips on the
+device instead (`FusedAdamW.step(max_grad_norm=...)`: the norm is accumulated by the scan of the gradient arena that also
+serves as the finite guard, and the coefficient is applied in the AdamW kernel, no host read), inside the graph on one GPU
+and in the update that follows the NCCL all-reduce on several, so it clips the rank mean as DDP + clip_grad_norm_ does.
+`optimizer.last_grad_norm` holds the norm of the last captured step. Not available with `symmetric_group` in the captured
+step (raises NotImplementedError): the fused peer-memory exchange has no cross-rank norm between its reduce and update.
 """
 import torch
 import torch.distributed as dist
@@ -31,6 +39,11 @@ class Trainer(object):
                  use_cuda_graph=False, graph_warmup=2):
         if not next(model.parameters()).is_cuda:
             raise RuntimeError("monoflex_b200 trains on sm_90a GPUs only; no CPU fallback")
+        self.grad_norm_clip = getattr(cfg.SOLVER, "GRAD_NORM_CLIP", -1)
+        if use_cuda_graph and self.grad_norm_clip > 0 and symmetric_group is not None:
+            raise NotImplementedError("GRAD_NORM_CLIP > 0 with symmetric_group: the fused peer-memory exchange (step_exchange) "
+                                      "has no cross-rank gradient norm between its reduce and its update; use the NCCL "
+                                      "exchange (no symmetric_group) or use_cuda_graph=False")
         self.model = model.train()
         if loss_scale is not None:
             model.loss_scale = float(loss_scale)
@@ -41,14 +54,11 @@ class Trainer(object):
         self.optimizer = solver.FusedAdamW(groups, lr=cfg.SOLVER.BASE_LR, weight_decay=cfg.SOLVER.WEIGHT_DECAY, betas=(0.9, 0.99),
                                            symmetric_group=symmetric_group)
         self.scheduler, _ = solver.build_scheduler(self.optimizer, cfg.SOLVER)
-        self.grad_norm_clip = getattr(cfg.SOLVER, "GRAD_NORM_CLIP", -1)
         self.iteration = 0
         self._unused_marked = False
         self.use_cuda_graph = bool(use_cuda_graph)
         self.graph_warmup = int(graph_warmup)
         self._graph = None
-        if self.use_cuda_graph and self.grad_norm_clip > 0:
-            raise NotImplementedError("GRAD_NORM_CLIP > 0 reads the norm on the host; not available in the captured step")
 
     @property
     def world(self):
@@ -79,14 +89,14 @@ class Trainer(object):
         self.iteration += 1
         return {k: v.detach() for k, v in loss_dict.items()}, log
 
-    def _exchange_and_update(self):
+    def _exchange_and_update(self, max_grad_norm=None):
         opt, world = self.optimizer, self.world
         if opt._symm is not None:
             opt.step_exchange()                                      # reduce + AdamW + broadcast in one peer-memory kernel
         else:
             if world > 1:
                 solver.allreduce_grads(opt.arena, self.bucket_bytes, self.group)
-            opt.step(grad_scale=1.0 / world)
+            opt.step(grad_scale=1.0 / world, max_grad_norm=max_grad_norm)   # clips the rank mean, as DDP + clip_grad_norm_
 
     # ------------------------------------------------------------------ captured step
     def _capture(self, images, targets):
@@ -109,7 +119,7 @@ class Trainer(object):
                 opt.zero_grad()
                 losses.backward()
                 if g["update_inside"]:
-                    opt.step(grad_scale=1.0)
+                    opt.step(grad_scale=1.0, max_grad_norm=self.grad_norm_clip)
         finally:
             pred._targets_preloaded = False
         if g["update_inside"]:                 # capture only records: undo the host-side bookkeeping of the captured step()
@@ -141,7 +151,7 @@ class Trainer(object):
             for p in opt.arena.tensors:
                 torch.autograd.graph.increment_version(p)
         else:
-            self._exchange_and_update()
+            self._exchange_and_update(max_grad_norm=self.grad_norm_clip)
         self.scheduler.step()
         self.iteration += 1
         return g["loss_dict"], (g["log"].resolve() if sync_log else g["log"].snapshot())
