@@ -325,6 +325,22 @@ int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* e
                            long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
                            float lr_scale, long long* state4, void* dyn16, int check_finite, float max_norm, double* partials,
                            float* total_norm_out, void* stream);
+/* The guarded (and optionally clipping) step of mf_adamw_step_dyn_clip for the reference's other SOLVER.OPTIMIZER values
+ * (solver/__init__.py:27-62), with the hyper-parameters a schedule moves every step read from device memory, so a captured
+ * graph follows them: hyper = device double[4] {lr_mult, beta1, weight_decay, unused}, rewritten in place by the host
+ * between launches / replays. The lr of a chunk is chunk_lr * lr_mult; bias correction 1 uses the current beta1
+ * (1 - beta1^step, as torch's Adam computes it from the group's betas each step). rule:
+ *   MF_OPTIM_ADAM  (1): torch.optim.Adam: g <- g + weight_decay * p (after clipping), then Adam ('adam');
+ *   MF_OPTIM_ADAMW (0): p <- p * (1 - lr * weight_decay), then Adam (AdamW; fastai OptimWrapper true_wd + Adam with
+ *                       weight_decay 0, 'adam_onecycle').
+ * A chunk with chunk_lr < 0 is decay-only under either rule: p <- p * (1 - |lr| * weight_decay), gradient and moments
+ * unread (a one-cycle grouped tensor whose gradient is None). chunk_lr 0: untouched. Finite guard, clipping (max_norm > 0,
+ * partials / total_norm_out as in mf_adamw_step_dyn_clip), state4 and dyn16 as in mf_adamw_step_dyn. */
+#define MF_OPTIM_ADAMW 0
+#define MF_OPTIM_ADAM 1
+int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
+                      long long n_chunks, const double* hyper, float beta2, float eps, float grad_scale, long long* state4,
+                      void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out, void* stream);
 
 /* DDP gradient all-reduce (tools/plain_train_net.py:100-104) FUSED with the AdamW step for world > 1: one kernel over
  * peer-mapped memory. param_ptrs / grad_ptrs: HOST arrays [world] of device addresses of every rank's parameter / gradient

@@ -79,6 +79,7 @@ SIGNATURES = {
     "mf_adamw_step_dyn": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _P, _P, _I, _P],
     "mf_adamw_step_dyn_clip": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _F, _F, _P, _P, _I, _F, _P, _P, _P],
     "mf_adamw_step": [_P, _P, _P, _P, _P, _LL, _F, _F, _F, _F, _LL, _F, _F, _P],
+    "mf_optim_step_dyn": [_I, _P, _P, _P, _P, _P, _LL, _P, _F, _F, _F, _P, _P, _I, _F, _P, _P, _P],
     "mf_preprocess_images_u8": [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P],
     "mf_draw_heatmaps": [_P, _I, _I, _I, _I, _I, _P, _P],
     "mf_encode_targets": [_P, _P, _P, _P, _I, _I, _I, _I] + [_P] * 14,

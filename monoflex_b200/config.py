@@ -32,5 +32,6 @@ def default_cfg(width=1280, height=384, device="cuda"):
                   EVAL_DIS_IOUS=False, EVAL_DEPTH=False)
     # runs/monoflex.yaml:61-78 over config/defaults.py:252-299
     cfg.SOLVER = NS(OPTIMIZER="adamw", BASE_LR=3e-4, WEIGHT_DECAY=1e-5, BIAS_LR_FACTOR=2.0, STEPS=(20000, 25000),
-                    LR_DECAY=0.1, LR_CLIP=1e-7, LR_WARMUP=False, GRAD_NORM_CLIP=-1, IMS_PER_BATCH=8)
+                    LR_DECAY=0.1, LR_CLIP=1e-7, LR_WARMUP=False, WARMUP_STEPS=2000, GRAD_NORM_CLIP=-1, IMS_PER_BATCH=8,
+                    MAX_ITERATION=30000, MOMS=[0.95, 0.85], PCT_START=0.4, DIV_FACTOR=10)
     return cfg

@@ -476,7 +476,7 @@ int mf_adamw_step_dyn(float* params, const float* grads, float* exp_avg, float* 
   // without clipping the gradient arena is only read
   return launch_adamw_arena_dyn(params, const_cast<float*>(grads), exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps,
                                 weight_decay, grad_scale, lr_scale, state4, dyn16, check_finite, 0.f, nullptr, nullptr,
-                                MF_STREAM(stream));
+                                MF_OPTIM_ADAMW, nullptr, MF_STREAM(stream));
 }
 int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
                            long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
@@ -484,6 +484,14 @@ int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* e
                            float* total_norm_out, void* stream) {
   return launch_adamw_arena_dyn(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps, weight_decay,
                                 grad_scale, lr_scale, state4, dyn16, check_finite, max_norm, partials, total_norm_out,
+                                MF_OPTIM_ADAMW, nullptr, MF_STREAM(stream));
+}
+int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
+                      long long n_chunks, const double* hyper, float beta2, float eps, float grad_scale, long long* state4,
+                      void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out, void* stream) {
+  if (hyper == nullptr) { set_error("optim_step_dyn: hyper (device double[4]) is NULL"); return -1; }
+  return launch_adamw_arena_dyn(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, 0.f, beta2, eps, 0.f, grad_scale, 1.f,
+                                state4, dyn16, check_finite, max_norm, partials, total_norm_out, rule, hyper,
                                 MF_STREAM(stream));
 }
 int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,

@@ -62,6 +62,8 @@ int launch_adamw_p2p(const unsigned long long* param_ptrs, const unsigned long l
                      long long n_chunks, float beta1, float beta2, float eps, float wd, long long step, float lr_scale,
                      cudaStream_t st);
 #define MF_ADAMW_CHUNK 512   /* arena granularity (elements) of the per-chunk lr table */
+#define MF_OPTIM_ADAMW 0     /* update rules of mf_optim_step_dyn: decoupled weight decay (AdamW, fastai true_wd) */
+#define MF_OPTIM_ADAM 1      /* coupled L2 weight decay (torch.optim.Adam) */
 int launch_focal_loss_backward(const float* pred, const float* tgt, long long n, const float* scale, float* grad,
                                cudaStream_t st);
 int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
@@ -70,7 +72,7 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
 int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
                            void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out,
-                           cudaStream_t st);
+                           int rule, const double* hyper, cudaStream_t st);
 // OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
 enum {
   MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,

@@ -5,6 +5,9 @@
 //    name) => ~280 groups and ~1000 tiny kernels per step in eager torch; here each tensor is padded to a multiple of
 //    ADAMW_CHUNK elements inside the arena and a per-chunk lr table selects the group's lr, so the whole step is one
 //    launch that streams 28 B/parameter (read p, g, m, v; write p, m, v).
+//    The same update also runs torch.optim.Adam (coupled L2 weight decay, the reference's SOLVER.OPTIMIZER 'adam') and the
+//    fastai one-cycle Adam ('adam_onecycle') through the rule template of adamw_arena_dyn_kernel and a device block of
+//    hyper-parameters (lr multiplier, beta1, weight decay) the host rewrites in place between captured replays.
 //  * focal_loss_backward_kernel: d/dpred of FocalLoss.forward (model/layers/focal_loss.py:35-55) scaled by a device
 //    scalar (loss weight / clamp(num_pos, 1), detector_loss.py:276).
 #include "mf_common.cuh"
@@ -18,9 +21,12 @@ namespace mf {
 //   v   <- v * beta2 + (1 - beta2) * g * g          (torch: exp_avg_sq.mul_(beta2).addcmul_(g, g, value = 1 - beta2))
 //   p   <- p - (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps)
 // g is first multiplied by grad_scale (1 / world_size when the arena holds an NCCL SUM; 1 otherwise).
+// torch.optim.Adam (torch/optim/adam.py single-tensor semantics, RULE = MF_OPTIM_ADAM) differs only in the weight decay:
+//   g   <- g + wd * p                                (coupled L2: torch's grad.add(param, alpha=weight_decay)), no p decay
 struct AdamwConsts {
   float beta1, beta2, eps, wd, bc1, rsqrt_bc2, grad_scale, lr_scale;
 };
+template <int RULE = MF_OPTIM_ADAMW>
 __device__ __forceinline__ void adamw_update4(float4& pp, const float4& gg, float4& mm, float4& vv, float lr,
                                               const AdamwConsts& k) {
   const float omb1 = 1.f - k.beta1, omb2 = 1.f - k.beta2;
@@ -31,8 +37,14 @@ __device__ __forceinline__ void adamw_update4(float4& pp, const float4& gg, floa
   const float* ge = reinterpret_cast<const float*>(&gg);
 #pragma unroll
   for (int e = 0; e < 4; ++e) {
-    const float gk = ge[e] * k.grad_scale;
-    float pk = pe[e] * decay;
+    float gk, pk;
+    if (RULE == MF_OPTIM_ADAMW) {
+      gk = ge[e] * k.grad_scale;
+      pk = pe[e] * decay;
+    } else {
+      pk = pe[e];
+      gk = ge[e] * k.grad_scale + k.wd * pk;
+    }
     const float mk = me[e] + (gk - me[e]) * omb1;
     const float vk = ve[e] * k.beta2 + omb2 * gk * gk;
     const float denom = sqrtf(vk) * k.rsqrt_bc2 + k.eps;
@@ -201,11 +213,12 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
 //                           then the update as above.
 struct AdamwDyn { float bc1, rsqrt_bc2; int skip; float clip_coef; };
 
-__device__ __forceinline__ void adamw_prepare_step(long long* state, AdamwDyn* dyn, float beta1, float beta2, bool skip) {
+// beta1: the kernel argument, or hyper[1] (double) when the step reads the hyper-parameter block
+__device__ __forceinline__ void adamw_prepare_step(long long* state, AdamwDyn* dyn, double beta1, float beta2, bool skip) {
   if (skip) state[2] += 1; else state[0] += 1;
   state[1] = 0;
   const double step = static_cast<double>(state[0] < 1 ? 1 : state[0]);
-  const double bc1 = 1.0 - pow(static_cast<double>(beta1), step);
+  const double bc1 = 1.0 - pow(beta1, step);
   const double bc2 = 1.0 - pow(static_cast<double>(beta2), step);
   dyn->bc1 = static_cast<float>(bc1);
   dyn->rsqrt_bc2 = static_cast<float>(1.0 / sqrt(bc2));
@@ -241,7 +254,8 @@ __global__ void __launch_bounds__(256) grad_sumsq_kernel(const float* __restrict
 
 __global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2,
                                                                  int check, const double* __restrict__ partials, int n_partials,
-                                                                 float grad_scale, float max_norm, float* total_norm_out) {
+                                                                 float grad_scale, float max_norm, float* total_norm_out,
+                                                                 const double* __restrict__ hyper) {
   __shared__ double red[8];
   double s = 0.0;
   for (int i = threadIdx.x; i < n_partials; i += 256) s += partials[i];
@@ -249,7 +263,7 @@ __global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* stat
   if (threadIdx.x != 0) return;
   const float norm = static_cast<float>(sqrt(s) * static_cast<double>(grad_scale));
   *total_norm_out = norm;
-  adamw_prepare_step(state, dyn, beta1, beta2, check != 0 && !isfinite(norm));
+  adamw_prepare_step(state, dyn, hyper != nullptr ? hyper[1] : static_cast<double>(beta1), beta2, check != 0 && !isfinite(norm));
   const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
   dyn->clip_coef = c > 1.f ? 1.f : c;                          // torch.clamp(max=1.0) keeps a NaN
 }
@@ -265,19 +279,29 @@ __global__ void __launch_bounds__(256) grad_finite_kernel(const float* __restric
   }
   if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) atomicExch(reinterpret_cast<unsigned long long*>(state + 1), 1ull);
 }
-__global__ void adamw_prepare_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2, int check) {
+__global__ void adamw_prepare_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2, int check,
+                                     const double* __restrict__ hyper) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  adamw_prepare_step(state, dyn, beta1, beta2, check != 0 && state[1] != 0);
+  adamw_prepare_step(state, dyn, hyper != nullptr ? hyper[1] : static_cast<double>(beta1), beta2, check != 0 && state[1] != 0);
 }
-// CLIP = false never writes g; chunks with lr 0 (padding-only, mark_unused) are neither updated nor clipped
-template <bool CLIP>
+// CLIP = false never writes g; chunks with lr 0 (padding-only, mark_unused) are neither updated nor clipped.
+// HYPER (mf_optim_step_dyn): lr multiplier, beta1 and weight decay come from the device block hyper = double[4]
+// {lr_mult, beta1, weight_decay, unused}, and a chunk whose lr is negative is decay-only: p <- p * (1 - |lr| * wd), no
+// gradient, no moments (fastai's OptimWrapper decays every grouped tensor, torch's Adam then skips the ones with grad None).
+template <bool CLIP, int RULE, bool HYPER>
 __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict__ p, float* __restrict__ g,
                                                               float* __restrict__ m, float* __restrict__ v,
                                                               const float* __restrict__ chunk_lr, long long n_chunks,
-                                                              AdamwConsts k, const AdamwDyn* __restrict__ dyn) {
+                                                              AdamwConsts k, const AdamwDyn* __restrict__ dyn,
+                                                              const double* __restrict__ hyper) {
   if (dyn->skip) return;
   k.bc1 = dyn->bc1;
   k.rsqrt_bc2 = dyn->rsqrt_bc2;
+  if (HYPER) {
+    k.lr_scale *= static_cast<float>(hyper[0]);
+    k.beta1 = static_cast<float>(hyper[1]);
+    k.wd = static_cast<float>(hyper[2]);
+  }
   const float coef = CLIP ? dyn->clip_coef : 1.f;
   constexpr int VEC_PER_CHUNK = MF_ADAMW_CHUNK / 4;
   const long long n_vec = n_chunks * VEC_PER_CHUNK;
@@ -286,6 +310,12 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
     const float lr = __ldg(chunk_lr + i / VEC_PER_CHUNK) * k.lr_scale;
     if (lr == 0.f) continue;
     float4 pp = reinterpret_cast<float4*>(p)[i];
+    if (HYPER && lr < 0.f) {
+      const float decay = 1.f - (-lr) * k.wd;
+      pp.x *= decay; pp.y *= decay; pp.z *= decay; pp.w *= decay;
+      reinterpret_cast<float4*>(p)[i] = pp;
+      continue;
+    }
     float4 gg = __ldcs(reinterpret_cast<const float4*>(g) + i);
     if (CLIP && coef != 1.f) {
       gg.x *= coef; gg.y *= coef; gg.z *= coef; gg.w *= coef;
@@ -293,17 +323,40 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
     }
     float4 mm = reinterpret_cast<float4*>(m)[i];
     float4 vv = reinterpret_cast<float4*>(v)[i];
-    adamw_update4(pp, gg, mm, vv, lr, k);
+    adamw_update4<RULE>(pp, gg, mm, vv, lr, k);
     reinterpret_cast<float4*>(p)[i] = pp;
     reinterpret_cast<float4*>(m)[i] = mm;
     reinterpret_cast<float4*>(v)[i] = vv;
   }
 }
-// max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL)
+template <bool CLIP>
+static void launch_dyn_update(int rule, const double* hyper, dim3 grid, cudaStream_t st, float* p, float* g, float* m,
+                              float* v, const float* chunk_lr, long long n_chunks, const AdamwConsts& k, const AdamwDyn* dyn) {
+  if (hyper == nullptr)
+    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW, false>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
+                   k, dyn, hyper);
+  else if (rule == MF_OPTIM_ADAM)
+    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAM, true>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
+                   k, dyn, hyper);
+  else
+    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW, true>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
+                   k, dyn, hyper);
+}
+// max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL).
+// hyper == NULL: the mf_adamw_step_dyn* semantics (rule must be MF_OPTIM_ADAMW; beta1 / wd / lr_scale from the arguments).
+// hyper != NULL: mf_optim_step_dyn (beta1 and wd arguments ignored, taken from hyper; lr = chunk_lr * lr_scale * hyper[0]).
 int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
                            void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out,
-                           cudaStream_t st) {
+                           int rule, const double* hyper, cudaStream_t st) {
+  if (rule != MF_OPTIM_ADAMW && rule != MF_OPTIM_ADAM) {
+    set_error("optim_step_dyn: rule %d (0 = AdamW, 1 = Adam with L2 weight decay)", rule);
+    return -1;
+  }
+  if (rule != MF_OPTIM_ADAMW && hyper == nullptr) {
+    set_error("optim_step_dyn: the Adam rule reads the hyper-parameter block; hyper is NULL");
+    return -1;
+  }
   if (n_chunks <= 0) return 0;
   const bool clip = max_norm > 0.f;
   if (clip && (partials == nullptr || total_norm_out == nullptr)) {
@@ -318,18 +371,21 @@ int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* 
   if (clip) {
     (void)launch_k(grad_sumsq_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, partials);
     (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta1, beta2, check_finite, partials,
-                   static_cast<int>(blocks), grad_scale, max_norm, total_norm_out);
+                   static_cast<int>(blocks), grad_scale, max_norm, total_norm_out, hyper);
   } else {
     if (check_finite)
       (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
-    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta1, beta2, check_finite);
+    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta1, beta2, check_finite, hyper);
   }
   AdamwConsts k;
   k.beta1 = beta1; k.beta2 = beta2; k.eps = eps; k.wd = wd; k.bc1 = 1.f; k.rsqrt_bc2 = 1.f;
   k.grad_scale = grad_scale; k.lr_scale = lr_scale;
-  (void)launch_k(clip ? adamw_arena_dyn_kernel<true> : adamw_arena_dyn_kernel<false>, dim3(static_cast<unsigned>(blocks)),
-                 dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
-  return check_cuda(cudaGetLastError(), clip ? "adamw_arena_dyn_clip" : "adamw_arena_dyn");
+  const dim3 grid(static_cast<unsigned>(blocks));
+  if (clip)
+    launch_dyn_update<true>(rule, hyper, grid, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
+  else
+    launch_dyn_update<false>(rule, hyper, grid, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
+  return check_cuda(cudaGetLastError(), hyper != nullptr ? "optim_step_dyn" : clip ? "adamw_arena_dyn_clip" : "adamw_arena_dyn");
 }
 
 // ---------------------------------------------------------------- focal loss backward (layers/focal_loss.py:35-55)

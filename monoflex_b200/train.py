@@ -26,6 +26,15 @@ serves as the finite guard, and the coefficient is applied in the AdamW kernel, 
 and in the update that follows the NCCL all-reduce on several, so it clips the rank mean as DDP + clip_grad_norm_ does.
 `optimizer.last_grad_norm` holds the norm of the last captured step. Not available with `symmetric_group` in the captured
 step (raises NotImplementedError): the fused peer-memory exchange has no cross-rank norm between its reduce and update.
+
+`cfg.SOLVER.OPTIMIZER` picks the optimiser through `solver.build_optimizer`: 'adamw' (FusedAdamW, as before), 'adam'
+(FusedAdam) or 'adam_onecycle' (FusedOneCycleAdam); the last two only without `symmetric_group` (the peer-memory exchange
+kernel is AdamW only). With `LR_WARMUP` or a one-cycle optimiser the schedules step as the reference's do_train steps them
+(engine/trainer.py:123-126): `warmup.step(i)` while i < WARMUP_STEPS, then `scheduler.step(i)`, i the 0-based index of the
+step just taken; 'adam_onecycle' with LR_WARMUP raises (the reference asserts a warm-up scheduler it never builds). The
+plain adamw / LambdaLR case keeps calling `scheduler.step()` without an index. The captured step refreshes the optimiser's
+device lr table and hyper-parameter block (lr, beta1 and weight decay a schedule moves) before every replay, so the
+one-GPU update stays inside the graph for every optimiser.
 """
 import torch
 import torch.distributed as dist
@@ -40,6 +49,16 @@ class Trainer(object):
         if not next(model.parameters()).is_cuda:
             raise RuntimeError("monoflex_b200 trains on sm_90a GPUs only; no CPU fallback")
         self.grad_norm_clip = getattr(cfg.SOLVER, "GRAD_NORM_CLIP", -1)
+        name = cfg.SOLVER.OPTIMIZER
+        if name not in solver.OPTIMIZERS:
+            raise NotImplementedError("optimizer %r: the fused optimisers are %s" % (name, ", ".join(solver.OPTIMIZERS)))
+        if name != "adamw" and symmetric_group is not None:
+            raise NotImplementedError("optimizer %r with symmetric_group: the fused peer-memory exchange kernel runs AdamW "
+                                      "only; use the NCCL exchange (no symmetric_group)" % name)
+        onecycle = name.find("onecycle") >= 0
+        if onecycle and cfg.SOLVER.LR_WARMUP:
+            raise ValueError("optimizer %r with LR_WARMUP: the one-cycle schedule has no warm-up scheduler (the reference's "
+                             "do_train asserts one)" % name)
         if use_cuda_graph and self.grad_norm_clip > 0 and symmetric_group is not None:
             raise NotImplementedError("GRAD_NORM_CLIP > 0 with symmetric_group: the fused peer-memory exchange (step_exchange) "
                                       "has no cross-rank gradient norm between its reduce and its update; use the NCCL "
@@ -50,10 +69,12 @@ class Trainer(object):
         self.cfg = cfg
         self.group = process_group
         self.bucket_bytes = bucket_bytes
-        groups = solver.get_model_params(model, cfg)
-        self.optimizer = solver.FusedAdamW(groups, lr=cfg.SOLVER.BASE_LR, weight_decay=cfg.SOLVER.WEIGHT_DECAY, betas=(0.9, 0.99),
-                                           symmetric_group=symmetric_group)
-        self.scheduler, _ = solver.build_scheduler(self.optimizer, cfg.SOLVER)
+        self.optimizer = solver.build_optimizer(model, cfg, symmetric_group=symmetric_group)
+        self._arena_opt = getattr(self.optimizer, "opt", self.optimizer)    # FusedOneCycleAdam wraps its arena optimiser
+        self.scheduler, self.warmup_scheduler = solver.build_scheduler(self.optimizer, cfg.SOLVER)
+        # indexed stepping of do_train (engine/trainer.py:123-126) with a warm-up or one-cycle schedule
+        self._indexed_schedule = onecycle or self.warmup_scheduler is not None
+        self.warmup_iters = solver.solver_value(cfg.SOLVER, "WARMUP_STEPS") if cfg.SOLVER.LR_WARMUP else -1
         self.iteration = 0
         self._unused_marked = False
         self.use_cuda_graph = bool(use_cuda_graph)
@@ -85,13 +106,21 @@ class Trainer(object):
         if self.grad_norm_clip > 0:
             torch.nn.utils.clip_grad_norm_(model.parameters(), self.grad_norm_clip)
         self._exchange_and_update()
-        self.scheduler.step()
+        self._schedule_step()
         self.iteration += 1
         return {k: v.detach() for k, v in loss_dict.items()}, log
 
+    def _schedule_step(self):
+        if not self._indexed_schedule:
+            self.scheduler.step()
+        elif self.iteration < self.warmup_iters:
+            self.warmup_scheduler.step(self.iteration)
+        else:
+            self.scheduler.step(self.iteration)
+
     def _exchange_and_update(self, max_grad_norm=None):
         opt, world = self.optimizer, self.world
-        if opt._symm is not None:
+        if self._arena_opt._symm is not None:
             opt.step_exchange()                                      # reduce + AdamW + broadcast in one peer-memory kernel
         else:
             if world > 1:
@@ -100,7 +129,7 @@ class Trainer(object):
 
     # ------------------------------------------------------------------ captured step
     def _capture(self, images, targets):
-        model, opt = self.model, self.optimizer
+        model, opt = self.model, self._arena_opt
         dev = images.device
         pred, lossev = model.heads.predictor, model.heads.loss_evaluator
         if isinstance(targets, EncodedTargets):
@@ -108,7 +137,7 @@ class Trainer(object):
         else:
             prep = lossev.prepare_targets(targets, dev)
         g = {"x": images.clone(), "prep": tuple(t.clone() for t in prep), "update_inside": self.world == 1 and opt._symm is None}
-        opt._lr_table()
+        opt._lr_table()                        # table and hyper-parameter block current: the captured step() copies nothing
         pred._targets_preloaded = True
         graph = torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
@@ -119,7 +148,7 @@ class Trainer(object):
                 opt.zero_grad()
                 losses.backward()
                 if g["update_inside"]:
-                    opt.step(grad_scale=1.0, max_grad_norm=self.grad_norm_clip)
+                    self.optimizer.step(grad_scale=1.0, max_grad_norm=self.grad_norm_clip)
         finally:
             pred._targets_preloaded = False
         if g["update_inside"]:                 # capture only records: undo the host-side bookkeeping of the captured step()
@@ -130,7 +159,7 @@ class Trainer(object):
         return g
 
     def _step_graph(self, images, targets, sync_log=True):
-        model, opt = self.model, self.optimizer
+        model, opt = self.model, self._arena_opt
         g = self._graph
         if g is None:
             g = self._capture(images, targets)
@@ -143,7 +172,7 @@ class Trainer(object):
             for dst, src in zip(g["prep"], model.heads.loss_evaluator.prepare_targets(targets, images.device)):
                 dst.copy_(src, non_blocking=True)
             model.heads.predictor.load_targets(g["plan_h"], targets)
-        opt._lr_table()                                              # in-place refresh when the scheduler moved the lr
+        opt._lr_table()                              # in-place refresh of the lr table / hyper block the schedule moved
         g["graph"].replay()
         if g["update_inside"]:
             opt.step_count += 1
@@ -152,6 +181,6 @@ class Trainer(object):
                 torch.autograd.graph.increment_version(p)
         else:
             self._exchange_and_update(max_grad_norm=self.grad_norm_clip)
-        self.scheduler.step()
+        self._schedule_step()
         self.iteration += 1
         return g["loss_dict"], (g["log"].resolve() if sync_log else g["log"].snapshot())
