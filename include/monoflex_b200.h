@@ -379,12 +379,21 @@ int mf_draw_heatmaps(const int* obj6, int B, int max_objs, int ncls, int H, int 
  *   with K = 2 (W/4 + H/4) and edge_len int64 [B] (count - 1). status int32 [1] = number of objects the reference would raise
  *   on (an edge object with two non-zero radii, an outside object whose 2D box centre is outside the image) plus images
  *   larger than W x H; they are left out of every output. No host synchronisation.
+ * mf_encode_targets_views: the same with right DEVICE int32 [B] or NULL (all left). For an image with right[b] != 0 (a
+ *   DATASETS.USE_RIGHT_IMAGE item, kitti.py:232-252) P2[b] is the calibration's P3 and sizes[b] the right image's size; the
+ *   label box columns are ignored and the box is rebuilt from the eight corners projected with the unflipped P3, clamped to
+ *   the image and rounded to float32; the flip of that box runs in float32. P2_out / img then hold the (flipped) P3.
+ *   mf_encode_targets(...) == mf_encode_targets_views(..., right = NULL, ...).
  * mf_encode_edges: edge_indices / edge_len alone (the test split's fields) for sizes [B][2]. */
 #define MF_TARGET_LABEL_COLS 16
 int mf_encode_targets(const double* labels, const double* P2, const int* sizes, const int* flips, int B, int M, int H, int W,
                       float* hm, float* obj, float* img, float* alphas, float* gt_bboxes, float* reg_weight,
                       double* occlusions, double* truncations, int* obj6, double* P2_out, long long* edge_indices,
                       long long* edge_len, int* status, void* stream);
+int mf_encode_targets_views(const double* labels, const double* P2, const int* sizes, const int* flips, const int* right, int B,
+                            int M, int H, int W, float* hm, float* obj, float* img, float* alphas, float* gt_bboxes,
+                            float* reg_weight, double* occlusions, double* truncations, int* obj6, double* P2_out,
+                            long long* edge_indices, long long* edge_len, int* status, void* stream);
 int mf_encode_edges(const int* sizes, int B, int H, int W, long long* edge_indices, long long* edge_len, void* stream);
 
 /* nms_hm alone (model/layers/utils.py:45-58): out = heat * (maxpool3x3(heat) == heat), planes = B*C */

@@ -83,6 +83,7 @@ SIGNATURES = {
     "mf_preprocess_images_u8": [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P],
     "mf_draw_heatmaps": [_P, _I, _I, _I, _I, _I, _P, _P],
     "mf_encode_targets": [_P, _P, _P, _P, _I, _I, _I, _I] + [_P] * 14,
+    "mf_encode_targets_views": [_P, _P, _P, _P, _P, _I, _I, _I, _I] + [_P] * 14,
     "mf_encode_edges": [_P, _I, _I, _I, _P, _P, _P],
     "mf_nms_hm": [_P, _P, _I, _I, _I, _P],
     "mf_decode_detections": [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _I, _I, _P, _I, _P, _P, _P, _P, _P,

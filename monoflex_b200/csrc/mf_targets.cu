@@ -90,9 +90,48 @@ MF_DEVINL float gaussian_radius_f32(float h, float w) {
 
 MF_DEVINL int py_int_nonneg(double r) { return r > 0 ? static_cast<int>(r) : 0; }     // max(0, int(r))
 
+// Object3d.generate_corners3d: R . [x; y; z] + t for the eight corners
+MF_DEVINL void box_corners(double ry, float tx, float ty, float tz, double oh_, double ow_, double ol_, double* X, double* Y,
+                           double* Z) {
+  const double cr = cos(ry), sr = sin(ry);
+  const double hl = ol_ / 2, hw = ow_ / 2;
+  const double xc[8] = {hl, hl, -hl, -hl, hl, hl, -hl, -hl};
+  const double yc[8] = {0, 0, 0, 0, -oh_, -oh_, -oh_, -oh_};
+  const double zc[8] = {hw, -hw, -hw, hw, hw, -hw, -hw, hw};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    X[k] = dadd(dadd(dadd(dmul(cr, xc[k]), dmul(0.0, yc[k])), dmul(sr, zc[k])), static_cast<double>(tx));
+    Y[k] = dadd(dadd(dadd(dmul(0.0, xc[k]), dmul(1.0, yc[k])), dmul(0.0, zc[k])), static_cast<double>(ty));
+    Z[k] = dadd(dadd(dadd(dmul(-sr, xc[k]), dmul(0.0, yc[k])), dmul(cr, zc[k])), static_cast<double>(tz));
+  }
+}
+
+// The right-camera label box (kitti.py:243-249), before the flip: the projected corners' extent under the unflipped P3,
+// clamped with Python's max(x, 0) / min(x, img - 1), rounded to float32 (Object3d.box2d and its np.float32 elements)
+MF_DEVINL void right_view_box(const double* P, double ry, float tx, float ty, float tz, double oh_, double ow_, double ol_,
+                              int img_w, int img_h, float* box) {
+  double X[8], Y[8], Z[8];
+  box_corners(ry, tx, ty, tz, oh_, ow_, ol_, X, Y, Z);
+  double u, v;
+  project(P, X[0], Y[0], Z[0], u, v);
+  double umin = u, umax = u, vmin = v, vmax = v;
+#pragma unroll
+  for (int k = 1; k < 8; ++k) {
+    project(P, X[k], Y[k], Z[k], u, v);
+    umin = fmin(umin, u); umax = fmax(umax, u);
+    vmin = fmin(vmin, v); vmax = fmax(vmax, v);
+  }
+  const double wm1 = img_w - 1, hm1 = img_h - 1;
+  box[0] = static_cast<float>(0 > umin ? 0.0 : umin);
+  box[1] = static_cast<float>(0 > vmin ? 0.0 : vmin);
+  box[2] = static_cast<float>(wm1 < umax ? wm1 : umax);
+  box[3] = static_cast<float>(hm1 < vmax ? hm1 : vmax);
+}
+
 __global__ void __launch_bounds__(128) encode_objects_kernel(const double* __restrict__ lab, const double* __restrict__ P2,
                                                              const int* __restrict__ sizes, const int* __restrict__ flips,
-                                                             int B, int M, int H, int W, TargetOut o) {
+                                                             const int* __restrict__ rights, int B, int M, int H, int W,
+                                                             TargetOut o) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= B * M) return;
   const int b = i / M;
@@ -109,6 +148,7 @@ __global__ void __launch_bounds__(128) encode_objects_kernel(const double* __res
   const int img_w = sizes[2 * b], img_h = sizes[2 * b + 1];
   const bool size_ok = img_w >= 1 && img_h >= 1 && img_w <= W && img_h <= H;
   const bool flip = flips != nullptr && flips[b] != 0;
+  const bool right = rights != nullptr && rights[b] != 0;
   double P[12];
   for (int k = 0; k < 12; ++k) P[k] = P2[12 * b + k];
   if (flip) {                                                          // augmentations.py:69-73
@@ -134,38 +174,42 @@ __global__ void __launch_bounds__(128) encode_objects_kernel(const double* __res
   const int cls = static_cast<int>(L[L_CLS]);
   if (cls < 0 || cls >= NCLS || static_cast<double>(cls) != L[L_CLS]) { atomicAdd(o.status, 1); return; }
   const double trunc = L[L_TRUNC], occ = L[L_OCC];
-  double xmin = L[L_X1], xmax = L[L_X2];
-  const double ymin = L[L_Y1], ymax = L[L_Y2];
   const double oh_ = L[L_H], ow_ = L[L_W], ol_ = L[L_L];
   float tx = static_cast<float>(L[L_TX]);
   const float ty = static_cast<float>(L[L_TY]), tz = static_cast<float>(L[L_TZ]);
   double ry = L[L_RY];
-  if (flip) {                                                          // augmentations.py:40-64
-    const double bw = dsub(xmax, xmin);
-    xmin = dsub(dsub(static_cast<double>(img_w), xmax), 1.0);
-    xmax = dadd(xmin, bw);
+  float lbox[4];
+  if (right) {                                                         // the box columns of the row are not used
+    right_view_box(P2 + 12 * b, ry, tx, ty, tz, oh_, ow_, ol_, img_w, img_h, lbox);
+    if (flip) {                                                        // augmentations.py:42-44 on np.float32 scalars
+      const float bw = __fsub_rn(lbox[2], lbox[0]);
+      lbox[0] = __fsub_rn(__fsub_rn(static_cast<float>(img_w), lbox[2]), 1.f);
+      lbox[2] = __fadd_rn(lbox[0], bw);
+    }
+  } else {
+    double xmin = L[L_X1], xmax = L[L_X2];
+    if (flip) {                                                        // augmentations.py:42-44 on Python floats
+      const double bw = dsub(xmax, xmin);
+      xmin = dsub(dsub(static_cast<double>(img_w), xmax), 1.0);
+      xmax = dadd(xmin, bw);
+    }
+    lbox[0] = static_cast<float>(xmin);
+    lbox[1] = static_cast<float>(L[L_Y1]);
+    lbox[2] = static_cast<float>(xmax);
+    lbox[3] = static_cast<float>(L[L_Y2]);
+  }
+  if (flip) {                                                          // augmentations.py:47-65
     ry = wrap_pi(ry < 0 ? dsub(-PI, ry) : dsub(PI, ry));
     tx = -tx;
   }
-  const float lbox[4] = {static_cast<float>(xmin), static_cast<float>(ymin), static_cast<float>(xmax), static_cast<float>(ymax)};
   const double alpha = wrap_pi(dsub(ry, atan2(static_cast<double>(tx), static_cast<double>(tz))));   // convertRot2Alpha
 
   const float locy = __fsub_rn(ty, static_cast<float>(oh_ / 2));      // float32 locs[1] - obj.h / 2
   if (tz <= 0.f) return;                                               // behind the camera
 
-  // generate_corners3d: R . [x; y; z] + t, then the two face centres; projected with P
-  const double cr = cos(ry), sr = sin(ry);
-  const double hl = ol_ / 2, hw = ow_ / 2;
-  const double xc[8] = {hl, hl, -hl, -hl, hl, hl, -hl, -hl};
-  const double yc[8] = {0, 0, 0, 0, -oh_, -oh_, -oh_, -oh_};
-  const double zc[8] = {hw, -hw, -hw, hw, hw, -hw, -hw, hw};
+  // generate_corners3d, then the two face centres; projected with P
   double X[10], Y[10], Z[10], U[10], V[10];
-#pragma unroll
-  for (int k = 0; k < 8; ++k) {
-    X[k] = dadd(dadd(dadd(dmul(cr, xc[k]), dmul(0.0, yc[k])), dmul(sr, zc[k])), static_cast<double>(tx));
-    Y[k] = dadd(dadd(dadd(dmul(0.0, xc[k]), dmul(1.0, yc[k])), dmul(0.0, zc[k])), static_cast<double>(ty));
-    Z[k] = dadd(dadd(dadd(dmul(-sr, xc[k]), dmul(0.0, yc[k])), dmul(cr, zc[k])), static_cast<double>(tz));
-  }
+  box_corners(ry, tx, ty, tz, oh_, ow_, ol_, X, Y, Z);
 #pragma unroll
   for (int f = 0; f < 2; ++f) {                                        // corners_3d[:4].mean(0), corners_3d[4:].mean(0)
     const int k0 = 4 * f;
@@ -347,12 +391,12 @@ using namespace mf;
 
 extern "C" {
 
-int mf_encode_targets(const double* labels, const double* P2, const int* sizes, const int* flips, int B, int M, int H, int W,
-                      float* hm, float* obj, float* img, float* alphas, float* gt_bboxes, float* reg_weight,
-                      double* occlusions, double* truncations, int* obj6, double* P2_out, long long* edge_indices,
-                      long long* edge_len, int* status, void* stream) {
+int mf_encode_targets_views(const double* labels, const double* P2, const int* sizes, const int* flips, const int* right, int B,
+                            int M, int H, int W, float* hm, float* obj, float* img, float* alphas, float* gt_bboxes,
+                            float* reg_weight, double* occlusions, double* truncations, int* obj6, double* P2_out,
+                            long long* edge_indices, long long* edge_len, int* status, void* stream) {
   if (B < 1 || M < 1 || H < DOWN || W < DOWN || H % DOWN || W % DOWN) {
-    set_error("mf_encode_targets: B=%d M=%d H=%d W=%d (H and W multiples of %d)", B, M, H, W, DOWN);
+    set_error("mf_encode_targets_views: B=%d M=%d H=%d W=%d (H and W multiples of %d)", B, M, H, W, DOWN);
     return -1;
   }
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
@@ -361,12 +405,24 @@ int mf_encode_targets(const double* labels, const double* P2, const int* sizes, 
   TargetOut o{obj, img, alphas, gt_bboxes, reg_weight, occlusions, truncations, obj6, P2_out, status};
   const int n = B * M;
   (void)launch_k(encode_objects_kernel, dim3(static_cast<unsigned>((n + 127) / 128)), dim3(128), 0, st, labels, P2, sizes, flips,
-                 B, M, H, W, o);
+                 right, B, M, H, W, o);
   int rc = check_cuda(cudaGetLastError(), "encode_objects");
   if (rc) return rc;
   rc = launch_draw_heatmap(obj6, B, M, NCLS, H / DOWN, W / DOWN, hm, st);
   if (rc) return rc;
   return launch_edges(sizes, B, H, W, edge_indices, edge_len, st);
+}
+
+int mf_encode_targets(const double* labels, const double* P2, const int* sizes, const int* flips, int B, int M, int H, int W,
+                      float* hm, float* obj, float* img, float* alphas, float* gt_bboxes, float* reg_weight,
+                      double* occlusions, double* truncations, int* obj6, double* P2_out, long long* edge_indices,
+                      long long* edge_len, int* status, void* stream) {
+  if (B < 1 || M < 1 || H < DOWN || W < DOWN || H % DOWN || W % DOWN) {
+    set_error("mf_encode_targets: B=%d M=%d H=%d W=%d (H and W multiples of %d)", B, M, H, W, DOWN);
+    return -1;
+  }
+  return mf_encode_targets_views(labels, P2, sizes, flips, nullptr, B, M, H, W, hm, obj, img, alphas, gt_bboxes, reg_weight,
+                                 occlusions, truncations, obj6, P2_out, edge_indices, edge_len, status, stream);
 }
 
 int mf_encode_edges(const int* sizes, int B, int H, int W, long long* edge_indices, long long* edge_len, void* stream) {

@@ -8,15 +8,18 @@ flip (data/augmentations/augmentations.py:28-77) on the GPU, for a whole batch, 
     enc.check()                                                                              # outside a captured step
 
 `flips` are the flags the caller also passes to `GpuInputPipeline.images(flips=...)`. What stays on the host is parsing the
-label text and the class filter, O(objects). Only the runs/monoflex.yaml configuration is built; anything else raises
-NotImplementedError. The reference raises on two label geometries (an edge object with two non-zero heat-map radii,
+label text and the class filter, O(objects). Only the runs/monoflex.yaml configuration is built, with DATASETS.USE_RIGHT_IMAGE
+either way (runs/monoflex_right.yaml); anything else raises NotImplementedError. A right-camera item (dataset index >=
+num_samples, see dataset_view) is encoded with `right` set for its image, its calibration's P3
+(read_kitti_calib(..., use_right_cam=True)) in place of P2 and the image_3 size; its label boxes are rebuilt from the
+projected 3D boxes on the device (kitti.py:232-252). The reference raises on two label geometries (an edge object with two non-zero heat-map radii,
 kitti.py:457; an outside object whose 2D box centre is outside the image, where approx_proj_center returns None); the kernel
 cannot raise, so it counts them in a device status word, leaves them out of every output, and `EncodedTargets.check()` raises.
 """
 import numpy as np
 import torch
 
-from ._lib import call, stream
+from ._lib import call, ptr, stream
 from .structures import Calibration, ParamsList
 
 LABEL_COLS = 16          # MF_TARGET_LABEL_COLS: valid + the 14 values of read_kitti_label + one zero column
@@ -54,8 +57,9 @@ def read_kitti_label(path_or_lines, classes=CLASSES):
     return np.array(rows, dtype=np.float64).reshape(-1, ROW_COLS)
 
 
-def read_kitti_calib(path):
-    """P2 of a KITTI calibration file (Calibration.read_calib_file, kitti_utils.py:220-238) as float64 [3, 4]."""
+def read_kitti_calib(path, use_right_cam=False):
+    """P2 (or P3 with use_right_cam, Calibration(..., use_right_cam=True)) of a KITTI calibration file
+    (Calibration.read_calib_file, kitti_utils.py:193-238) as float64 [3, 4]."""
     data = {}
     with open(path) as f:
         for line in f.readlines():
@@ -67,7 +71,26 @@ def read_kitti_calib(path):
                 data[key] = np.array([float(x) for x in value.split()])
             except ValueError:
                 pass
-    return np.reshape(data["P2"], [3, 4]).astype(np.float64)
+    return np.reshape(data["P3" if use_right_cam else "P2"], [3, 4]).astype(np.float64)
+
+
+def dataset_len(num_samples, cfg, is_train=True):
+    """len(KITTIDataset) (kitti.py:100-104): 2 * num_samples when DATASETS.USE_RIGHT_IMAGE and is_train, else num_samples."""
+    return 2 * num_samples if _use_right(cfg, is_train) else num_samples
+
+
+def dataset_view(idx, num_samples, cfg, is_train=True):
+    """The view a KITTIDataset index stands for (kitti.py:232-259), for a sampler feeding GpuTargetEncoder: (frame index,
+    right flag). Indices >= num_samples (present only with DATASETS.USE_RIGHT_IMAGE and is_train) are frame
+    idx - num_samples seen by the right camera: image_3, P3 and the right flag of encode()."""
+    idx = int(idx)
+    if not 0 <= idx < dataset_len(num_samples, cfg, is_train):
+        raise IndexError("dataset index %d outside 0..%d" % (idx, dataset_len(num_samples, cfg, is_train) - 1))
+    return (idx - num_samples, True) if idx >= num_samples else (idx, False)
+
+
+def _use_right(cfg, is_train):
+    return bool(_get(cfg.DATASETS, "USE_RIGHT_IMAGE", False)) and bool(is_train)
 
 
 def pack_labels(list_of_rows, max_objs):
@@ -92,7 +115,7 @@ class GpuTargetEncoder(object):
     """KITTIDataset's training targets for a batch, on the device (see the module docstring)."""
 
     def __init__(self, cfg, device="cuda"):
-        self._check_config(cfg)
+        self._check_config(cfg, right_views=True)
         self.H, self.W = int(cfg.INPUT.HEIGHT_TRAIN), int(cfg.INPUT.WIDTH_TRAIN)
         if self.H % DOWN_RATIO or self.W % DOWN_RATIO:
             raise ValueError("input size %dx%d is not a multiple of the down ratio %d" % (self.W, self.H, DOWN_RATIO))
@@ -102,16 +125,23 @@ class GpuTargetEncoder(object):
         self.device = torch.device(device)
 
     @staticmethod
-    def _check_config(cfg):
-        """Only runs/monoflex.yaml's INPUT / DATASETS options are built; an option the cfg does not carry takes that value."""
+    def _check_config(cfg, right_views=False):
+        """Only runs/monoflex.yaml's INPUT / DATASETS options are built; an option the cfg does not carry takes that value.
+        right_views=False checks them for a caller that encodes left views only, which cannot serve DATASETS.USE_RIGHT_IMAGE
+        (half of that training set is right-camera items); right_views=True, what the encoder itself checks, also accepts
+        USE_RIGHT_IMAGE = True (runs/monoflex_right.yaml), whose right items encode() takes with its `right` flags."""
         inp, ds = cfg.INPUT, cfg.DATASETS
+        right = _get(ds, "USE_RIGHT_IMAGE", False)
+        if right not in ((True, False) if right_views else (False,)):
+            raise NotImplementedError("GpuTargetEncoder: DATASETS.USE_RIGHT_IMAGE = %r; %s" % (
+                right, "True or False expected" if right_views else
+                "only False (runs/monoflex.yaml) is served by left views alone; right_views=True accepts True"))
         want = [(inp, "INPUT", "HEATMAP_CENTER", '3D'), (inp, "INPUT", "APPROX_3D_CENTER", 'intersect'),
                 (inp, "INPUT", "ADJUST_BOUNDARY_HEATMAP", True), (inp, "INPUT", "KEYPOINT_VISIBLE_MODIFY", True),
                 (inp, "INPUT", "HEATMAP_RATIO", 0.5), (inp, "INPUT", "ORIENTATION", 'multi-bin'),
                 (inp, "INPUT", "ORIENTATION_BIN_SIZE", 4), (inp, "INPUT", "AUG_PARAMS", [[0.5]]),
                 (ds, "DATASETS", "CONSIDER_OUTSIDE_OBJS", True), (ds, "DATASETS", "FILTER_ANNO_ENABLE", True),
-                (ds, "DATASETS", "FILTER_ANNOS", [0.9, 20]), (ds, "DATASETS", "USE_RIGHT_IMAGE", False),
-                (ds, "DATASETS", "DETECT_CLASSES", list(CLASSES)),
+                (ds, "DATASETS", "FILTER_ANNOS", [0.9, 20]), (ds, "DATASETS", "DETECT_CLASSES", list(CLASSES)),
                 (cfg.MODEL.BACKBONE, "MODEL.BACKBONE", "DOWN_RATIO", DOWN_RATIO),
                 (cfg.MODEL.HEAD, "MODEL.HEAD", "ENABLE_EDGE_FUSION", True)]
         for node, path, key, v in want:
@@ -126,24 +156,28 @@ class GpuTargetEncoder(object):
             t = t.to(self.device, non_blocking=True)
         return t.to(dtype).contiguous()
 
-    def encode(self, labels, P2, image_sizes, flips=None, out=None, edge_out=None):
+    def encode(self, labels, P2, image_sizes, flips=None, out=None, edge_out=None, right=None):
         """labels float64 [B, max_objs, 16] (pack_labels), P2 float64 [B, 3, 4], image_sizes [B, 2] original (w, h), flips [B]
         (or None). Host arrays are copied up; for a CUDA-graph capture pass device tensors and refill them between replays.
         out: (hm, obj, img) tensors to write instead of allocating (a captured step's static buffers); edge_out:
-        (edge_indices int64 [B, K, 2], edge_len int64 [B]) likewise. Returns EncodedTargets; nothing here reads the device."""
+        (edge_indices int64 [B, K, 2], edge_len int64 [B]) likewise. right [B] (or None: all left) marks right-camera items,
+        host or device like flips: for such an image P2[b] is its P3, image_sizes[b] the right image's size, and the label
+        rows' box columns are not read. Returns EncodedTargets; nothing here reads the device."""
         B, M = int(labels.shape[0]), self.max_objs
         if tuple(labels.shape) != (B, M, LABEL_COLS):
             raise ValueError("labels: [B, %d, %d] expected, got %s" % (M, LABEL_COLS, tuple(labels.shape)))
         if tuple(P2.shape) != (B, 3, 4) or tuple(image_sizes.shape) != (B, 2):
             raise ValueError("P2 [B, 3, 4] and image_sizes [B, 2] expected, got %s, %s" % (tuple(P2.shape), tuple(image_sizes.shape)))
-        if flips is not None and tuple(flips.shape if hasattr(flips, "shape") else (len(flips),)) != (B,):
-            raise ValueError("flips: one flag per image expected")
+        for name, flags in (("flips", flips), ("right", right)):
+            if flags is not None and tuple(flags.shape if hasattr(flags, "shape") else (len(flags),)) != (B,):
+                raise ValueError("%s: one flag per image expected" % name)
         if not (torch.is_tensor(image_sizes) and image_sizes.is_cuda):
             s = np.asarray(image_sizes.cpu() if torch.is_tensor(image_sizes) else image_sizes)
             if (s < 1).any() or (s[:, 0] > self.W).any() or (s[:, 1] > self.H).any():
                 raise ValueError("image sizes %s outside 1..%dx%d" % (s.tolist(), self.W, self.H))
         inputs = (self._dev(labels, torch.float64), self._dev(P2, torch.float64), self._dev(image_sizes, torch.int32),
-                  None if flips is None else self._dev(flips, torch.int32))
+                  None if flips is None else self._dev(flips, torch.int32),
+                  None if right is None else self._dev(right, torch.int32))
         dev, f32 = self.device, torch.float32
         h, w = self.H // DOWN_RATIO, self.W // DOWN_RATIO
         shapes = ((B, self.ncls, h, w), (B * M, _obj_cols()), (B, 8))
@@ -158,9 +192,9 @@ class GpuTargetEncoder(object):
                 any(t.dtype != torch.int64 or not t.is_contiguous() for t in edge_out):
             raise ValueError("edge_out: int64 [B, %d, 2] and [B] expected" % self.K)
         e = EncodedTargets(self, inputs, out, edge_out)
-        lab, p2, sz, fl = inputs
+        lab, p2, sz, fl, rt = inputs
         hm, obj, img = out
-        call("mf_encode_targets", lab.data_ptr(), p2.data_ptr(), sz.data_ptr(), None if fl is None else fl.data_ptr(), B, M,
+        call("mf_encode_targets_views", lab.data_ptr(), p2.data_ptr(), sz.data_ptr(), ptr(fl), ptr(rt), B, M,
              self.H, self.W, hm.data_ptr(), obj.data_ptr(), img.data_ptr(), e.alphas.data_ptr(), e.gt_bboxes.data_ptr(),
              e.reg_weight.data_ptr(), e.occlusions.data_ptr(), e.truncations.data_ptr(), e.obj6.data_ptr(), e.P2.data_ptr(),
              edge_out[0].data_ptr(), edge_out[1].data_ptr(), e.status.data_ptr(), stream())
@@ -201,8 +235,10 @@ class EncodedTargets(object):
     prepared      (hm, obj, img): what Loss_Computation.prepare_targets returns, for `_forward_train(..., prepared=)`
     edge_indices  int64 [B, K, 2], edge_len int64 [B]
     alphas, gt_bboxes, reg_weight, occlusions, truncations: the remaining per-slot fields of kitti.py:497-521
-    obj6          int32 [B, M, 6] heat-map table (valid, class, cx, cy, rx, ry); P2 the flipped projection matrices
-    status        int32 [1]: objects left out where the reference raises (read by check())"""
+    obj6          int32 [B, M, 6] heat-map table (valid, class, cx, cy, rx, ry)
+    P2            float64 [B, 3, 4]: the (flipped) camera matrix each image was encoded with (P3 for a right-camera item)
+    status        int32 [1]: objects left out where the reference raises (read by check())
+    inputs        (labels, P2, image_sizes, flips, right) on the device, as encode_into encodes them again"""
 
     def __init__(self, encoder, inputs, out, edge_out):
         B, M, dev = out[2].shape[0], encoder.max_objs, encoder.device
@@ -232,8 +268,8 @@ class EncodedTargets(object):
 
     def encode_into(self, out, edge_out):
         """Encode the same inputs again into other buffers (a captured training step's static targets)."""
-        lab, p2, sz, fl = self.inputs
-        return self.encoder.encode(lab, p2, sz, fl, out=out, edge_out=edge_out)
+        lab, p2, sz, fl, rt = self.inputs
+        return self.encoder.encode(lab, p2, sz, fl, out=out, edge_out=edge_out, right=rt)
 
     def edge_targets(self):
         """Per-image ParamsLists with only the edge-fusion fields (device views): what the predictor reads when the loss
@@ -249,7 +285,7 @@ class EncodedTargets(object):
 
     def param_lists(self):
         """Reference-shaped ParamsLists (kitti.py:496-521 without ori_img): device tensor views of the encoded tables and a
-        host Calibration of the flipped P2 (one device-to-host copy). prepare_targets(param_lists()) == prepared."""
+        host Calibration of the (flipped) P2 or P3 (one device-to-host copy). prepare_targets(param_lists()) == prepared."""
         enc = self
         hm, obj, img = self.prepared
         B, M = len(self), self.encoder.max_objs
