@@ -20,6 +20,10 @@
 // and the barriers persist across tiles, so the per-tile cost is the MMA time, not a pipeline fill + drain.
 // HEAD2 (strict predictor, EPI == 2) has neither producer nor epilogue warps: the consumers contract the 1x1 heads from their
 // own accumulators on the tensor cores and store the results (see IgemmParams).
+// MODE_DCN with 64-column tiles (NPW == 16, "wide gather", igemm2_wide): 16 producer warps (2 pixel rows per thread and K
+// block instead of 4) and ONE consumer warpgroup, which issues two m64n64k16 wgmmas per k16 step (rows [0, 64) and [64, 128))
+// and finishes its own tiles from the accumulator fragments; no epilogue warps and no chunk slot, whose shared memory goes to
+// the ring. At 64 columns a gathered A element feeds only 64 x 3 MACs, so the gather bounds the kernel, not the tensor pipe.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
 
@@ -34,7 +38,10 @@ static constexpr int A_STAGE = BM * BK * 2;   // 16 KB
 // EPI (see igemm2_kernel): 1 = SPLIT doubles the staging; 2 = HEAD2 has no output staging and no chunk slot, its staging area
 // holds the two slots of 1x1 head weights instead. HEAD2 at BLOCK_N = 128: FIXED = 32768 + 384 + 1024 + 1024 = 35200 B, and
 // (232448 - 35200) / (16384 + 16384) = 6.02, so a sixth ring stage fits (SMEM = 6 x 32768 + 35200 = 231808 B).
-template <int BLOCK_N, int MODE, int EPI = 0>
+// WIDE (the wide-gather DCN, see igemm2_wide): no chunk slot. Strict: FIXED = 32768 + 384 + 512 + 36864 + 1024 = 71552 B, and
+// (232448 - 71552) / (16384 + 8192) = 6.5 stages would fit, but the ring keeps the DCN's 4: measured on one H100 80GB HBM3
+// (700 W), 6 stages made the strict 64 -> 64 layer at 96 x 320, B = 8, 4 % slower (0.313 against 0.301 ms).
+template <int BLOCK_N, int MODE, int EPI = 0, bool WIDE = false>
 struct Cfg2 {
   static constexpr bool SPLIT = EPI == 1;
   static constexpr int CTAS_PER_SM = BLOCK_N >= 64 ? 1 : 2;
@@ -50,7 +57,7 @@ struct Cfg2 {
   static constexpr int PRM_BYTES = MODE == MODE_DCN ? 9 * BM * 32 : 0;   // DCN sampling records
   static constexpr int CHUNK = BLOCK_N >= 32 ? 32 : 16;         // accumulator hand-over unit (columns)
   static constexpr int ACC_LD = CHUNK + 4;                      // fp32 row stride of the chunk slot (conflict-free, see gmma_store_cols)
-  static constexpr int ACC_BYTES = EPI == 2 ? 0 : BM * ACC_LD * 4;
+  static constexpr int ACC_BYTES = (EPI == 2 || WIDE) ? 0 : BM * ACC_LD * 4;
   static constexpr int BUDGET = (CTAS_PER_SM == 2 ? 113 : 227) * 1024;
   static constexpr int FIXED = OUT_STAGE + BAR_BYTES + 2 * BLOCK_N * 4 + PRM_BYTES + ACC_BYTES + 1024;
   // ring depth: the shallower of the preferred depth and what the shared-memory budget leaves
@@ -86,11 +93,14 @@ struct ChunkDump {                         // compile-time walk over the chunks 
   }
 };
 
+// the wide-gather DCN configuration (64-column tiles): 16 producer warps and one self-finishing consumer warpgroup
+__host__ __device__ constexpr bool igemm2_wide(int mode, int npw) { return mode == MODE_DCN && npw == 16; }
+
 // warps of a CTA: NPW producers, 8 consumers, the weight-TMA warp (MODE_DCN: the producers issue the weight loads, which
 // keeps 640 threads and 96 registers for the consumers' 64 accumulators), 4 epilogue warps (none for HEAD2, whose consumers
-// finish their own tiles)
+// finish their own tiles). Wide-gather DCN: 16 producers + 4 consumers, the same 640 threads.
 __host__ __device__ constexpr int igemm2_warps(int mode, int npw, int epi) {
-  return npw + 8 + (mode == MODE_DCN ? 0 : 1) + (epi == 2 ? 0 : 4);
+  return igemm2_wide(mode, npw) ? npw + 4 : npw + 8 + (mode == MODE_DCN ? 0 : 1) + (epi == 2 ? 0 : 4);
 }
 
 template <int N>
@@ -119,7 +129,9 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   constexpr bool SPLIT = EPI == 1;
   constexpr bool HEAD2 = EPI == 2;
   static_assert(!HEAD2 || (A_TMA && NPW == 0 && BLOCK_N == 128), "HEAD2: TMA-only warps, 128-column tiles");
-  using C = Cfg2<BLOCK_N, MODE, EPI>;
+  constexpr bool WIDE = igemm2_wide(MODE, NPW);
+  static_assert(!WIDE || BLOCK_N == 64, "wide-gather DCN: 64-column tiles (two m64n64 accumulators per consumer thread)");
+  using C = Cfg2<BLOCK_N, MODE, EPI, WIDE>;
   constexpr int STAGES = C::STAGES;
   constexpr int LAG = C::LAG;
   const bool split_out = SPLIT || p.split_out != 0;      // SPLIT == staged hi/lo tiles; narrow tiles store both halves directly
@@ -162,7 +174,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
     if (A_TMA) tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], A_TMA ? 1 : NPT + 1);
-      mbar_init(&empty_bar[s], 8);                                 // released by the 8 consumer warps
+      mbar_init(&empty_bar[s], WIDE ? 4 : 8);                      // released by every consumer warp
     }
     mbar_init(&acc_full[0], 8);
     mbar_init(&acc_full[1], 8);
@@ -641,12 +653,23 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
   } else if (warp < NPW + 8) {
     // ================================================================ consumers: warpgroup wg issues the wgmmas of tile rows
     // [64 wg, 64 wg + 64) and hands its accumulators to the epilogue chunk by chunk. Every MMA batch is waited for before
-    // the stage it read is released (empty barriers count the 8 consumer warps).
+    // the stage it read is released (empty barriers count the consumer warps). WIDE: the one warpgroup issues every MMA
+    // twice, rows [0, 64) into d and rows [64, 128) into d1, so each row sees the MMA sequence of the two-warpgroup kernel.
     {
       const int wg = (warp - NPW) >> 2;
       float d[BLOCK_N / 2];
-      auto mma = [&](uint64_t ad, uint64_t bd, uint32_t accum) { Gmma<BLOCK_N>::template mma<0, 0>(d, ad, bd, accum); };
-      auto done = [&]() { gmma_commit(); gmma_wait<0>(); gmma_hold(d); __syncwarp(); };
+      float d1[WIDE ? BLOCK_N / 2 : 1];
+      auto mma = [&](uint64_t ad, uint64_t bd, uint32_t accum) {
+        Gmma<BLOCK_N>::template mma<0, 0>(d, ad, bd, accum);
+        if constexpr (WIDE) Gmma<BLOCK_N>::template mma<0, 0>(d1, ad + ((64 * 128) >> 4), bd, accum);
+      };
+      auto done = [&]() {
+        gmma_commit();
+        gmma_wait<0>();
+        gmma_hold(d);
+        if constexpr (WIDE) gmma_hold(d1);
+        __syncwarp();
+      };
       auto release = [&](uint64_t* bar) { if (lane == 0) mbar_arrive(bar); };
       // Descriptors are "base + small delta": everything except the 14-bit start-address field is loop invariant, and
       // the field is linear in the byte address, so the hot loop only does 64-bit adds.
@@ -775,6 +798,107 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
               }
             }
           }
+        } else if constexpr (WIDE) {
+          // ---- the tile's epilogue from the accumulator fragments: scale/shift, activation, fp16 (strict: the hi/lo pair,
+          // the expressions of run_epilogue), then the swizzled staging and one 4-D TMA store per half, or direct stores
+          // (no residual: the DCN entry points have none). d[4 j + 2 h + e] is row 16 w + l / 4 + 8 h, column 8 j + 2 tq + e.
+          const int n0 = (t % ntn) * BLOCK_N, m_tile = t / ntn;
+          const int tile_b = m_tile / (tiles_x * tiles_y);
+          const int tile_t = m_tile - tile_b * (tiles_x * tiles_y);
+          const int tile_y0 = (tile_t / tiles_x) << 3, tile_x0 = (tile_t % tiles_x) << 4;
+          const int et = threadIdx.x & 127, tq = lane & 3;
+          const bool staged = SPLIT || use_tma_store != 0;    // host guarantees OUT_F16_NHWC (strict: always staged)
+          const uint32_t sc_u = smem_u32(sc_s), sh_u = smem_u32(sh_s), o_u = smem_u32(o_smem);
+          if (staged && et == 0) bulk_wait_read0();           // previous tile's TMA store has finished reading the staging
+          if (et < BLOCK_N) {
+            sts32f(sc_u + et * 4, __ldg(p.scale + n0 + et));
+            sts32f(sh_u + et * 4, __ldg(p.shift + n0 + et));
+          }
+          bar_sync_named(1, 128);
+          // one walk over the fragments per output form (the form is chosen outside the loop, so the rarely used direct
+          // stores cost the staged path no registers); store(row, j, nb, v) writes columns nb, nb + 1 of tile row `row`
+          auto finish = [&](auto&& store) {
+#pragma unroll
+            for (int mh = 0; mh < 2; ++mh) {
+              float(&dh)[BLOCK_N / 2] = mh == 0 ? d : d1;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int row = 64 * mh + 16 * (warp - NPW) + (lane >> 2) + 8 * h;
+#pragma unroll
+                for (int j = 0; j < BLOCK_N / 8; ++j) {
+                  const int nb = n0 + 8 * j + 2 * tq;
+                  const float2 s2 = lds64f(sc_u + (nb - n0) * 4), h2 = lds64f(sh_u + (nb - n0) * 4);
+                  float v[2];
+                  v[0] = dh[4 * j + 2 * h] * s2.x + h2.x;
+                  v[1] = dh[4 * j + 2 * h + 1] * s2.y + h2.y;
+                  // the next tile's first MMA does not read the accumulators (scale-d = 0), but its asm operands do:
+                  // zeroed, they need no registers through the rest of the epilogue (see HEAD2)
+                  dh[4 * j + 2 * h] = 0.f;
+                  dh[4 * j + 2 * h + 1] = 0.f;
+                  act_chunk<2>(v, p.act, nb);
+                  store(row, j, nb, v);
+                }
+              }
+            }
+          };
+          // pixel of tile row r: image tile_b, (y, x) = (tile_y0 + r / 16, tile_x0 + r % 16); false outside the image
+          auto pixel = [&](int r, long long& m, int& yx) {
+            const int yy = tile_y0 + (r >> 4), xx = tile_x0 + (r & 15);
+            yx = yy * p.W + xx;
+            m = static_cast<long long>(tile_b) * HoWo + yx;
+            return yy < p.H && xx < p.W;
+          };
+          if (staged) {
+            finish([&](int row, int j, int nb, const float (&v)[2]) {
+              const __half2 hi = __floats2half2_rn(v[0], v[1]);
+              const uint32_t off = sw128_off(row, j) + 4 * tq;
+              sts32(o_u + off, *reinterpret_cast<const uint32_t*>(&hi));
+              if constexpr (SPLIT) {
+                const float2 hf = __half22float2(hi);
+                const __half2 lo = __floats2half2_rn(v[0] - hf.x, v[1] - hf.y);
+                sts32(o_u + C::OUT_HALF + off, *reinterpret_cast<const uint32_t*>(&lo));
+              }
+            });
+            fence_proxy_async();
+            bar_sync_named(1, 128);
+            if (et == 0) {
+              if (n0 < p.Cout) {
+#pragma unroll
+                for (int hl = 0; hl < (SPLIT ? 2 : 1); ++hl)
+                  tma_store_4d(&tmap_y, o_u + hl * C::OUT_HALF, n0 + hl * p.y_lo, tile_x0, tile_y0, tile_b);
+              }
+              bulk_commit();
+            }
+          } else if constexpr (!SPLIT) {
+            // the column guards of run_epilogue: fp16 per 8-column group, fp32 NHWC per 4-column group against the row
+            // stride, fp32 NCHW per column
+            if (p.out_mode == OUT_F16_NHWC) {
+              finish([&](int row, int j, int nb, const float (&v)[2]) {
+                long long m;
+                int yx;
+                if (pixel(row, m, yx) && n0 + 8 * j < p.Cout)
+                  *reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.y) + m * p.y_ld + nb) = __floats2half2_rn(v[0], v[1]);
+              });
+            } else if (p.out_mode == OUT_F32_NHWC) {
+              finish([&](int row, int j, int nb, const float (&v)[2]) {
+                long long m;
+                int yx;
+                if (pixel(row, m, yx) && (nb & ~3) < p.y_ld)
+                  *reinterpret_cast<float2*>(reinterpret_cast<float*>(p.y) + m * p.y_ld + nb) = make_float2(v[0], v[1]);
+              });
+            } else {
+              finish([&](int row, int j, int nb, const float (&v)[2]) {
+                long long m;
+                int yx;
+                if (pixel(row, m, yx)) {
+                  float* yp = reinterpret_cast<float*>(p.y) + (static_cast<long long>(tile_b) * p.y_ld + nb) * HoWo + yx;
+                  if (nb < p.Cout) yp[0] = v[0];
+                  if (nb + 1 < p.Cout) yp[HoWo] = v[1];
+                }
+              });
+            }
+            bar_sync_named(1, 128);                           // sc_s / sh_s are rewritten by the next tile
+          }
         } else {
           // hand-over: one chunk slot, chunk parity selects the full barrier (with two epilogue groups each waits on its own)
           ChunkDump<BLOCK_N, C::CHUNK, 0>::run(d, [&](int ch, auto store) {
@@ -786,8 +910,11 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
           });
         }
       }
+      if constexpr (WIDE) {
+        if (use_tma_store && (threadIdx.x & 127) == 0) bulk_wait0();   // all stores complete before the CTA exits
+      }
     }
-  } else if constexpr (!HEAD2) {
+  } else if constexpr (!HEAD2 && !WIDE) {
     run_epilogue(0, (warp - W_EPI) * 32 + lane);          // first epilogue group (even chunks, or all of them)
   }
 }
@@ -846,7 +973,7 @@ static int num_sms() {
 template <int BLOCK_N, int MODE, int NPW, int EPI = 0>
 static int launch2_cfg(const CUtensorMap& tw, const CUtensorMap& ty, const CUtensorMap& tx, const IgemmParams& p,
                        int use_tma_store, cudaStream_t st) {
-  using C = Cfg2<BLOCK_N, MODE, EPI>;
+  using C = Cfg2<BLOCK_N, MODE, EPI, igemm2_wide(MODE, NPW)>;
   auto kern = igemm2_kernel<BLOCK_N, MODE, NPW, EPI>;
   static bool attr = false;
   if (!attr) {
@@ -999,7 +1126,7 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
     return launch2_cfg<128, MODE_CONV_TMA, 0, 2>(tw, ty, tx, pp, 0, st);
   }
   if (p.split_out && use_tma_store) {          // staged hi/lo tiles: the SPLIT instantiations (N tiles of 64 / 128 only)
-    if (mode == MODE_DCN && bn == 64) return launch2_cfg<64, MODE_DCN, 8, 1>(tw, ty, tx, pp, use_tma_store, st);
+    if (mode == MODE_DCN && bn == 64) return launch2_cfg<64, MODE_DCN, 16, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (mode == MODE_DCN && bn == 128) return launch2_cfg<128, MODE_DCN, 8, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (a_tma && bn == 64) return launch2_cfg<64, MODE_CONV_TMA, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
     if (a_tma && bn == 128) return launch2_cfg<128, MODE_CONV_TMA, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
@@ -1007,16 +1134,17 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
     if (bn == 128) return launch2_cfg<128, MODE_CONV, 4, 1>(tw, ty, tx, pp, use_tma_store, st);
   }
   if (mode == MODE_DCN && p.split_in) { set_error("dcn igemm: strict precision needs the staged TMA-store epilogue"); return -1; }
-#define MF_DISPATCH2(BN)                                                                          \
-  if (bn == BN) {                                                                                 \
-    if (mode == MODE_DCN) return launch2_cfg<BN, MODE_DCN, 8>(tw, ty, tx, pp, use_tma_store, st);  \
-    if (a_tma) return launch2_cfg<BN, MODE_CONV_TMA, 4>(tw, ty, tx, pp, use_tma_store, st);        \
-    return launch2_cfg<BN, MODE_CONV, 4>(tw, ty, tx, pp, use_tma_store, st);                       \
+  // DCN producer warps: 16 (the wide-gather configuration) for 64-column tiles, 8 otherwise
+#define MF_DISPATCH2(BN, DCN_NPW)                                                                        \
+  if (bn == BN) {                                                                                        \
+    if (mode == MODE_DCN) return launch2_cfg<BN, MODE_DCN, DCN_NPW>(tw, ty, tx, pp, use_tma_store, st);  \
+    if (a_tma) return launch2_cfg<BN, MODE_CONV_TMA, 4>(tw, ty, tx, pp, use_tma_store, st);               \
+    return launch2_cfg<BN, MODE_CONV, 4>(tw, ty, tx, pp, use_tma_store, st);                              \
   }
-  MF_DISPATCH2(16)
-  MF_DISPATCH2(32)
-  MF_DISPATCH2(64)
-  MF_DISPATCH2(128)
+  MF_DISPATCH2(16, 8)
+  MF_DISPATCH2(32, 8)
+  MF_DISPATCH2(64, 16)
+  MF_DISPATCH2(128, 8)
 #undef MF_DISPATCH2
   set_error("igemm2: unsupported block_n %d", bn);
   return -1;
