@@ -44,6 +44,13 @@ class Act(object):
         self.npar = 0        # > 0: planar stem layout with `npar` column parities (16-byte pixels)
         self.split = False   # strict precision: rows are [hi channels | lo channels], lo block `lo` elements after hi
 
+    @classmethod
+    def on(cls, buf, B, H, W, C=None, ch_off=0):
+        """activation over caller-owned rows `buf` [B*H*W, ld] fp16: channels [ch_off, ch_off + C), C defaults to the rest"""
+        a = cls(B, H, W, buf.shape[1] - ch_off if C is None else C)
+        a.buf, a.ch_off = buf, ch_off
+        return a
+
     @property
     def M(self):
         return self.B * self.H * self.W
@@ -360,11 +367,15 @@ class Plan(object):
             residual.ld if residual is not None else 0, act, OUT_F16_NHWC, y.ptr(), y.ld))
         return y
 
-    def conv_dgrad(self, dy, weight, pad, out):
-        """out += dL/dx of the stride-1 convolution y = conv(x, weight, padding=pad) given dy = dL/dy rows (its channel count
-        may be the zero-padded Cout): the forward kernel on dY with the 180-degree rotated, in/out-transposed taps, packed
-        straight from the live OIHW parameter by ONE kernel (mf_pack_conv_weight_dgrad)."""
+    def conv_dgrad(self, dy, weight, pad, out=None):
+        """dL/dx of the stride-1 convolution y = conv(x, weight, padding=pad) given dy = dL/dy rows (its channel count may be
+        the zero-padded Cout): the forward kernel on dY with the 180-degree rotated, in/out-transposed taps, packed straight
+        from the live OIHW parameter by ONE kernel (mf_pack_conv_weight_dgrad). out=None: written to a new activation;
+        otherwise accumulated in place, out += dL/dx, through the kernel's residual input. Returns the output activation."""
         cout, cin, kh, kw = weight.shape
+        res = out
+        if out is None:
+            out = self.act(dy.B, dy.H + kh - 1 - 2 * pad, dy.W + kw - 1 - 2 * pad, cin)
         assert kh == kw and kh - 1 - pad >= 0 and dy.C >= cout and (out.H, out.W) == (dy.H + kh - 1 - 2 * pad, dy.W + kw - 1 - 2 * pad)
         w = weight.detach()
         assert w.dtype == torch.float32 and w.is_contiguous()
@@ -378,7 +389,8 @@ class Plan(object):
         cpad, p2 = dy.C, kh - 1 - pad
         self.add("mf_conv2d_nhwc_f16", lambda: (
             dy.ptr(), dy.ld, dy.B, dy.H, dy.W, cpad, wp.data_ptr(), n_pad, k_pad, kh, kw, 1, p2, cin,
-            scale.data_ptr(), shift.data_ptr(), out.ptr(), out.ld, ACT_NONE, OUT_F16_NHWC, out.ptr(), out.ld))
+            scale.data_ptr(), shift.data_ptr(), res.ptr() if res is not None else None, res.ld if res is not None else 0,
+            ACT_NONE, OUT_F16_NHWC, out.ptr(), out.ld))
         return out
 
     def conv_to_f32(self, x, weight, bias, out_tensor, out_mode, act, y_ld, stride=1, pad=0, bn=None):

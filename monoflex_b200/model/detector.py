@@ -3,7 +3,7 @@ engine/trainer.py:109 and engine/inference.py:38 call it unchanged.
 
 Training mode (engine/trainer.py:103-126): `loss_dict, log_loss_dict = model(images, targets)` runs the train-mode plans
 (batch-statistics BatchNorm, running statistics updated) and the fused loss; `sum(loss_dict.values()).backward()` then
-reaches `_TapeBridge.backward`, which replays the backward tape of the two plans (monoflex_b200/tape.py, head_backward.py)
+reaches `_TapeBridge.backward`, which replays the backward tape of the two plans (monoflex_b200/tape.py)
 and ACCUMULATES the gradient of every parameter the forward used into `p.grad` - exactly what autograd does for the
 reference, so `optimizer.zero_grad(); losses.backward(); optimizer.step()` works unchanged with torch.optim.AdamW or with
 solver.FusedAdamW (whose `.grad`s are views of one arena).
@@ -97,8 +97,7 @@ class KeypointDetector(nn.Module):
     @torch.no_grad()
     def _tape_backward(self, g_cls, g_reg):
         """dL/dcls, dL/dreg -> accumulate dL/dp into p.grad for every parameter the forward used (the backward tape)."""
-        from ..head_backward import predictor_backward
-        from ..tape import backbone_backward
+        from ..tape import backbone_backward, predictor_backward
         pred_mod, S = self.heads.predictor, self.loss_scale
         plan_h, plan_b = pred_mod.last_plan, self.backbone.last_plan
         if g_cls is None:
@@ -106,7 +105,7 @@ class KeypointDetector(nn.Module):
         if g_reg is None:
             g_reg = torch.zeros_like(plan_h.reg)
         hgrads, d_feat = predictor_backward(pred_mod, plan_h, g_cls * S, g_reg * S)
-        bgrads = backbone_backward(self.backbone, plan_b, d_feat, stem_wgrad=True)
+        bgrads = backbone_backward(self.backbone, plan_b, d_feat)
         params = getattr(self, "_param_by_name", None)
         if params is None:
             params = self._param_by_name = dict(self.named_parameters())
@@ -115,8 +114,6 @@ class KeypointDetector(nn.Module):
         acc_dst, acc_src = [], []
         for prefix, grads in (("heads.predictor.", hgrads), ("backbone.", bgrads)):
             for name, g in grads.items():
-                if g is None:
-                    raise RuntimeError("backward tape produced no gradient for %s%s" % (prefix, name))
                 p = params[prefix + name]
                 used.add(prefix + name)
                 if not p.requires_grad:

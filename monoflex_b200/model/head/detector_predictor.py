@@ -265,10 +265,11 @@ class _predictor(nn.Module):
         P.cls, P.reg, P.hidden = cls, reg, hid
         # the edge fusion's gathered rows [B,1,K+2,256] and the border-pixel mask of the hidden rows (None where not built)
         P.ea, P.eb, P.hid_mask = ea, eb, hid_mask
-        if P.train:       # what head_backward.predictor_backward needs: activations kept by the train-mode forward
-            P.ctx = dict(x=x, hid=hid, ea=ea, eb=eb,
-                         bn={id(m): (raw, y, st, c0, cc) for (m, raw, y, st, c0, cc) in P.bn_saved}, K_edge=K_edge,
-                         off_ch0=off_ch0, ch0s=ch0s)
+        if P.train:       # what tape.predictor_backward needs: activations kept by the train-mode forward
+            bn = {}       # normalisation module -> its Plan.bn_saved entries
+            for entry in P.bn_saved:
+                bn.setdefault(id(entry[0]), []).append(entry)
+            P.ctx = dict(x=x, hid=hid, ea=ea, eb=eb, bn=bn, K_edge=K_edge, off_ch0=off_ch0, ch0s=ch0s)
         return P
 
     def plan_for(self, features, K_edge):
@@ -293,7 +294,7 @@ class _predictor(nn.Module):
 
     def train_forward(self, features, targets):
         """Train-mode forward (InPlaceABN / BatchNorm1d on batch statistics); keeps the activations
-        head_backward.predictor_backward needs (driven by KeypointDetector's tape bridge)."""
+        tape.predictor_backward needs (driven by KeypointDetector's tape bridge)."""
         if not self.training:
             raise RuntimeError("train_forward needs module.train()")
         return self._run(features, targets)

@@ -1,207 +1,170 @@
-"""Backward of the backbone (DLA-34 base + DLAUp/IDAUp with DCNv2, model/backbone/dla_dcn.py) from the tape the train-mode
-forward plan recorded (engine.Plan.tape): one record per emitted layer, replayed in reverse emission order, each record's
-backward composed from the operators of the C ABI (csrc/mf_wgrad.cu, mf_bn_train.cu, mf_dcn_bwd.cu, mf_bwd_misc.cu and
-the forward implicit-GEMM kernel for the data gradients).
+"""Whole-network backward from what the train-mode forward plans kept, every layer's backward one operator of backward.py:
 
-Gradient bookkeeping: every activation buffer of the plan gets a zero-initialised fp16 gradient buffer of the same shape
-(channel slices of a Root concatenation share their parent's, exactly like the forward shares storage) and EVERY backward
-operator accumulates into it - stride-1 data gradients through the forward kernel's fused residual input (in place), the
-others through a temporary + `mf_add_rows_f16`. Accumulating everywhere makes the result independent of which consumer of
-a multiply-used activation runs first. Weight gradients are fp32. Gradients travel in fp16, so the seed must carry a loss
-scale (see head_backward.py).
+  * predictor_backward: the predictor (detector_predictor.py:121-165) from the activations its plan kept (`plan.ctx`,
+    model/head/detector_predictor.py): loss gradients -> sigmoid_hm -> edge-fusion tail -> 1x1 heads -> InPlaceABN -> the
+    nine 3x3 convs -> gradient of the backbone's feature map;
+  * backbone_backward: the backbone (DLA-34 base + DLAUp/IDAUp with DCNv2, model/backbone/dla_dcn.py) from the tape its
+    plan recorded (engine.Plan.tape), one record per emitted layer, replayed in reverse emission order.
 
-The 7x7 stem convolution reads the 8-channel packed image; with `stem_wgrad=True` its weight gradient runs on a 16-channel
-zero-padded copy of the rows (the narrowest box the tensor-core wgrad takes) - written but NOT yet run on hardware (the
-round's GPU budget ended), so it is opt-in and the default reports that one gradient as missing (None).
+Both return {parameter name: fp32 gradient} for every parameter the forward used. Gradients flow in fp16 NHWC rows, so the
+caller multiplies the loss gradients by a loss scale (>= 128) and divides the results by it, like any fp16 training step.
+
+Backbone bookkeeping: every activation buffer of the plan gets a zero-initialised fp16 gradient buffer of the same shape
+(channel slices of a Root concatenation share their parent's, exactly like the forward shares storage) and every backward
+operator accumulates into it. That makes the result independent of which consumer of a multiply-used activation runs first.
 """
 import torch
 
-from . import engine
-from ._lib import call, load
-from .backward import column_sum, conv2d_dgrad_stride2
+from . import backward, engine
+from ._lib import call, stream
 
 
-def _st():
-    return torch.cuda.current_stream().cuda_stream
+def _collector(module):
+    """({parameter name: fp32 gradient}, put(param, value)) for the parameters of `module`; put(None, ...) does nothing"""
+    names = {id(p): n for n, p in module.named_parameters()}
+    grads = {}
+
+    def put(param, value):
+        if param is not None:
+            grads[names[id(param)]] = value.reshape(param.shape).float()
+    return grads, put
 
 
-class _Grads(object):
-    """fp16 gradient buffers mirroring the plan's activation buffers."""
-
-    def __init__(self, device):
-        self.device = device
-        self.bufs = {}
-
-    def of(self, act):
-        key = act.buf.data_ptr()
-        g = self.bufs.get(key)
-        if g is None:
-            g = torch.zeros_like(act.buf)
-            self.bufs[key] = g
-        return g
-
-    def ptr(self, act):
-        return self.of(act).data_ptr() + 2 * act.ch_off
-
-    def ld(self, act):
-        return self.of(act).shape[1]
-
-    def add(self, act, src, src_ld=None):
-        """grad(act) += src ([M, >= C] fp16 rows)"""
-        call("mf_add_rows_f16", self.ptr(act), self.ld(act), src.data_ptr(), src.shape[1] if src_ld is None else src_ld, act.M, act.C,
-             _st())
-
-    def bound(self, plan, act):
-        """an engine.Act of `plan` whose storage is grad(act) (for kernels driven through engine.Plan)"""
-        a = plan.act(act.B, act.H, act.W, act.C)
-        a.buf, a.ch_off = self.of(act), act.ch_off
-        return a
-
-
-def _bn_backward(rec_bn, raw, y, dy_ptr, dy_ld, d_raw, d_res, act, abs_weight, put):
-    M, dev = raw.M, d_raw.device
-    for (mod, _raw, _y, stats, c0, cc) in rec_bn:
-        dg = torch.empty(2, cc, dtype=torch.float32, device=dev)
-        ws = torch.empty(max(1, load().mf_bn_train_workspace(M, cc) // 4), dtype=torch.float32, device=dev)
-        engine.bn_backward_launch(mod, raw.ptr() + 2 * c0, raw.ld, dy_ptr + 2 * c0, dy_ld, y.ptr() + 2 * c0, y.ld, M, cc, stats, act,
-                                  d_raw.data_ptr() + 2 * c0, d_raw.shape[1],
-                                  (d_res.data_ptr() + 2 * c0) if d_res is not None else None,
-                                  d_res.shape[1] if d_res is not None else 0, dg, ws, _st())
-        off = c0 - rec_bn[0][4]                                   # slices of one module are consecutive 256-channel chunks
-        put(mod.weight, dg[0] * torch.sign(mod.weight.detach()[off:off + cc]) if abs_weight else dg[0], off, cc)
-        put(mod.bias, dg[1], off, cc)
-
-
-def _conv_backward(G, x, weight, bias, stride, pad, d_raw, B, Ho, Wo, put, need_dx=True, stem_wgrad=False):
-    """gradients of y = conv(x, weight) + bias given d_raw = dL/dy rows [B*Ho*Wo, Cout(_padded)] fp16."""
-    dev = d_raw.device
-    cout, cin, kh, kw = weight.shape
-    cout_p = d_raw.shape[1]
-    if x.C != 8 and (cin in (16, 32) or cin % 64 == 0):
-        dw = torch.empty(cout_p, cin, kh, kw, dtype=torch.float32, device=dev)
-        call("mf_conv2d_wgrad_nhwc_f16", x.ptr(), x.ld, x.B, x.H, x.W, cin, d_raw.data_ptr(), cout_p, cout_p, kh, stride, pad,
-             dw.data_ptr(), _st())
-        put(weight, dw[:cout])
-    elif x.C == 8 and stem_wgrad:
-        # 7x7 stem on the packed image (8 channels = 3 real + 5 zero): widen the rows to the narrowest supported box (16)
-        cin_w_real = weight.shape[1]
-        x16 = torch.zeros(x.M, 16, dtype=torch.half, device=dev)
-        x16[:, :8] = x.buf.view(x.M, -1)[:, x.ch_off:x.ch_off + 8]
-        dw = torch.empty(cout_p, 16, kh, kw, dtype=torch.float32, device=dev)
-        call("mf_conv2d_wgrad_nhwc_f16", x16.data_ptr(), 16, x.B, x.H, x.W, 16, d_raw.data_ptr(), cout_p, cout_p, kh, stride, pad,
-             dw.data_ptr(), _st())
-        put(weight, dw[:cout, :cin_w_real])
-    else:
-        put(weight, None)
-    if bias is not None:
-        put(bias, column_sum(d_raw)[:cout])
-    if not need_dx:
-        return
-    w = weight.detach().float()
-    if stride == 1 and w.is_contiguous() and kh == kw:
-        P = engine.Plan(str(dev))
-        dya = P.act(B, Ho, Wo, cout_p)
-        dya.buf = d_raw
-        gx = G.bound(P, x)
-        P.conv_dgrad(dya, w, pad, gx)                                # grad(x) += dgrad, in place (rotated taps packed in one kernel)
-        P.finalize()
-        P.run()
-        return
-    if cout_p != cout:
-        w = torch.cat([w, torch.zeros(cout_p - cout, cin, kh, kw, device=dev)], 0)
-    if stride == 1:
-        w_rot = w.flip(2, 3).transpose(0, 1).contiguous()           # [Cin, Cout_p, k, k]
-        P = engine.Plan(str(dev))
-        dya = P.act(B, Ho, Wo, cout_p)
-        dya.buf = d_raw
-        gx = G.bound(P, x)
-        P.conv(dya, w_rot, 1, kh - 1 - pad, None, act=engine.ACT_NONE, residual=gx, out=gx)      # grad(x) += dgrad, in place
-        P.finalize()
-        P.run()
-    else:
-        if (stride, kh, pad) != (2, 3, 1):
-            raise NotImplementedError("tape: data gradient of a %dx%d stride-%d pad-%d convolution" % (kh, kw, stride, pad))
-        G.add(x, conv2d_dgrad_stride2(d_raw, w, B, Ho, Wo))
+def _put_bn(put, results):
+    for mod, dgamma, dbeta in results:
+        put(mod.weight, dgamma)
+        put(mod.bias, dbeta)
 
 
 @torch.no_grad()
-def backbone_backward(backbone, plan, d_feat_rows, stem_wgrad=False):
+def predictor_backward(pred, plan, grad_cls, grad_reg):
+    """pred: the `_predictor` module in train mode, plan: its last train-mode plan (pred.last_plan), grad_cls [B,3,H,W] /
+    grad_reg [B,50,H,W] fp32: (scaled) loss gradients w.r.t. the predictor outputs.
+    Returns (grads, d_features: [B*H*W, 64] fp16 rows)."""
+    ctx = plan.ctx
+    x, hid = ctx["x"], ctx["hid"]
+    B, H, W, hc = x.B, x.H, x.W, pred.head_conv
+    M, dev = B * H * W, grad_reg.device
+    HW = H * W
+    grads, put = _collector(pred)
+    branches = [pred.class_head] + list(pred.reg_features)
+    head_lists = [[pred.class_head[2]]] + [list(h) for h in pred.reg_heads]
+    nb = len(branches)
+    # ---- sigmoid_hm
+    g_logits = backward.sigmoid_clamp_backward(plan.cls, grad_cls.contiguous())
+    d_hid = torch.zeros(M, nb * hc, dtype=torch.half, device=dev)          # gradient of the activated hidden map [M, 2304]
+    # ---- 1x1 heads: weight / bias gradients and d_hid = dY W
+    dys = []
+    for i, heads in enumerate(head_lists):
+        n_i = sum(h.weight.shape[0] for h in heads)
+        src = g_logits if i == 0 else grad_reg[:, ctx["ch0s"][i - 1]:ctx["ch0s"][i - 1] + n_i].contiguous()
+        dy = torch.zeros(M, 32, dtype=torch.half, device=dev)
+        call("mf_nchw_f32_to_nhwc_f16", src.data_ptr(), dy.data_ptr(), B, n_i, HW, 32, stream())
+        dys.append(dy)
+        dw = backward.conv2d_wgrad(engine.Act.on(hid.buf, B, H, W, hc, hid.ch_off + i * hc), dy, B, H, W, 1)
+        db = backward.column_sum(dy)
+        r = 0
+        for h in heads:
+            n = h.weight.shape[0]
+            put(h.weight, dw[r:r + n])
+            put(h.bias, db[r:r + n])
+            r += n
+
+    def heads_dgrad(P):
+        for i, heads in enumerate(head_lists):
+            wcat = torch.cat([h.weight.detach().float().reshape(h.weight.shape[0], hc) for h in heads], 0)      # [n_i, 256]
+            wd = torch.zeros(hc, 32, 1, 1, dtype=torch.float32, device=dev)
+            wd[:, :wcat.shape[0], 0, 0] = wcat.t()
+            P.conv(engine.Act.on(dys[i], B, H, W), wd, 1, 0, None, act=engine.ACT_NONE, out=engine.Act.on(d_hid, B, H, W, hc, i * hc))
+    backward.run_plan(dev, heads_dgrad)
+    # ---- edge-fusion tail
+    if pred.enable_edge_fusion:
+        K = ctx["K_edge"]
+        d_e = []
+        for seq, g_map, ctot, ch0, src in ((pred.trunc_heatmap_conv, g_logits, pred.num_classes, 0, ctx["ea"]),
+                                          (pred.trunc_offset_conv, grad_reg.contiguous(), pred.num_reg, ctx["off_ch0"], ctx["eb"])):
+            entries = ctx["bn"][id(seq[1])]
+            t_y = entries[0][2]
+            n_out = seq[3].weight.shape[0]
+            w2 = seq[3].weight.detach().float().reshape(n_out, hc).contiguous()
+            d_t = torch.empty(B * K, hc, dtype=torch.half, device=dev)
+            dw2 = torch.empty(n_out, hc, dtype=torch.float32, device=dev)
+            db2 = torch.empty(n_out, dtype=torch.float32, device=dev)
+            call("mf_edge_head_add_bwd", t_y.ptr(), w2.data_ptr(), n_out, plan.edge_idx.data_ptr(), plan.edge_len.data_ptr(),
+                 g_map.data_ptr(), ctot, ch0, d_t.data_ptr(), dw2.data_ptr(), db2.data_ptr(), B, K, H, W, stream())
+            put(seq[3].weight, dw2)
+            put(seq[3].bias, db2)
+            d_raw = torch.empty(B * K, hc, dtype=torch.half, device=dev)
+            _put_bn(put, backward.bn_backward(entries, d_t, d_raw, engine.ACT_NONE))
+            dw1 = torch.empty(hc, hc, 1, 3, dtype=torch.float32, device=dev)
+            call("mf_conv2d_wgrad_rect_nhwc_f16", src.ptr(), src.ld, B, 1, K + 2, hc, d_raw.data_ptr(), hc, hc, 1, 3, 1, 0, 0,
+                 dw1.data_ptr(), stream())
+            put(seq[0].weight, dw1)
+            put(seq[0].bias, backward.column_sum(d_raw))
+            # Conv1d data gradient: correlation of d_raw with the flipped, transposed taps, 2 columns of zero padding
+            w5 = torch.zeros(hc, hc, 5, 3, dtype=torch.float32, device=dev)
+            w5[:, :, 2, :] = seq[0].weight.detach().float().flip(2).transpose(0, 1)
+            d_e.append(backward.run_plan(dev, lambda P: P.conv(engine.Act.on(d_raw, B, 1, K), w5, 1, 2, None, act=engine.ACT_NONE)))
+        cols = (0, (pred.offset_index[0] + 1) * hc)
+        call("mf_edge_gather_bwd", d_e[0].ptr(), d_e[1].ptr(), cols[0], cols[1], plan.edge_idx.data_ptr(), d_hid.data_ptr(), nb * hc,
+             B, H, W, K, pred.output_width, pred.output_height, stream())
+    # ---- InPlaceABN (leaky 0.01) per branch, in place on the gradient buffer: d_hid -> d_hid_raw
+    entries = [e for b in branches for e in ctx["bn"][id(b[1])]]
+    _put_bn(put, backward.bn_backward(entries, d_hid, d_hid, engine.ACT_LEAKY, abs_weight=True))
+    # ---- the nine 3x3 convolutions: one wgrad with Cout = 2304, one dgrad with Cin = 2304
+    dw_all = backward.conv2d_wgrad(x, d_hid, B, H, W, 3, 1, 1)
+    for i, b in enumerate(branches):
+        put(b[0].weight, dw_all[i * hc:(i + 1) * hc])
+    w_all = torch.cat([b[0].weight.detach() for b in branches], 0)
+    return grads, backward.conv2d_dgrad(d_hid, w_all, B, H, W, 1)
+
+
+@torch.no_grad()
+def backbone_backward(backbone, plan, d_feat_rows):
     """backbone: DLASeg in train mode, plan: its last train-mode plan (backbone.last_plan), d_feat_rows [B*H/4*W/4, 64] fp16:
-    (scaled) gradient of the loss w.r.t. the backbone's output feature map.
-    Returns {parameter name: fp32 gradient or None (not built)} for every parameter the forward used."""
-    dev = d_feat_rows.device
-    G = _Grads(dev)
-    names = {id(p): n for n, p in backbone.named_parameters()}
-    grads = {}
+    (scaled) gradient of the loss w.r.t. the backbone's output feature map. Returns grads."""
+    grads, put = _collector(backbone)
+    bufs = {}
 
-    def put(param, value, off=0, cc=None):
-        n = names[id(param)]
-        if value is None:
-            grads[n] = None
-            return
-        if cc is None or cc == param.numel():
-            grads[n] = value.reshape(param.shape).float()
-        else:                                                       # one 256-channel chunk of a wider normalisation layer
-            if n not in grads or grads[n] is None:
-                grads[n] = torch.zeros(param.shape, dtype=torch.float32, device=dev)
-            grads[n].view(-1)[off:off + cc] = value
+    def grad(a):
+        """engine.Act over the gradient buffer of activation `a`"""
+        g = bufs.get(a.buf.data_ptr())
+        if g is None:
+            g = bufs[a.buf.data_ptr()] = torch.zeros_like(a.buf)
+        return engine.Act.on(g, a.B, a.H, a.W, a.C, a.ch_off)
 
-    G.add(plan.output, d_feat_rows.contiguous())
+    backward.add_rows(grad(plan.output), d_feat_rows.contiguous())
     for rec in reversed(plan.tape):
-        kind = rec["kind"]
+        kind, x, y = rec["kind"], rec["x"], rec["y"]
         if kind == "conv_bn":
-            x, raw, y, residual = rec["x"], rec["raw"], rec["y"], rec["residual"]
-            d_raw = torch.empty(raw.M, raw.C, dtype=torch.half, device=dev)
-            d_res = torch.empty(raw.M, raw.C, dtype=torch.half, device=dev) if residual is not None else None
-            _bn_backward(rec["bn"], raw, y, G.ptr(y), G.ld(y), d_raw, d_res, rec["act"], rec["abs_weight"], put)
+            raw, residual = rec["raw"], rec["residual"]
+            d_raw = torch.empty(raw.M, raw.C, dtype=torch.half, device=raw.buf.device)
+            d_res = torch.empty_like(d_raw) if residual is not None else None
+            _put_bn(put, backward.bn_backward(rec["bn"], grad(y), d_raw, rec["act"], rec["abs_weight"], d_res))
             if residual is not None:
-                G.add(residual, d_res)
-            _conv_backward(G, x, rec["weight"], rec["bias"], rec["stride"], rec["pad"], d_raw, raw.B, raw.H, raw.W, put,
-                           need_dx=x is not plan.input, stem_wgrad=stem_wgrad)
+                backward.add_rows(grad(residual), d_res)
+            dw, db = backward.conv_backward(x, rec["weight"], rec["bias"], rec["stride"], rec["pad"], d_raw,
+                                            None if x is plan.input else grad(x))
+            put(rec["weight"], dw)
+            put(rec["bias"], db)
         elif kind == "dcn":
-            x, raw, y, mod, om = rec["x"], rec["raw"], rec["y"], rec["mod"], rec["om"]
-            d_raw = torch.empty(raw.M, raw.C, dtype=torch.half, device=dev)
-            _bn_backward(rec["bn"], raw, y, G.ptr(y), G.ld(y), d_raw, None, engine.ACT_RELU, False, put)
-            C, cout = x.C, raw.C
-            # grad columns (1x1 forward conv of dY with W^T), sampled columns, col2im + coord, wgrad - backward.dcn_backward
-            # inlined so that x may be a channel slice (ld != C)
-            wt = mod.weight.detach().float().permute(2, 3, 1, 0).reshape(9 * C, cout, 1, 1).contiguous()
-            P = engine.Plan(str(dev))
-            dya = P.act(x.B, x.H, x.W, cout)
-            dya.buf = d_raw
-            gcol = P.conv(dya, wt, 1, 0, None, act=engine.ACT_NONE)
-            P.finalize()
-            P.run()
-            cols = torch.empty(x.M, 9 * C, dtype=torch.half, device=dev)
-            call("mf_dcn_sample_cols_nhwc_f16", x.ptr(), x.ld, om.data_ptr(), 32, cols.data_ptr(), x.B, x.H, x.W, C, _st())
-            dw9 = torch.empty(cout, 9 * C, 1, 1, dtype=torch.float32, device=dev)
-            call("mf_conv2d_wgrad_nhwc_f16", cols.data_ptr(), 9 * C, x.B, x.H, x.W, 9 * C, d_raw.data_ptr(), cout, cout, 1, 1, 0,
-                 dw9.data_ptr(), _st())
-            put(mod.weight, dw9.view(cout, 3, 3, C).permute(0, 3, 1, 2).contiguous())
-            put(mod.bias, column_sum(d_raw))
-            dx = torch.empty(x.M, C, dtype=torch.half, device=dev)
-            dom = torch.empty(x.M, 32, dtype=torch.float32, device=dev)
-            call("mf_dcn_col2im_nhwc_f16", x.ptr(), x.ld, om.data_ptr(), 32, gcol.ptr(), dx.data_ptr(), C, dom.data_ptr(), x.B, x.H,
-                 x.W, C, _st())
-            G.add(x, dx)
+            raw, mod = rec["raw"], rec["mod"]
+            d_raw = torch.empty(raw.M, raw.C, dtype=torch.half, device=raw.buf.device)
+            _put_bn(put, backward.bn_backward(rec["bn"], grad(y), d_raw, engine.ACT_RELU))
+            _, dom, dw, db = backward.dcn_backward(x, rec["om"], d_raw, mod.weight, x.B, x.H, x.W, grad(x))
+            put(mod.weight, dw)
+            put(mod.bias, db)
             # offset / mask convolution (3x3, bias, 27 -> padded 32 output channels): its pre-activation gradient is `dom`
-            _conv_backward(G, x, mod.conv_offset_mask.weight, mod.conv_offset_mask.bias, 1, 1, dom.half(), x.B, x.H, x.W, put)
+            om = mod.conv_offset_mask
+            dw, db = backward.conv_backward(x, om.weight, om.bias, 1, 1, dom.half(), grad(x))
+            put(om.weight, dw)
+            put(om.bias, db)
         elif kind == "maxpool2":
-            x, y = rec["x"], rec["y"]
-            dx = torch.empty(x.M, x.C, dtype=torch.half, device=dev)
-            call("mf_maxpool2_bwd_nhwc_f16", x.ptr(), G.ptr(y), dx.data_ptr(), x.B, x.H, x.W, x.C, x.ld, G.ld(y), x.C, _st())
-            G.add(x, dx)
+            backward.maxpool2_backward(x, grad(y), x.B, x.H, x.W, grad(x))
         elif kind == "upsample_add":
-            x, y, skip, f, wt = rec["x"], rec["y"], rec["skip"], rec["f"], rec["wt"]
-            C = x.C
-            if skip is not None:
-                call("mf_add_rows_f16", G.ptr(skip), G.ld(skip), G.ptr(y), G.ld(y), y.M, C, _st())
-            dx = torch.empty(x.M, C, dtype=torch.half, device=dev)
-            dw = torch.empty(4 * f * f, C, dtype=torch.float32, device=dev)
-            ws = torch.empty(max(1, load().mf_upsample_bwd_workspace(x.B, x.H, x.W, C, f) // 4), dtype=torch.float32, device=dev)
-            call("mf_upsample_bwd_nhwc_f16", x.ptr(), wt.data_ptr(), G.ptr(y), dx.data_ptr(), dw.data_ptr(), x.B, x.H, x.W, C, f, x.ld,
-                 G.ld(y), C, ws.data_ptr(), _st())
-            G.add(x, dx)
+            skip = rec["skip"]
+            _, dw = backward.upsample_backward(x, rec["wt"], grad(y), x.B, x.H, x.W, rec["f"], grad(x),
+                                              grad(skip) if skip is not None else None)
             put(rec["weight"], dw.t().contiguous())
         else:
             raise NotImplementedError("tape record %r" % kind)

@@ -403,10 +403,12 @@ def test_training_backward_on_edge_menu(case):
 
 
 def test_tape_call_form_on_a_channel_slice():
-    """the tape's inline form: mf_dcn_sample_cols_nhwc_f16 and mf_dcn_col2im_nhwc_f16 read x as a channel slice
-    (x_ld != C) of a wider buffer, with a given fp16 column gradient. The sampled columns must equal those of the compact
-    layout bit for bit; with gcol given exactly, dOffset and dMask are fp32 sums over exact products (1e-5), dX carries the
-    fp16 atomics (1e-2)."""
+    """the tape's call form: x is a channel slice (x_ld != C) of a wider buffer. Kernels: mf_dcn_sample_cols_nhwc_f16 and
+    mf_dcn_col2im_nhwc_f16 with a given fp16 column gradient - the sampled columns must equal those of the compact layout bit
+    for bit; with gcol given exactly, dOffset and dMask are fp32 sums over exact products (1e-5), dX carries the fp16 atomics
+    (1e-2). Operator: backward.dcn_backward on the slice, dX accumulated into the same slice of a gradient buffer (whose
+    other channels stay untouched), against float64 with the tolerances of test_training_backward_on_edge_menu."""
+    from monoflex_b200 import backward
     B, C, H, W = 2, 128, 11, 13
     M = B * H * W
     gen = np.random.Generator(np.random.PCG64(21))
@@ -443,6 +445,23 @@ def test_tape_call_form_on_a_channel_slice():
     for name, got, want, tol in (("dX", nchw(dx, B, H, W), dx64, 1e-2), ("dOffset", dom[:, :18], doff64, 1e-5),
                                  ("dMask pre-activation", dom[:, 18:27], dm64 * m * (1 - m), 1e-5)):
         assert rel(got, want) < tol, (name, rel(got, want), worst(got, want))
+    # the full operator on the slice
+    Co = 64
+    w = h16(torch.from_numpy((gen.standard_normal((Co, C, 3, 3)) / np.sqrt(9 * C)).astype(np.float32))).cuda()
+    dy = h16(torch.from_numpy(gen.standard_normal((B, Co, H, W)).astype(np.float32))).cuda()
+    gbuf = torch.zeros(M, lx, dtype=torch.half, device="cuda")
+    _, dom, dw, db = backward.dcn_backward(engine.Act.on(xbuf, B, H, W, C, xo), om, rows16(dy), w, B, H, W,
+                                           dx=engine.Act.on(gbuf, B, H, W, C, xo))
+    torch.cuda.synchronize()
+    assert (gbuf[:, :xo] == 0).all() and (gbuf[:, xo + C:] == 0).all(), "channels outside the dX slice were written"
+    dx64, doff64, dm64 = dcn_ref.backward(x, offset, mask, _gcol64(w, dy))
+    dw64 = torch.einsum("bohw,bcthw->oct", dy.double(), dcn_ref.columns(x, offset, mask)).reshape(Co, C, 3, 3)
+    dom = nchw(dom, B, H, W)
+    for name, got, want, tol in (("dX", nchw(gbuf[:, xo:xo + C], B, H, W), dx64, 1e-2), ("dOffset", dom[:, :18], doff64, 1e-2),
+                                 ("dMask pre-activation", dom[:, 18:27], dm64 * m * (1 - m), 1e-2), ("dW", dw, dw64, 3e-3),
+                                 ("dB", db, dy.double().sum((0, 2, 3)), 1e-4)):
+        assert rel(got, want) < tol, ("operator", name, rel(got, want), worst(got, want))
+    assert (dom[:, 27:] == 0).all()
 
 
 def test_zero_offsets_half_mask_backward_known_answer():

@@ -7,7 +7,6 @@ import sys
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from monoflex_b200 import backward                                        # noqa: E402
 from monoflex_b200._lib import call                                       # noqa: E402
 
 SHAPES = [(8, 96, 320, 64, 64, 3, 1, 1), (8, 48, 160, 128, 128, 3, 1, 1), (8, 24, 80, 256, 256, 3, 1, 1),

@@ -42,12 +42,10 @@ def main():
     S = 64.0
     ms = build(True)
     f_r = ms.backbone.train_forward(x[rank:rank + 1]).float()
-    g_r = backbone_backward(ms.backbone, ms.backbone.last_plan, (f_r * S).permute(0, 2, 3, 1).reshape(-1, f_r.shape[1]).half().contiguous(),
-                            stem_wgrad=True)
+    g_r = backbone_backward(ms.backbone, ms.backbone.last_plan, (f_r * S).permute(0, 2, 3, 1).reshape(-1, f_r.shape[1]).half().contiguous())
     mb = build(False)
     f_b = mb.backbone.train_forward(x).float()
-    g_b = backbone_backward(mb.backbone, mb.backbone.last_plan, (f_b * S).permute(0, 2, 3, 1).reshape(-1, f_b.shape[1]).half().contiguous(),
-                            stem_wgrad=True)
+    g_b = backbone_backward(mb.backbone, mb.backbone.last_plan, (f_b * S).permute(0, 2, 3, 1).reshape(-1, f_b.shape[1]).half().contiguous())
     torch.cuda.synchronize()
     feat_err = float((f_r[0] - f_b[rank]).abs().max() / f_b[rank].abs().max())
     # the statistics agree to fp32 rounding; what differs downstream are fp16 storage roundings that flip on last-bit differences
