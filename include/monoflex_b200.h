@@ -289,17 +289,18 @@ int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* 
  *   out48 (device): [0..10] the 11 losses in LOSS_NAMES order; [16..27] 2D_IoU, depth_loss(log), keypoint_depth_loss(log),
  *       depth_MAE, center_MAE, 02_MAE, 13_MAE, lower_MAE, hard_MAE, soft_MAE, mean_MAE, 3D_IoU (mean over the labelled
  *       objects of get_iou_3d of the predicted and the label corners, 0 without objects); [32..38] counts
- *   ws64 (device): normalisers kept for the backward call.  No host synchronisation in either call.
+ *   ws96 (device, 96 floats): normalisers and the per-image key-point f_u kept for the backward call (24 + B <= 88
+ *       floats are used at B = 64).  No host synchronisation in either call.
  * mf_loss_backward: grad_losses11 (device) = upstream gradient of each loss (ones for the trainer's plain sum,
  * engine/trainer.py:109-110); writes grad_reg [B,50,H,W] (zero except at object centres) and grad_cls [B,ncls,H,W];
  * either may be NULL. */
 int mf_loss_obj_cols(void);
 int mf_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                     const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                    float* out48, float* ws64, void* stream);
+                    float* out48, float* ws96, void* stream);
 int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                      const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                     const float* ws64, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream);
+                     const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream);
 
 /* get_iou_3d (model/layers/iou_loss.py:99-136): out[i] = float32 3D IoU of the boxes pred[i] and target[i], each given by its
  * 8 corners in Anno_Encoder.encode_box3d's order (model/anno_encoder.py:88-122); pred, target [N,8,3] float32, out [N] float32,

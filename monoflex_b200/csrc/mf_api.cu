@@ -453,14 +453,14 @@ int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* 
 int mf_loss_obj_cols(void) { return MF_LOSS_OBJ_COLS; }
 int mf_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                     const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                    float* out48, float* ws64, void* stream) {
-  return launch_loss_forward(pred_cls, hm, pred_reg, obj, img, weights11, dim_mean9, B, ncls, M, H, W, C, out48, ws64,
+                    float* out48, float* ws96, void* stream) {
+  return launch_loss_forward(pred_cls, hm, pred_reg, obj, img, weights11, dim_mean9, B, ncls, M, H, W, C, out48, ws96,
                              MF_STREAM(stream));
 }
 int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                      const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                     const float* ws64, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream) {
-  return launch_loss_backward(pred_cls, hm, pred_reg, obj, img, weights11, dim_mean9, B, ncls, M, H, W, C, ws64,
+                     const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream) {
+  return launch_loss_backward(pred_cls, hm, pred_reg, obj, img, weights11, dim_mean9, B, ncls, M, H, W, C, ws96,
                               grad_losses11, grad_cls, grad_reg, MF_STREAM(stream));
 }
 int mf_adamw_chunk(void) { return MF_ADAMW_CHUNK; }

@@ -21,12 +21,13 @@ int launch_edge_mask(const long long* edge_idx, unsigned char* mask, int B, int 
                      cudaStream_t st);
 int launch_focal_loss(const float* pred, const float* tgt, long long n, float* out2, cudaStream_t st);
 #define MF_LOSS_OBJ_COLS 64   /* floats per (image, object slot) row of the packed label table (mf_loss.cu) */
+#define MF_LOSS_WS_FLOATS 96  /* floats of the loss workspace: 24 fixed slots + f_u of up to 64 images (mf_loss.cu) */
 int launch_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                         const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                        float* out48, float* ws64, cudaStream_t st);
+                        float* out48, float* ws96, cudaStream_t st);
 int launch_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                          const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                         const float* ws64, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st);
+                         const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st);
 int launch_mn_major_selftest(const __half* a_km, const __half* b_kn, float* d_mn, cudaStream_t st);
 int launch_maxpool2_bwd(const __half* x, const __half* dy, __half* dx, int B, int H, int W, int C, int x_ld, int dy_ld,
                         int dx_ld, cudaStream_t st);

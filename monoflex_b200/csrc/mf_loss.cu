@@ -262,12 +262,14 @@ __device__ void object_terms(const T* p, const float* __restrict__ o, const floa
 }
 
 // ------------------------------------------------------------------------------------------------ kernels
-// ws layout (floats): [0..NTERM) coef (weight / normaliser) per internal term, [16] hm scale = w_hm / clamp(num_pos, 1),
-// [17] hm scale * upstream grad (written by backward), [24..24+B) f_u used for the key-point depths of image b
+// ws layout (MF_LOSS_WS_FLOATS floats): [0..NTERM) coef (weight / normaliser) per internal term, [16] hm scale =
+// w_hm / clamp(num_pos, 1), [17] hm scale * upstream grad (written by backward), [20..22) focal sum and num_pos,
+// [24..24+B) f_u used for the key-point depths of image b (B <= 64)
 #define WS_COEF 0
 #define WS_HM 16
 #define WS_HMG 17
 #define WS_FUKP 24
+static_assert(WS_FUKP + 64 <= MF_LOSS_WS_FLOATS, "loss workspace too small for the f_u of 64 images");
 
 template <int N>
 __device__ void block_sum(float (&v)[N], float* sm /* [32*N] */) {
@@ -325,8 +327,10 @@ __global__ void __launch_bounds__(256) loss_forward_kernel(const float* __restri
     s_coef[T_KD_VALID] = w[8] / fmaxf(nkv, 1.f);
     s_coef[T_KD_INVALID] = w[8] / fmaxf(3.f * n3 - nkv, 1.f);
     s_coef[T_WAD] = w[10] / n3;
-    if (n3 == 0.f)                                                         // no object in the whole batch (reference crashes)
-      for (int k = 0; k < NTERM; ++k) s_coef[k] = 0.f;
+    if (n3 == 0.f)                                                         // no object in the whole batch (reference crashes):
+      for (int k = 0; k < NTERM; ++k) s_coef[k] = 0.f;                     // every regression loss and gradient is 0, the
+                                                                           // logged means 0 but keypoint_depth_loss, the
+                                                                           // mean over no valid group (NaN, as below)
     // anno_encoder.py:186: `calib = calibs[idx]` with idx = rank of the image among the images that own objects
     int rank = 0;
     for (int b = 0; b < c.B && b < 64; ++b) {
@@ -424,33 +428,33 @@ static int fill_cfg(LossCfg& c, const float* weights11, const float* dim_mean9, 
 
 int launch_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                         const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                        float* out48, float* ws64, cudaStream_t st) {
+                        float* out48, float* ws96, cudaStream_t st) {
   LossCfg c;
   if (fill_cfg(c, weights11, dim_mean9, B, M, H, W, C)) return -1;
-  float* focal2 = ws64 + 20;                                               // [20] loss sum, [21] num_pos
+  float* focal2 = ws96 + 20;                                               // [20] loss sum, [21] num_pos
   if (launch_focal_loss(pred_cls, hm, static_cast<long long>(B) * ncls * H * W, focal2, st)) return -1;
   (void)launch_k(loss_forward_kernel, dim3(1), dim3(256), 0, st, pred_reg, obj, img, static_cast<const float*>(focal2), c,
-                 out48, ws64);
+                 out48, ws96);
   return check_cuda(cudaGetLastError(), "loss_forward");
 }
 
 int launch_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
                          const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                         const float* ws64, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st) {
+                         const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st) {
   LossCfg c;
   if (fill_cfg(c, weights11, dim_mean9, B, M, H, W, C)) return -1;
   const long long n_reg = static_cast<long long>(B) * C * H * W, n_cls = static_cast<long long>(B) * ncls * H * W;
   if (grad_reg) {
     if (check_cuda(cudaMemsetAsync(grad_reg, 0, n_reg * sizeof(float), st), "loss_backward memset")) return -1;
     const int threads = B * M * 50;
-    (void)launch_k(loss_backward_kernel, dim3((threads + 127) / 128), dim3(128), 0, st, pred_reg, obj, img, ws64,
+    (void)launch_k(loss_backward_kernel, dim3((threads + 127) / 128), dim3(128), 0, st, pred_reg, obj, img, ws96,
                    grad_losses11, c, grad_reg);
     if (check_cuda(cudaGetLastError(), "loss_backward")) return -1;
   }
   if (grad_cls) {
-    float* wsm = const_cast<float*>(ws64);
+    float* wsm = const_cast<float*>(ws96);
     (void)launch_k(loss_hm_scale_kernel, dim3(1), dim3(1), 0, st, wsm, grad_losses11);
-    if (launch_focal_loss_backward(pred_cls, hm, n_cls, ws64 + WS_HMG, grad_cls, st)) return -1;
+    if (launch_focal_loss_backward(pred_cls, hm, n_cls, ws96 + WS_HMG, grad_cls, st)) return -1;
   }
   return 0;
 }

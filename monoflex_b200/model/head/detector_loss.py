@@ -13,6 +13,10 @@ Differences, on purpose:
     for corner_loss, with the clip of csrc/mf_iou3d.cuh (float64 bird's-eye-view clip, the reference's float32 steps); no
     extra launch, no host read. A simple non-convex ring counts as invalid there, valid in shapely (DESIGN.md §9);
     encode_box3d never builds one. Without any labelled object the value is 0, like the other logged means;
+  * a batch without any labelled object (the reference crashes in prepare_predictions) gives 0 for every regression loss
+    and gradient and for the logged means, except the logged keypoint_depth_loss: the mean over no valid key-point-depth
+    group, NaN as in the reference whenever no group is valid; a batch without any 2D box (the reference raises NameError
+    at detector_loss.py:291) gives bbox_loss = 2D_IoU = 0;
   * only the runs/monoflex.yaml loss configuration is built - anything else raises NotImplementedError (no fallback).
 """
 import ctypes
@@ -24,6 +28,7 @@ from ..layers.utils import Converter_key2channel
 
 LOG_KEYS = ['2D_IoU', '3D_IoU', 'depth_loss', 'keypoint_depth_loss', 'depth_MAE', 'center_MAE', '02_MAE', '13_MAE',
             'lower_MAE', 'hard_MAE', 'soft_MAE', 'mean_MAE']                  # the reference's log_loss_dict order
+LOSS_WS_FLOATS = 96                                      # ws96 of mf_loss_forward / mf_loss_backward, include/monoflex_b200.h
 LOG_SLOTS = [0, 11, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10]        # out[16 + slot] of each LOG_KEYS entry, include/monoflex_b200.h
 OBJ_FIELDS = [("cls_ids", 1), ("target_centers", 2), ("2d_bboxes", 4), ("reg_mask", 1), ("trunc_mask", 1), ("dimensions", 3),
               ("locations", 3), ("rotys", 1), ("offset_3D", 2), ("orientations", 8), ("keypoints_depth_mask", 3),
@@ -43,7 +48,7 @@ class _FusedLoss(torch.autograd.Function):
     def forward(ctx, cls, reg, hm, obj, img, owner):
         B, C, H, W = reg.shape
         out = torch.zeros(48, dtype=torch.float32, device=reg.device)
-        ws = torch.zeros(64, dtype=torch.float32, device=reg.device)
+        ws = torch.zeros(LOSS_WS_FLOATS, dtype=torch.float32, device=reg.device)
         st = torch.cuda.current_stream().cuda_stream
         call("mf_loss_forward", cls.data_ptr(), hm.data_ptr(), reg.data_ptr(), obj.data_ptr(), img.data_ptr(),
              ctypes.addressof(owner._w11), ctypes.addressof(owner._dm9), B, cls.shape[1], owner.max_objs, H, W, C,

@@ -76,7 +76,7 @@ def bench_loss(iters, lib_path, dump):
     hm, obj, img = lc.prepare_targets([t.to("cuda") for t in syn.make_train_param_lists(fields)], torch.device("cuda"))
     cls, reg = cls.cuda().contiguous(), reg.cuda().contiguous()
     out = torch.zeros(48, dtype=torch.float32, device="cuda")
-    ws = torch.zeros(64, dtype=torch.float32, device="cuda")
+    ws = torch.zeros(96, dtype=torch.float32, device="cuda")        # ws96
     st = torch.cuda.current_stream().cuda_stream
     _, C, H, W = reg.shape
 
