@@ -277,6 +277,10 @@ int mf_bn_sync_backward_apply(const void* x, int x_ld, const void* dy, int dy_ld
 /* diagnostics: D[128,128] = A^T B with A [64,128] and B [64,128] fp16 row-major (reduction index = rows), computed with
  * MN-major wgmma operand descriptors - the operand form the weight-gradient GEMM of the training path needs */
 int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* stream);
+/* diagnostics: K-major SWIZZLE_128B A descriptors started s = 0..7 rows past a swizzle atom, as the offset/mask convolution
+ * uses them: a_rows [80,64], b_rows [32,64] fp16 row-major; d [2][8][64][32] fp32 = A[s .. s + 63] B^T with the matrix
+ * base-offset field 0 (first half) or (start >> 7) & 7 (second half) */
+int mf_selftest_sw128_shift(const void* a_rows, const void* b_rows, float* d, void* stream);
 
 /* Loss_Computation.__call__ (model/head/detector_loss.py:267-493, prepare_predictions :116-265, Real_MultiBin_loss
  * :495-517, IOULoss layers/iou_loss.py:12-49, decoders model/anno_encoder.py:88-295) for the runs/monoflex.yaml losses.

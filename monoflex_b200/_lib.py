@@ -70,6 +70,7 @@ SIGNATURES = {
     "mf_bn_sync_backward_stats": [_P, _I, _P, _I, _P, _I, _LL, _I, _P, _P, _I, _P, _P, _P, _P, _P],
     "mf_bn_sync_backward_apply": [_P, _I, _P, _I, _P, _I, _LL, _I, _P, _P, _P, _P, ctypes.c_double, _I, _P, _I, _P, _I, _P, _P],
     "mf_selftest_mn_major": [_P, _P, _P, _P],
+    "mf_selftest_sw128_shift": [_P, _P, _P, _P],
     "mf_loss_obj_cols": [],
     "mf_loss_forward": [_P] * 7 + [_I] * 6 + [_P, _P, _P],
     "mf_loss_backward": [_P] * 7 + [_I] * 6 + [_P, _P, _P, _P, _P],

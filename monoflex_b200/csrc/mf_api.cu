@@ -105,6 +105,17 @@ int igemm_block_n(int cout) {
   return 128;
 }
 
+// ACT_OFFMASK = the DCN offset/mask convolution, which has one kernel (mf_offset_conv.cu): 3x3, stride 1, pad 1,
+// Cin % 64 == 0, no residual, fp32 NHWC rows
+static bool offset_conv_shape(const IgemmParams& p) {
+  if (p.out_mode == OUT_F32_NHWC && p.kh == 3 && p.kw == 3 && p.stride == 1 && p.pad == 1 && p.Cin % 64 == 0 &&
+      p.res == nullptr)
+    return true;
+  set_error("offset/mask conv (ACT_OFFMASK): only 3x3 stride 1 pad 1, Cin %% 64 == 0, fp32 NHWC rows, no residual "
+            "(got %dx%d stride %d pad %d Cin %d out_mode %d)", p.kh, p.kw, p.stride, p.pad, p.Cin, p.out_mode);
+  return false;
+}
+
 static int run_gemm(const IgemmParams& p, const void* wp, int n_pad, int k_pad, int mode, cudaStream_t st) {
   if (g_conv_impl == 1) return launch_simt_gemm(p, static_cast<const __half*>(wp), n_pad, k_pad, mode, st);
   return launch_igemm2(p, static_cast<const __half*>(wp), n_pad, k_pad, mode, st);
@@ -156,6 +167,11 @@ int mf_conv2d_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, co
   p.Cout = Cout; p.scale = scale; p.shift = shift;
   p.res = static_cast<const __half*>(res); p.res_ld = res_ld; p.act = act; p.out_mode = out_mode; p.y = y; p.y_ld = y_ld;
   if (p.Ho <= 0 || p.Wo <= 0 || Cout <= 0) { set_error("mf_conv2d_nhwc_f16: empty output"); return -1; }
+  if (act == ACT_OFFMASK && g_conv_impl == 0) {
+    if (!offset_conv_shape(p)) return -1;
+    return launch_offset_conv(p.x, x_ld, 0, B, H, W, Cin, static_cast<const __half*>(w_packed), n_pad, k_pad, scale, shift,
+                              static_cast<float*>(y), y_ld, false, MF_STREAM(stream));
+  }
   return run_gemm(p, w_packed, n_pad, k_pad, MODE_CONV, MF_STREAM(stream));
 }
 
@@ -184,6 +200,12 @@ int mf_conv2d_nhwc_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W,
   p.res = static_cast<const __half*>(res); p.res_ld = res_ld; p.act = act; p.out_mode = out_mode; p.y = y; p.y_ld = y_ld;
   if (p.Ho <= 0 || p.Wo <= 0 || Cout <= 0) { set_error("mf_conv2d_nhwc_f16x2: empty output"); return -1; }
   if (g_conv_impl == 1) { set_error("mf_conv2d_nhwc_f16x2: no CUDA-core cross-check of the split path"); return -1; }
+  if (act == ACT_OFFMASK) {
+    if (!offset_conv_shape(p)) return -1;
+    if (p.split_out) { set_error("mf_conv2d_nhwc_f16x2: the offset/mask rows are fp32, not a split output"); return -1; }
+    return launch_offset_conv(p.x, x_ld, x_lo, B, H, W, Cin, static_cast<const __half*>(w_packed), n_pad, k_pad, scale, shift,
+                              static_cast<float*>(y), y_ld, p.split_in != 0, MF_STREAM(stream));
+  }
   return launch_igemm2(p, static_cast<const __half*>(w_packed), n_pad, k_pad, MODE_CONV, MF_STREAM(stream));
 }
 int mf_head_conv_f16x2(const void* x, int x_ld, int x_lo, int B, int H, int W, int Cin, const void* w_packed, int n_pad, int k_pad,
@@ -449,6 +471,9 @@ int mf_bn_sync_backward_apply(const void* x, int x_ld, const void* dy, int dy_ld
 }
 int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* stream) {
   return launch_mn_major_selftest(static_cast<const __half*>(a_km), static_cast<const __half*>(b_kn), d_mn, MF_STREAM(stream));
+}
+int mf_selftest_sw128_shift(const void* a_rows, const void* b_rows, float* d, void* stream) {
+  return launch_sw128_shift_selftest(static_cast<const __half*>(a_rows), static_cast<const __half*>(b_rows), d, MF_STREAM(stream));
 }
 int mf_loss_obj_cols(void) { return MF_LOSS_OBJ_COLS; }
 int mf_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,

@@ -104,16 +104,13 @@ __host__ __device__ constexpr int igemm2_warps(int mode, int npw, int epi) {
 }
 
 template <int N>
-MF_DEVINL void act_chunk(float (&v)[N], int act, int nb) {
+MF_DEVINL void act_chunk(float (&v)[N], int act) {
   if (act == ACT_RELU) {
 #pragma unroll
     for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.f);
   } else if (act == ACT_LEAKY) {
 #pragma unroll
     for (int i = 0; i < N; ++i) v[i] = fmaxf(v[i], 0.01f * v[i]);      // == v > 0 ? v : 0.01 v
-  } else if (act == ACT_OFFMASK) {
-#pragma unroll
-    for (int i = 0; i < N; ++i) v[i] = (nb + i >= 18) ? 1.f / (1.f + __expf(-v[i])) : v[i];
   }
 }
 
@@ -267,7 +264,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
             }
           }
         }
-        act_chunk<CHUNK>(v, p.act, nb);
+        act_chunk<CHUNK>(v, p.act);
         if (p.out_mode == OUT_F16_NHWC) {
           if (staged) {
             if constexpr (BLOCK_N >= 64) {
@@ -835,7 +832,7 @@ igemm2_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant_
                   // zeroed, they need no registers through the rest of the epilogue (see HEAD2)
                   dh[4 * j + 2 * h] = 0.f;
                   dh[4 * j + 2 * h + 1] = 0.f;
-                  act_chunk<2>(v, p.act, nb);
+                  act_chunk<2>(v, p.act);
                   store(row, j, nb, v);
                 }
               }
@@ -1023,6 +1020,7 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
   // HEAD2 tiles: 128 columns (a 256-column tile would need 128 accumulator registers per consumer thread)
   const int bn = p.h2_w != nullptr ? 128 : igemm_block_n(p.Cout);
   const bool store_ok = p.out_mode == OUT_F16_NHWC && bn >= 64 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0 && p.y_ld % 8 == 0;
+  if (p.act == ACT_OFFMASK) { set_error("igemm2: the offset/mask convolution runs in mf_offset_conv.cu"); return -1; }
   if (n_pad % bn != 0 || k_pad % BK != 0 || k_pad < p.nkb * BK) {
     set_error("igemm: packed weight shape [%d,%d] incompatible with block_n=%d nkb=%d", n_pad, k_pad, bn, p.nkb);
     return -1;

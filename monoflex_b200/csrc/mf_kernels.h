@@ -75,6 +75,8 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
                       const unsigned char* hid_mask, cudaStream_t st);
 int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* dy, int dy_ld, int Cout, int kh,
                       int kw, int stride, int pad_h, int pad_w, float* dw, cudaStream_t st);
+int launch_offset_conv(const __half* x, int x_ld, int x_lo, int B, int H, int W, int Cin, const __half* wp, int n_pad, int k_pad,
+                       const float* scale, const float* shift, float* y, int y_ld, bool pair, cudaStream_t st);
 int launch_simt_gemm(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, int mode, cudaStream_t st);
 
 }  // namespace mf

@@ -29,6 +29,7 @@ int launch_loss_backward(const float* pred_cls, const float* hm, const float* pr
                          const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
                          const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st);
 int launch_mn_major_selftest(const __half* a_km, const __half* b_kn, float* d_mn, cudaStream_t st);
+int launch_sw128_shift_selftest(const __half* a_rows, const __half* b_rows, float* d, cudaStream_t st);
 int launch_maxpool2_bwd(const __half* x, const __half* dy, __half* dx, int B, int H, int W, int C, int x_ld, int dy_ld,
                         int dx_ld, cudaStream_t st);
 size_t upsample_bwd_workspace_floats(int B, int Hi, int Wi, int C, int f);

@@ -4,7 +4,8 @@ Plan.run, median of 20 after 3 warm-ups), the two launches separately (Plan.run_
 layers of that shape in the backbone and the fused DCN's algorithmic TFLOP/s (2 x pixels x Cout x 9 Cin); then one line
 with the layer-weighted totals and the share of the 64-column-tile (Cout <= 64) layers.
 
-Offsets come from a random offset conv scaled so the rms offset is about 1.5 px, as in the calibrated synthetic weights."""
+Offsets come from a random offset conv scaled so the rms offset is about 1.5 px, as in the calibrated synthetic weights.
+Each line also gives the offset conv's L2 -> SM bytes, computed from the shape (offset_conv_traffic)."""
 import json
 import os
 import sys
@@ -65,6 +66,39 @@ class _BN(object):
         self.eps = 1e-5
 
 
+def offset_conv_traffic(B, cin, H, W, pair, nsm=132):
+    """L2 -> SM bytes of one offset/mask conv (csrc/mf_offset_conv.cu): the tile launch_offset_conv picks (the same search and
+    cost estimate, restated), its input boxes per (tile, chunk, hi | lo) and the weight boxes (once per CTA when resident,
+    per tile and chunk otherwise). Returns (bytes, (R, S, resident))."""
+    nch, nhl, w_stage, smem_max = cin // 64, 2 if pair else 1, 3 * (64 if pair else 32) * 128, 232448
+    best = None
+    for nseg in range(1, W + 1):
+        S = (W + nseg - 1) // nseg
+        if nseg > 1 and S < 8:
+            break
+        if S + 2 > 256 or (W + S - 1) // S != nseg:
+            continue
+        P = S + 2
+        for R in range(1, min(H, 254) + 1):
+            nblk = (R * P - 2 + 127) // 128 * 2
+            if nblk > 8:
+                break
+            a_half = ((nblk * 64 + 2 * P + 2) * 128 + 1023) & ~1023
+            res = 3 * nch <= 24 and 3 * nch * w_stage + 2 * nhl * a_half + 2048 <= smem_max
+            nas = min(4, (smem_max - 2048 - (3 * nch if res else 3) * w_stage) // (nhl * a_half))
+            if nas < 2:
+                continue
+            ntiles = B * ((H + R - 1) // R) * nseg
+            mma = nch * nblk * 36.0 * (26.2 if pair else 8.7)
+            load = nch * (nhl * (R + 2.0) * P * 128 + (0.0 if res else 3.0 * w_stage)) / 30.0
+            cost = -(-ntiles // nsm) * (max(mma, load) + 300.0)
+            if best is None or cost < best[0]:
+                a = ntiles * nch * nhl * (R + 2) * P * 128
+                w = (min(ntiles, nsm) if res else ntiles) * nch * 3 * w_stage
+                best = (cost, a + w, (R, S, res))
+    return best[1], best[2]
+
+
 def time_plan(P, n=20, warm=3):
     for _ in range(warm):
         P.run()
@@ -110,8 +144,10 @@ def main():
             total[prec] += n * ms
             if cout <= 64:
                 narrow[prec] += n * ms
+            l2_bytes, tile = offset_conv_traffic(B, cin, H, W, prec == "strict")
             print(json.dumps({"shape": [B, cin, cout, H, W], "precision": prec, "layers": n, "plan_ms": ms,
-                              "offset_conv_ms": off_ms, "dcn_ms": dcn_ms,
+                              "offset_conv_ms": off_ms, "offset_conv_l2_MB": l2_bytes / 1e6, "offset_conv_tile": tile,
+                              "dcn_ms": dcn_ms,
                               "dcn_TFLOPs": 2.0 * B * H * W * cout * 9 * cin / dcn_ms / 1e9}), flush=True)
             del P, xa, x
             torch.cuda.empty_cache()
