@@ -418,8 +418,9 @@ int mf_nms_hm(const float* heat, float* out, int planes, int H, int W, void* str
 /* nms_hm + select_topk + select_point_of_interest + PostProcessor decode (model/layers/utils.py:45-145,
  * model/head/detector_infer.py:77-237, model/anno_encoder.py:69-295) for a whole batch.
  * heat [B,C,H,W] fp32 (apply_sigmoid=1: raw logits), reg [B,R=50,H,W] fp32, calib [B,6] = f_u,f_v,c_u,c_v,b_x,b_y,
- * pad [B,2], size [B,2] = (W,H) of the padded image, dim_mean [C,3]. Workspaces ws_score/ws_idx: [B*C*K*8]
- * (stage 1 runs 8 CTAs per (image, class) plane; stage 2 merges their candidates).
+ * pad [B,2], size [B,2] = (W,H) of the padded image, dim_mean [C,3], 1 <= K <= min(64, H*W), H*W <= 32768, C <= 3.
+ * Workspaces ws_score/ws_idx: [B*C*K*8] (stage 1 runs up to 8 CTAs per (image, class) plane; stage 2 merges their
+ * candidates).
  * depth_mode selects the OUTPUT_DEPTH estimator (detector_infer.py:148-209): 0 soft, 1 hard, 2 mean, 3 oracle, 4 direct,
  * 5 keypoints_avg, 6 keypoints_center, 7 keypoints_02, 8 keypoints_13. The oracle matches every detection against its
  * own image's ground truth gt [B,G,7] = (valid, class, x1, y1, x2, y2, z); gt may be NULL for the other modes.

@@ -2,9 +2,9 @@
 // model/anno_encoder.py:69-295). Integer outputs (indices, classes) are bit-exact against the oracle; the tie rule is
 // (score desc, flat index asc) at both selection stages (torch.topk leaves ties unspecified, SURVEY H5).
 //
-// Stage 1: one CTA per (image, class). Each thread keeps its pixels' 47-bit keys (score bits << 15 | (32767-idx)) in
-//          registers; an MSB-first 8-bit radix select with a shared-memory histogram finds the K-th largest key exactly
-//          (keys are unique), the K survivors are compacted and bitonic-sorted. The 3x3 local-max test reads the logits'
+// Stage 1: S CTAs per (image, class). Each thread keeps its pixels' 48-bit keys (ordered score bits << 15 | (32767-idx))
+//          in shared memory; an MSB-first 8-bit radix select with a shared-memory histogram finds the K-th largest key
+//          exactly (keys are unique), the K survivors are compacted and bitonic-sorted. The 3x3 local-max test reads the logits'
 //          neighbourhood straight from global memory (L1/L2 resident), so the heat map is read from HBM once.
 // Stage 2: one CTA per image merges C*K candidates, gathers the 50 regression channels of each survivor and decodes.
 #include "mf_common.cuh"
@@ -17,6 +17,17 @@ namespace mf {
 #define MF_DECODE_SLABS 8
 static constexpr int S1_THREADS = 1024;
 static constexpr int S1_CAND = 2048;                   // candidate-list capacity of the rank-by-counting fast path (16 KB)
+
+// Scores enter both selection stages as order-preserving unsigned keys: flipping the sign bit of a non-negative float and
+// every bit of a negative one makes unsigned order equal float order, so a signed map ranks like torch.topk (negatives
+// last). -0 is keyed as +0, so they tie and the index decides. Zero keys to 0x80000000, every strictly positive score
+// above it.
+static constexpr unsigned int KEY_ZERO = 0x80000000u;
+__device__ __forceinline__ unsigned int score_key(float s) {
+  const unsigned int u = __float_as_uint(s) == KEY_ZERO ? 0u : __float_as_uint(s);
+  return (u & KEY_ZERO) ? ~u : (u | KEY_ZERO);
+}
+__device__ __forceinline__ float key_score(unsigned int k) { return __uint_as_float((k & KEY_ZERO) ? (k & ~KEY_ZERO) : ~k); }
 
 // hm: [B, C, H, W] fp32 (already sigmoid-ed when apply_sigmoid == 0). out_*: [B, C, K]
 __global__ void __launch_bounds__(S1_THREADS)
@@ -33,20 +44,20 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
   __shared__ unsigned long long sel[256];
   __shared__ unsigned long long s_prefix;
   __shared__ int s_remaining, s_count;
-  // Fast path (round 2): after the 3x3 NMS only the local maxima are non-zero (~1/9 of the pixels), so the slab's non-zero keys are
-  // compacted into `cand` and every candidate computes its RANK by counting the larger keys (keys are unique; all threads read
+  // Fast path (round 2): after the 3x3 NMS only the local maxima are non-zero (~1/9 of the pixels), so the slab's strictly
+  // positive keys are compacted into `cand` and every candidate computes its RANK by counting the larger keys (keys are unique; all threads read
   // the same shared-memory word per iteration = broadcast, no barriers inside): O(n^2 / threads) comparisons instead of six
   // radix passes with three block-wide barriers each plus a 36-step bitonic sort. The exact radix path below remains the
-  // fallback for degenerate maps (fewer non-zero maxima than K - zero-score pixels then enter by index order - or plateaus
-  // with more than S1_CAND candidates).
+  // fallback for degenerate maps (fewer positive maxima than K - zero-score pixels, then negative maxima, enter after
+  // them - or plateaus with more than S1_CAND candidates).
   __shared__ unsigned long long cand[S1_CAND];
   __shared__ int s_ncand;
   if (threadIdx.x == 0) s_ncand = 0;
   __syncthreads();
 
-  // per-thread score bits; the pixel index of item `it` is implicit (it*S1_THREADS + tid), the 47-bit key is rebuilt
-  // on the fly: key = ((bits << 15) | (32767 - idx)) + 1   (0 = "no pixel")
-  extern __shared__ unsigned int vbits_sm[];      // [S1_ITEMS][S1_THREADS] score bits (dynamic smem, <= 128 KB)
+  // per-thread score keys (score_key); the pixel index of item `it` is implicit (it*S1_THREADS + tid), the 48-bit key is
+  // rebuilt on the fly: key = ((score_key << 15) | (32767 - idx)) + 1   (0 = "no pixel")
+  extern __shared__ unsigned int vbits_sm[];      // [S1_ITEMS][S1_THREADS] score keys (dynamic smem, <= 128 KB)
   unsigned int* vbits = vbits_sm + threadIdx.x;   // item `it` of this thread lives at vbits[it * S1_THREADS]
   const int n_items = (hi - lo + S1_THREADS - 1) / S1_THREADS;
   // The slab and its one-row halo are staged in shared memory first: coalesced, independent loads (6 per thread) instead of
@@ -85,13 +96,12 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
           mx = fmaxf(mx, tile[yy * W + xx - t_lo]);
         }
       }
-      const float kept = (mx == v) ? v : 0.f;         // heat * (hmax == heat)
-      key = __float_as_uint(kept);
+      key = score_key((mx == v) ? v : 0.f);           // heat * (hmax == heat)
     }
     vbits[it * S1_THREADS] = key;
-    my_cnt += key != 0u ? 1 : 0;
+    my_cnt += key > KEY_ZERO ? 1 : 0;
   }
-  // append the non-zero keys to the candidate list: ONE shared-memory atomic per warp (the per-item form issued 32 warps x 5
+  // append the strictly positive keys to the candidate list: ONE shared-memory atomic per warp (the per-item form issued 32 warps x 5
   // items = 160 serialised read-modify-writes on one address), then a second pass over the thread's own score bits
   {
     const int lane = threadIdx.x & 31;
@@ -108,7 +118,7 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
     int slot = base + incl - my_cnt;
     for (int it = 0; it < n_items; ++it) {
       const unsigned int key = vbits[it * S1_THREADS];
-      if (key != 0u) {
+      if (key > KEY_ZERO) {
         const int idx = lo + it * S1_THREADS + threadIdx.x;
         if (slot < S1_CAND) cand[slot] = ((static_cast<unsigned long long>(key) << 15) | static_cast<unsigned long long>(32767 - idx)) + 1ull;
         ++slot;
@@ -125,7 +135,7 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
       for (int j = 0; j < ncand; ++j) rank += cand[j] > mine ? 1 : 0;
       if (rank < K) {
         const unsigned long long k = mine - 1ull;
-        out_score[static_cast<long long>(blockIdx.x) * K + rank] = __uint_as_float(static_cast<unsigned int>(k >> 15));
+        out_score[static_cast<long long>(blockIdx.x) * K + rank] = key_score(static_cast<unsigned int>(k >> 15));
         out_idx[static_cast<long long>(blockIdx.x) * K + rank] = 32767 - static_cast<int>(k & 32767ull);
       }
     }
@@ -212,7 +222,7 @@ nms_topk_stage1_kernel(const float* __restrict__ hm_all, int H, int W, int K, in
   if (threadIdx.x < K) {
     const bool have = threadIdx.x < k_eff;
     const unsigned long long k = have ? sel[threadIdx.x] - 1ull : 0ull;
-    out_score[static_cast<long long>(blockIdx.x) * K + threadIdx.x] = have ? __uint_as_float(static_cast<unsigned int>(k >> 15)) : 0.f;
+    out_score[static_cast<long long>(blockIdx.x) * K + threadIdx.x] = have ? key_score(static_cast<unsigned int>(k >> 15)) : 0.f;
     out_idx[static_cast<long long>(blockIdx.x) * K + threadIdx.x] = have ? 32767 - static_cast<int>(k & 32767ull) : -1;
   }
 }
@@ -232,7 +242,7 @@ __global__ void nms_hm_kernel(const float* __restrict__ hm, float* __restrict__ 
       const int yy = y + dy, xx = x + dx;
       if (yy >= 0 && yy < H && xx >= 0 && xx < W) mx = fmaxf(mx, p[yy * W + xx]);
     }
-  out[i] = (mx == v) ? v : 0.f;
+  out[i] = (mx == v) ? v : v * 0.f;                   // heat * 0 keeps the sign of a negative pixel, like the reference
 }
 int launch_nms_hm(const float* hm, float* out, int planes, int H, int W, cudaStream_t st) {
   const long long n = static_cast<long long>(planes) * H * W;
@@ -318,7 +328,7 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   const int SK = p.S * p.K, CSK = p.C * SK;     // candidates per class / per image (<= 2048)
   __shared__ unsigned long long sel[S2_KEYS];
   __shared__ float s_poi[64 * 50];
-  // key = score bits << 17 | (3 - class) << 15 | (32767 - pixel index): (score desc, class asc, index asc) is exactly the
+  // key = score_key << 17 | (3 - class) << 15 | (32767 - pixel index): (score desc, class asc, index asc) is exactly the
   // order of the reference's two-stage top-k (per class, then over the concatenated [class][rank] list, utils.py:61-100)
   for (int i = threadIdx.x; i < S2_KEYS; i += S2_THREADS) {
     unsigned long long key = 0ull;
@@ -327,7 +337,7 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
       if (idx >= 0) {
         const float sc = p.s1_score[static_cast<long long>(b) * CSK + i];
         const int c = i / SK;
-        key = ((static_cast<unsigned long long>(__float_as_uint(sc)) << 17) | (static_cast<unsigned long long>(3 - c) << 15) |
+        key = ((static_cast<unsigned long long>(score_key(sc)) << 17) | (static_cast<unsigned long long>(3 - c) << 15) |
                static_cast<unsigned long long>(32767 - idx)) + 1ull;
       }
     }
@@ -377,7 +387,7 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   if (threadIdx.x == 0) {
     int n = 0;
     for (int d = 0; d < p.K; ++d) {
-      const float sc = __uint_as_float(static_cast<unsigned int>((sel[d] - 1ull) >> 17));
+      const float sc = key_score(static_cast<unsigned int>((sel[d] - 1ull) >> 17));
       if (sc >= p.thresh) ++n;
     }
     p.count[b] = n;
@@ -385,7 +395,7 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   const int d = threadIdx.x;
   if (d >= p.K) return;
   const unsigned long long k = sel[d] - 1ull;
-  const float score = __uint_as_float(static_cast<unsigned int>(k >> 17));
+  const float score = key_score(static_cast<unsigned int>(k >> 17));
   const int cls = 3 - static_cast<int>((k >> 15) & 3ull);
   const int idx = 32767 - static_cast<int>(k & 32767ull);
   const float yf = static_cast<float>(idx / p.W), xf = static_cast<float>(idx % p.W);
@@ -510,7 +520,12 @@ int launch_decode(const float* heat, const float* reg, const float* calib, const
     set_error("decode: the oracle depth needs the ground-truth table gt [B, G, 7] (gt=%p, G=%d)", static_cast<const void*>(gt), G);
     return -1;
   }
-  // score bits of the slab's pixels + the staged slab with its one-row halo
+  // torch.topk raises for K > H*W; here the empty slots would decode as rows with a NaN score
+  if (K < 1 || K > 64 || K > H * W) {
+    set_error("decode: K=%d must be in 1..64 and at most H*W=%d (the top-K of each %dx%d class plane)", K, H * W, H, W);
+    return -1;
+  }
+  // score keys of the slab's pixels + the staged slab with its one-row halo
   auto smem_for = [&](int s) {
     const int items = ((H * W + s - 1) / s + S1_THREADS - 1) / S1_THREADS;
     return items * S1_THREADS * static_cast<int>(sizeof(unsigned int)) + ((H * W + s - 1) / s + 2 * W + 2) * static_cast<int>(sizeof(float));
