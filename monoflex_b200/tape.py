@@ -120,9 +120,12 @@ def predictor_backward(pred, plan, grad_cls, grad_reg):
 
 
 @torch.no_grad()
-def backbone_backward(backbone, plan, d_feat_rows):
+def backbone_backward(backbone, plan, d_feat_rows, observe=None):
     """backbone: DLASeg in train mode, plan: its last train-mode plan (backbone.last_plan), d_feat_rows [B*H/4*W/4, 64] fp16:
-    (scaled) gradient of the loss w.r.t. the backbone's output feature map. Returns grads."""
+    (scaled) gradient of the loss w.r.t. the backbone's output feature map. Returns grads.
+    observe: optional observe(rec, grad, done), called before (done=False) and after (done=True) each tape record is
+    replayed, with `grad` the accessor below (activation -> engine.Act over its gradient buffer). It exists for the
+    layer-by-layer test (tests/test_gpu_tape_layers.py), which checks every record on the inputs it actually saw."""
     grads, put = _collector(backbone)
     bufs = {}
 
@@ -135,6 +138,8 @@ def backbone_backward(backbone, plan, d_feat_rows):
 
     backward.add_rows(grad(plan.output), d_feat_rows.contiguous())
     for rec in reversed(plan.tape):
+        if observe is not None:
+            observe(rec, grad, False)
         kind, x, y = rec["kind"], rec["x"], rec["y"]
         if kind == "conv_bn":
             raw, residual = rec["raw"], rec["residual"]
@@ -168,4 +173,6 @@ def backbone_backward(backbone, plan, d_feat_rows):
             put(rec["weight"], dw.t().contiguous())
         else:
             raise NotImplementedError("tape record %r" % kind)
+        if observe is not None:
+            observe(rec, grad, True)
     return grads
