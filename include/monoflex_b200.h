@@ -313,65 +313,53 @@ int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_r
  * pair; N = 0 launches nothing. */
 int mf_iou3d_corners(const float* pred, const float* target, long long n, float* out, void* stream);
 
-/* torch.optim.AdamW as configured by solver/__init__.py:10-37 (one param group per tensor, lr x BIAS_LR_FACTOR for
- * "bias" tensors, betas (0.9, 0.99), weight decay 1e-5) over ONE flat fp32 arena: every tensor starts at a multiple of
- * mf_adamw_chunk() elements and chunk_lr[n_chunks] (device) holds its group's lr (0 = padding / frozen). step is the
- * 1-based update count; grads are multiplied by grad_scale first (1/world_size after an NCCL SUM of the arena);
- * lr_scale is the scheduler's multiplier (solver/__init__.py:64-92). One launch, 28 B per parameter. */
+/* The optimisers of solver/__init__.py:10-62 run over ONE flat fp32 arena: every tensor starts at a multiple of
+ * mf_adamw_chunk() elements and chunk_lr[n_chunks] (device) holds its param group's lr (one group per tensor, lr x
+ * BIAS_LR_FACTOR for "bias" tensors; 0 = padding / frozen). */
 int mf_adamw_chunk(void);
-/* CUDA-graph-safe AdamW step with a finite guard (the reference's optimizer.step(), engine/trainer.py:121, for a training
- * step captured in one graph): the 1-based step count lives in device memory (state4[0]) instead of being a host scalar;
- * with check_finite the gradient arena is scanned first and a non-finite gradient SKIPS the update (state4[2] counts the
- * skipped steps) instead of being written into params / exp_avg / exp_avg_sq. state4: long long[4] zero-initialised by the
- * caller; dyn16: 16 bytes of device scratch. Three launches: scan, 1-thread prepare (bias corrections in double), update. */
-int mf_adamw_step_dyn(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                      long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
-                      float lr_scale, long long* state4, void* dyn16, int check_finite, void* stream);
-/* mf_adamw_step_dyn with torch.nn.utils.clip_grad_norm_(params, max_norm) in front of the update (the reference's
+/* The optimiser step (the reference's optimizer.step(), engine/trainer.py:121), CUDA-graph-safe so a whole training step
+ * can be captured in one graph: the 1-based step count lives in device memory (state4[0]) instead of being a host scalar,
+ * and the hyper-parameters a schedule moves every step are read from device memory, so a captured graph follows them:
+ * hyper = device double[4] {lr_mult, beta1, weight_decay, unused}, never NULL, rewritten in place by the host between
+ * launches / replays. The lr of a chunk is chunk_lr * lr_mult; bias correction 1 uses the current beta1 (1 - beta1^step
+ * in double, as torch computes it from the group's betas each step). grads are multiplied by grad_scale first
+ * (1/world_size after an NCCL SUM of the arena). rule:
+ *   MF_OPTIM_ADAMW (0): p <- p * (1 - lr * weight_decay), then Adam (torch.optim.AdamW, 'adamw'; fastai OptimWrapper
+ *                       true_wd + Adam with weight_decay 0, 'adam_onecycle');
+ *   MF_OPTIM_ADAM  (1): torch.optim.Adam: g <- g + weight_decay * p (after clipping), then Adam ('adam').
+ * A chunk with chunk_lr < 0 is decay-only under either rule: p <- p * (1 - |lr| * weight_decay), gradient and moments
+ * unread (a one-cycle grouped tensor whose gradient is None). chunk_lr 0: neither updated nor rewritten.
+ * Finite guard: the gradient arena is scanned first and a non-finite gradient SKIPS the update (state4[2] counts the
+ * skipped steps) instead of being written into params / exp_avg / exp_avg_sq.
+ * max_norm > 0: torch.nn.utils.clip_grad_norm_(params, max_norm) in front of the update (the reference's
  * SOLVER.GRAD_NORM_CLIP, engine/trainer.py:119). The scan launch computes the float64 sum of squares of the gradient arena
  * per CTA into partials (device double[(n_chunks + 1) / 2], scratch); the prepare launch reduces them in a fixed order and
  * writes *total_norm_out (device float) = the 2-norm of grad_scale * grads, the value clip_grad_norm_ returns, and
  * clip_coef = min(reciprocal(total_norm + 1e-6) * max_norm, 1) in torch's float32 steps. The update multiplies the
  * gradient by clip_coef and, when clip_coef != 1, writes it back to grads (the arena keeps its convention: with
- * grad_scale = 1/world it holds the clipped SUM). With check_finite, a total norm that is not finite skips the step
- * (state4[2] += 1; params, moments and grads untouched). Chunks with chunk_lr 0 are neither updated nor rewritten.
- * Deterministic: the partials depend on n_chunks only. max_norm <= 0 is exactly mf_adamw_step_dyn (partials and
- * total_norm_out unused). */
-int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                           long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
-                           float lr_scale, long long* state4, void* dyn16, int check_finite, float max_norm, double* partials,
-                           float* total_norm_out, void* stream);
-/* The guarded (and optionally clipping) step of mf_adamw_step_dyn_clip for the reference's other SOLVER.OPTIMIZER values
- * (solver/__init__.py:27-62), with the hyper-parameters a schedule moves every step read from device memory, so a captured
- * graph follows them: hyper = device double[4] {lr_mult, beta1, weight_decay, unused}, rewritten in place by the host
- * between launches / replays. The lr of a chunk is chunk_lr * lr_mult; bias correction 1 uses the current beta1
- * (1 - beta1^step, as torch's Adam computes it from the group's betas each step). rule:
- *   MF_OPTIM_ADAM  (1): torch.optim.Adam: g <- g + weight_decay * p (after clipping), then Adam ('adam');
- *   MF_OPTIM_ADAMW (0): p <- p * (1 - lr * weight_decay), then Adam (AdamW; fastai OptimWrapper true_wd + Adam with
- *                       weight_decay 0, 'adam_onecycle').
- * A chunk with chunk_lr < 0 is decay-only under either rule: p <- p * (1 - |lr| * weight_decay), gradient and moments
- * unread (a one-cycle grouped tensor whose gradient is None). chunk_lr 0: untouched. Finite guard, clipping (max_norm > 0,
- * partials / total_norm_out as in mf_adamw_step_dyn_clip), state4 and dyn16 as in mf_adamw_step_dyn. */
+ * grad_scale = 1/world it holds the clipped SUM). A total norm that is not finite skips the step (state4[2] += 1; params,
+ * moments and grads untouched). Deterministic: the partials depend on n_chunks only. max_norm <= 0: no clipping, grads
+ * only read, partials and total_norm_out unused (may be NULL).
+ * state4: long long[4] zero-initialised by the caller; dyn16: 16 bytes of device scratch. Three launches: scan, prepare
+ * (bias corrections in double), one update pass of 28 B per parameter (read p, g, m, v; write p, m, v). */
 #define MF_OPTIM_ADAMW 0
 #define MF_OPTIM_ADAM 1
 int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
                       long long n_chunks, const double* hyper, float beta2, float eps, float grad_scale, long long* state4,
-                      void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out, void* stream);
+                      void* dyn16, float max_norm, double* partials, float* total_norm_out, void* stream);
 
 /* DDP gradient all-reduce (tools/plain_train_net.py:100-104) FUSED with the AdamW step for world > 1: one kernel over
  * peer-mapped memory. param_ptrs / grad_ptrs: HOST arrays [world] of device addresses of every rank's parameter / gradient
  * arena as mapped into THIS process (symmetric memory / CUDA IPC); mc_params / mc_grads: NVLS multicast addresses of the
  * same arenas (both 0 = plain NVLink peer loads/stores). Rank r reduces the gradients of its 1/world shard of chunks
  * (multimem.ld_reduce or a fixed-order peer sum), scales by 1/world, updates with ITS shard of exp_avg / exp_avg_sq, and
- * writes the new parameters into all world arenas. The caller brackets the call with two cross-rank barriers (gradients
- * complete everywhere before, parameters visible everywhere after). */
+ * writes the new parameters into all world arenas. step: the 1-based update count; beta1 in double like torch's Python
+ * scalar (the bias correction of mf_optim_step_dyn); the lr of a chunk is chunk_lr * lr_scale. The caller brackets the
+ * call with two cross-rank barriers (gradients complete everywhere before, parameters visible everywhere after). */
 int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
                       unsigned long long mc_params, unsigned long long mc_grads, float* exp_avg, float* exp_avg_sq,
-                      const float* chunk_lr, long long n_chunks, float beta1, float beta2, float eps, float weight_decay,
+                      const float* chunk_lr, long long n_chunks, double beta1, float beta2, float eps, float weight_decay,
                       long long step, float lr_scale, void* stream);
-int mf_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                  long long n_chunks, float beta1, float beta2, float eps, float weight_decay, long long step,
-                  float grad_scale, float lr_scale, void* stream);
 
 /* ---- GPU input pipeline (SURVEY 8f N4). mf_preprocess_images_u8: B uint8 HWC RGB images of individual sizes h x w <= H x W
  * (src_ptrs: DEVICE array of B device pointers; hw4: DEVICE int32 [B][4] = h, w, pad_x, pad_y with pad = (W - w) / 2, (H - h) / 2

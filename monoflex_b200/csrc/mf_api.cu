@@ -489,39 +489,16 @@ int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_r
                               grad_losses11, grad_cls, grad_reg, MF_STREAM(stream));
 }
 int mf_adamw_chunk(void) { return MF_ADAMW_CHUNK; }
-int mf_adamw_step(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                  long long n_chunks, float beta1, float beta2, float eps, float weight_decay, long long step,
-                  float grad_scale, float lr_scale, void* stream) {
-  return launch_adamw_arena(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps, weight_decay, step,
-                            grad_scale, lr_scale, MF_STREAM(stream));
-}
-int mf_adamw_step_dyn(float* params, const float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                      long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
-                      float lr_scale, long long* state4, void* dyn16, int check_finite, void* stream) {
-  // without clipping the gradient arena is only read
-  return launch_adamw_arena_dyn(params, const_cast<float*>(grads), exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps,
-                                weight_decay, grad_scale, lr_scale, state4, dyn16, check_finite, 0.f, nullptr, nullptr,
-                                MF_OPTIM_ADAMW, nullptr, MF_STREAM(stream));
-}
-int mf_adamw_step_dyn_clip(float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
-                           long long n_chunks, float beta1, float beta2, float eps, float weight_decay, float grad_scale,
-                           float lr_scale, long long* state4, void* dyn16, int check_finite, float max_norm, double* partials,
-                           float* total_norm_out, void* stream) {
-  return launch_adamw_arena_dyn(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, beta1, beta2, eps, weight_decay,
-                                grad_scale, lr_scale, state4, dyn16, check_finite, max_norm, partials, total_norm_out,
-                                MF_OPTIM_ADAMW, nullptr, MF_STREAM(stream));
-}
 int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, float* exp_avg_sq, const float* chunk_lr,
                       long long n_chunks, const double* hyper, float beta2, float eps, float grad_scale, long long* state4,
-                      void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out, void* stream) {
-  if (hyper == nullptr) { set_error("optim_step_dyn: hyper (device double[4]) is NULL"); return -1; }
-  return launch_adamw_arena_dyn(params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, 0.f, beta2, eps, 0.f, grad_scale, 1.f,
-                                state4, dyn16, check_finite, max_norm, partials, total_norm_out, rule, hyper,
-                                MF_STREAM(stream));
+                      void* dyn16, float max_norm, double* partials, float* total_norm_out, void* stream) {
+  if (hyper == nullptr) { set_error("mf_optim_step_dyn: hyper (device double[4]) is NULL"); return -1; }
+  return launch_adamw_arena_dyn(rule, params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, hyper, beta2, eps, grad_scale,
+                                state4, dyn16, max_norm, partials, total_norm_out, MF_STREAM(stream));
 }
 int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
                       unsigned long long mc_params, unsigned long long mc_grads, float* exp_avg, float* exp_avg_sq,
-                      const float* chunk_lr, long long n_chunks, float beta1, float beta2, float eps, float weight_decay,
+                      const float* chunk_lr, long long n_chunks, double beta1, float beta2, float eps, float weight_decay,
                       long long step, float lr_scale, void* stream) {
   return launch_adamw_p2p(param_ptrs, grad_ptrs, world, rank, mc_params, mc_grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks,
                           beta1, beta2, eps, weight_decay, step, lr_scale, MF_STREAM(stream));

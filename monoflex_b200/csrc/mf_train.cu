@@ -1,13 +1,13 @@
 // Training-side HBM kernels (SURVEY §8 rows R11 backward, R13).
 //
-//  * adamw_arena_kernel: torch.optim.AdamW over ONE flat parameter / gradient / moment arena. The reference builds one
+//  * adamw_arena_dyn_kernel: torch.optim.AdamW over ONE flat parameter / gradient / moment arena. The reference builds one
 //    param group per tensor (solver/__init__.py:10-24, lr = BASE_LR or BASE_LR * BIAS_LR_FACTOR when "bias" is in the
 //    name) => ~280 groups and ~1000 tiny kernels per step in eager torch; here each tensor is padded to a multiple of
-//    ADAMW_CHUNK elements inside the arena and a per-chunk lr table selects the group's lr, so the whole step is one
+//    ADAMW_CHUNK elements inside the arena and a per-chunk lr table selects the group's lr, so the update is one
 //    launch that streams 28 B/parameter (read p, g, m, v; write p, m, v).
 //    The same update also runs torch.optim.Adam (coupled L2 weight decay, the reference's SOLVER.OPTIMIZER 'adam') and the
-//    fastai one-cycle Adam ('adam_onecycle') through the rule template of adamw_arena_dyn_kernel and a device block of
-//    hyper-parameters (lr multiplier, beta1, weight decay) the host rewrites in place between captured replays.
+//    fastai one-cycle Adam ('adam_onecycle') through its rule template; the hyper-parameters a schedule moves (lr
+//    multiplier, beta1, weight decay) come from a device block the host rewrites in place between captured replays.
 //  * focal_loss_backward_kernel: d/dpred of FocalLoss.forward (model/layers/focal_loss.py:35-55) scaled by a device
 //    scalar (loss weight / clamp(num_pos, 1), detector_loss.py:276).
 #include "mf_common.cuh"
@@ -50,27 +50,6 @@ __device__ __forceinline__ void adamw_update4(float4& pp, const float4& gg, floa
     const float denom = sqrtf(vk) * k.rsqrt_bc2 + k.eps;
     pk -= step * (mk / denom);
     pe[e] = pk; me[e] = mk; ve[e] = vk;
-  }
-}
-
-__global__ void __launch_bounds__(256) adamw_arena_kernel(float* __restrict__ p, const float* __restrict__ g,
-                                                          float* __restrict__ m, float* __restrict__ v,
-                                                          const float* __restrict__ chunk_lr, long long n_chunks,
-                                                          AdamwConsts k) {
-  constexpr int VEC_PER_CHUNK = MF_ADAMW_CHUNK / 4;
-  const long long n_vec = n_chunks * VEC_PER_CHUNK;
-  for (long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x; i < n_vec;
-       i += static_cast<long long>(gridDim.x) * blockDim.x) {
-    const float lr = __ldg(chunk_lr + i / VEC_PER_CHUNK) * k.lr_scale;
-    if (lr == 0.f) continue;                                   // padding-only chunk / frozen tensor
-    float4 pp = reinterpret_cast<float4*>(p)[i];
-    const float4 gg = __ldcs(reinterpret_cast<const float4*>(g) + i);
-    float4 mm = reinterpret_cast<float4*>(m)[i];
-    float4 vv = reinterpret_cast<float4*>(v)[i];
-    adamw_update4(pp, gg, mm, vv, lr, k);
-    reinterpret_cast<float4*>(p)[i] = pp;
-    reinterpret_cast<float4*>(m)[i] = mm;
-    reinterpret_cast<float4*>(v)[i] = vv;
   }
 }
 
@@ -133,13 +112,13 @@ __global__ void __launch_bounds__(256) adamw_p2p_kernel(PeerPtrs peers, int worl
   }
 }
 
-static AdamwConsts adamw_consts(float beta1, float beta2, float eps, float wd, long long step, float grad_scale,
+static AdamwConsts adamw_consts(double beta1, float beta2, float eps, float wd, long long step, float grad_scale,
                                 float lr_scale) {
-  // bias corrections in double like torch's Python scalars
-  const double bc1 = 1.0 - pow(static_cast<double>(beta1), static_cast<double>(step));
+  // bias corrections in double like torch's Python scalars (beta1 is the Python double itself, as in the hyper block)
+  const double bc1 = 1.0 - pow(beta1, static_cast<double>(step));
   const double bc2 = 1.0 - pow(static_cast<double>(beta2), static_cast<double>(step));
   AdamwConsts k;
-  k.beta1 = beta1; k.beta2 = beta2; k.eps = eps; k.wd = wd;
+  k.beta1 = static_cast<float>(beta1); k.beta2 = beta2; k.eps = eps; k.wd = wd;
   k.bc1 = static_cast<float>(bc1); k.rsqrt_bc2 = static_cast<float>(1.0 / sqrt(bc2));
   k.grad_scale = grad_scale; k.lr_scale = lr_scale;
   return k;
@@ -147,7 +126,7 @@ static AdamwConsts adamw_consts(float beta1, float beta2, float eps, float wd, l
 
 int launch_adamw_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
                      unsigned long long mc_params, unsigned long long mc_grads, float* m, float* v, const float* chunk_lr,
-                     long long n_chunks, float beta1, float beta2, float eps, float wd, long long step, float lr_scale,
+                     long long n_chunks, double beta1, float beta2, float eps, float wd, long long step, float lr_scale,
                      cudaStream_t st) {
   if (world < 1 || world > MF_MAX_PEERS || rank < 0 || rank >= world) {
     set_error("adamw_p2p: world %d (max %d) / rank %d", world, MF_MAX_PEERS, rank);
@@ -174,28 +153,17 @@ int launch_adamw_p2p(const unsigned long long* param_ptrs, const unsigned long l
   return check_cuda(cudaGetLastError(), "adamw_p2p");
 }
 
-int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
-                       float beta1, float beta2, float eps, float wd, long long step, float grad_scale, float lr_scale,
-                       cudaStream_t st) {
-  if (n_chunks <= 0) return 0;
-  if (step < 1) { set_error("adamw: step must be >= 1 (1-based count of the update being applied)"); return -1; }
-  const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
-  long long blocks = (n_vec + 255) / 256;
-  const long long cap = 132LL * 8 * 4;                          // a few waves; grid-stride for the rest
-  if (blocks > cap) blocks = cap;
-  (void)launch_k(adamw_arena_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, p, g, m, v, chunk_lr,
-                 n_chunks, adamw_consts(beta1, beta2, eps, wd, step, grad_scale, lr_scale));
-  return check_cuda(cudaGetLastError(), "adamw_arena");
-}
-
-// ---------------------------------------------------------------- CUDA-graph-safe AdamW step with a finite guard
-// `mf_adamw_step` takes the step count (for the bias corrections) as a host scalar, which a captured graph would freeze.
-// Here the count lives on the device and three launches make one optimiser step:
+// ---------------------------------------------------------------- CUDA-graph-safe optimiser step with a finite guard
+// The step count (for the bias corrections) lives on the device, so a captured graph does not freeze it, and the
+// hyper-parameters a schedule moves are read from the device block hyper = double[4] {lr_mult, beta1, weight_decay,
+// unused}, which the host rewrites in place between launches / replays. Three launches make one optimiser step:
 //   1. grad_finite_kernel : state[1] |= any non-finite element in the gradient arena (fp16 gradient flow under a loss
-//                           scale can overflow; one inf written by AdamW poisons params, exp_avg and exp_avg_sq for good);
+//                           scale can overflow; one inf written by the update poisons params, exp_avg and exp_avg_sq for
+//                           good);
 //   2. adamw_prepare_kernel (1 thread): if the flag is clean, step += 1 and the bias corrections of the new step are
-//                           computed in double (torch computes them in Python doubles); else the step is skipped
-//                           (state[2] += 1). Either way it publishes (bc1, rsqrt_bc2, skip) and clears the flag;
+//                           computed in double from beta1 = hyper[1] (torch computes them in Python doubles); else the
+//                           step is skipped (state[2] += 1). Either way it publishes (bc1, rsqrt_bc2, skip) and clears
+//                           the flag;
 //   3. adamw_arena_dyn_kernel: the arena update, reading those three values from device memory.
 // state = long long[4]: [0] step count, [1] found-non-finite flag of the current step, [2] skipped steps, [3] unused.
 //
@@ -213,7 +181,6 @@ int launch_adamw_arena(float* p, const float* g, float* m, float* v, const float
 //                           then the update as above.
 struct AdamwDyn { float bc1, rsqrt_bc2; int skip; float clip_coef; };
 
-// beta1: the kernel argument, or hyper[1] (double) when the step reads the hyper-parameter block
 __device__ __forceinline__ void adamw_prepare_step(long long* state, AdamwDyn* dyn, double beta1, float beta2, bool skip) {
   if (skip) state[2] += 1; else state[0] += 1;
   state[1] = 0;
@@ -252,8 +219,8 @@ __global__ void __launch_bounds__(256) grad_sumsq_kernel(const float* __restrict
   if (threadIdx.x == 0) partials[blockIdx.x] = s;
 }
 
-__global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2,
-                                                                 int check, const double* __restrict__ partials, int n_partials,
+__global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* state, AdamwDyn* dyn, float beta2,
+                                                                 const double* __restrict__ partials, int n_partials,
                                                                  float grad_scale, float max_norm, float* total_norm_out,
                                                                  const double* __restrict__ hyper) {
   __shared__ double red[8];
@@ -263,7 +230,7 @@ __global__ void __launch_bounds__(256) adamw_prepare_clip_kernel(long long* stat
   if (threadIdx.x != 0) return;
   const float norm = static_cast<float>(sqrt(s) * static_cast<double>(grad_scale));
   *total_norm_out = norm;
-  adamw_prepare_step(state, dyn, hyper != nullptr ? hyper[1] : static_cast<double>(beta1), beta2, check != 0 && !isfinite(norm));
+  adamw_prepare_step(state, dyn, hyper[1], beta2, !isfinite(norm));
   const float c = __fmul_rn(__frcp_rn(__fadd_rn(norm, 1e-6f)), max_norm);
   dyn->clip_coef = c > 1.f ? 1.f : c;                          // torch.clamp(max=1.0) keeps a NaN
 }
@@ -279,16 +246,15 @@ __global__ void __launch_bounds__(256) grad_finite_kernel(const float* __restric
   }
   if (__syncthreads_or(bad ? 1 : 0) && threadIdx.x == 0) atomicExch(reinterpret_cast<unsigned long long*>(state + 1), 1ull);
 }
-__global__ void adamw_prepare_kernel(long long* state, AdamwDyn* dyn, float beta1, float beta2, int check,
-                                     const double* __restrict__ hyper) {
+__global__ void adamw_prepare_kernel(long long* state, AdamwDyn* dyn, float beta2, const double* __restrict__ hyper) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
-  adamw_prepare_step(state, dyn, hyper != nullptr ? hyper[1] : static_cast<double>(beta1), beta2, check != 0 && state[1] != 0);
+  adamw_prepare_step(state, dyn, hyper[1], beta2, state[1] != 0);
 }
 // CLIP = false never writes g; chunks with lr 0 (padding-only, mark_unused) are neither updated nor clipped.
-// HYPER (mf_optim_step_dyn): lr multiplier, beta1 and weight decay come from the device block hyper = double[4]
-// {lr_mult, beta1, weight_decay, unused}, and a chunk whose lr is negative is decay-only: p <- p * (1 - |lr| * wd), no
-// gradient, no moments (fastai's OptimWrapper decays every grouped tensor, torch's Adam then skips the ones with grad None).
-template <bool CLIP, int RULE, bool HYPER>
+// lr = chunk_lr * hyper[0]; beta1 and weight decay are hyper[1] and hyper[2]. A chunk whose lr is negative is decay-only:
+// p <- p * (1 - |lr| * wd), no gradient, no moments (fastai's OptimWrapper decays every grouped tensor, torch's Adam then
+// skips the ones with grad None).
+template <bool CLIP, int RULE>
 __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict__ p, float* __restrict__ g,
                                                               float* __restrict__ m, float* __restrict__ v,
                                                               const float* __restrict__ chunk_lr, long long n_chunks,
@@ -297,11 +263,9 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
   if (dyn->skip) return;
   k.bc1 = dyn->bc1;
   k.rsqrt_bc2 = dyn->rsqrt_bc2;
-  if (HYPER) {
-    k.lr_scale *= static_cast<float>(hyper[0]);
-    k.beta1 = static_cast<float>(hyper[1]);
-    k.wd = static_cast<float>(hyper[2]);
-  }
+  k.lr_scale = static_cast<float>(hyper[0]);
+  k.beta1 = static_cast<float>(hyper[1]);
+  k.wd = static_cast<float>(hyper[2]);
   const float coef = CLIP ? dyn->clip_coef : 1.f;
   constexpr int VEC_PER_CHUNK = MF_ADAMW_CHUNK / 4;
   const long long n_vec = n_chunks * VEC_PER_CHUNK;
@@ -310,7 +274,7 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
     const float lr = __ldg(chunk_lr + i / VEC_PER_CHUNK) * k.lr_scale;
     if (lr == 0.f) continue;
     float4 pp = reinterpret_cast<float4*>(p)[i];
-    if (HYPER && lr < 0.f) {
+    if (lr < 0.f) {
       const float decay = 1.f - (-lr) * k.wd;
       pp.x *= decay; pp.y *= decay; pp.z *= decay; pp.w *= decay;
       reinterpret_cast<float4*>(p)[i] = pp;
@@ -330,37 +294,29 @@ __global__ void __launch_bounds__(256) adamw_arena_dyn_kernel(float* __restrict_
   }
 }
 template <bool CLIP>
-static void launch_dyn_update(int rule, const double* hyper, dim3 grid, cudaStream_t st, float* p, float* g, float* m,
-                              float* v, const float* chunk_lr, long long n_chunks, const AdamwConsts& k, const AdamwDyn* dyn) {
-  if (hyper == nullptr)
-    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW, false>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
-                   k, dyn, hyper);
-  else if (rule == MF_OPTIM_ADAM)
-    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAM, true>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
-                   k, dyn, hyper);
+static void launch_dyn_update(int rule, dim3 grid, cudaStream_t st, float* p, float* g, float* m, float* v,
+                              const float* chunk_lr, long long n_chunks, const AdamwConsts& k, const AdamwDyn* dyn,
+                              const double* hyper) {
+  if (rule == MF_OPTIM_ADAM)
+    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAM>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k,
+                   dyn, hyper);
   else
-    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW, true>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks,
-                   k, dyn, hyper);
+    (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k,
+                   dyn, hyper);
 }
 // max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL).
-// hyper == NULL: the mf_adamw_step_dyn* semantics (rule must be MF_OPTIM_ADAMW; beta1 / wd / lr_scale from the arguments).
-// hyper != NULL: mf_optim_step_dyn (beta1 and wd arguments ignored, taken from hyper; lr = chunk_lr * lr_scale * hyper[0]).
-int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
-                           float beta1, float beta2, float eps, float wd, float grad_scale, float lr_scale, long long* state4,
-                           void* dyn16, int check_finite, float max_norm, double* partials, float* total_norm_out,
-                           int rule, const double* hyper, cudaStream_t st) {
+// hyper: device double[4] {lr_mult, beta1, weight_decay, unused}, never NULL.
+int launch_adamw_arena_dyn(int rule, float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
+                           const double* hyper, float beta2, float eps, float grad_scale, long long* state4, void* dyn16,
+                           float max_norm, double* partials, float* total_norm_out, cudaStream_t st) {
   if (rule != MF_OPTIM_ADAMW && rule != MF_OPTIM_ADAM) {
-    set_error("optim_step_dyn: rule %d (0 = AdamW, 1 = Adam with L2 weight decay)", rule);
-    return -1;
-  }
-  if (rule != MF_OPTIM_ADAMW && hyper == nullptr) {
-    set_error("optim_step_dyn: the Adam rule reads the hyper-parameter block; hyper is NULL");
+    set_error("mf_optim_step_dyn: rule %d (0 = AdamW, 1 = Adam with L2 weight decay)", rule);
     return -1;
   }
   if (n_chunks <= 0) return 0;
   const bool clip = max_norm > 0.f;
   if (clip && (partials == nullptr || total_norm_out == nullptr)) {
-    set_error("adamw_step_dyn_clip: max_norm > 0 needs the partials buffer and total_norm_out");
+    set_error("mf_optim_step_dyn: max_norm > 0 needs the partials buffer and total_norm_out");
     return -1;
   }
   const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
@@ -370,22 +326,20 @@ int launch_adamw_arena_dyn(float* p, float* g, float* m, float* v, const float* 
   AdamwDyn* dyn = static_cast<AdamwDyn*>(dyn16);
   if (clip) {
     (void)launch_k(grad_sumsq_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, partials);
-    (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta1, beta2, check_finite, partials,
+    (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta2, partials,
                    static_cast<int>(blocks), grad_scale, max_norm, total_norm_out, hyper);
   } else {
-    if (check_finite)
-      (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
-    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta1, beta2, check_finite, hyper);
+    (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
+    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta2, hyper);
   }
-  AdamwConsts k;
-  k.beta1 = beta1; k.beta2 = beta2; k.eps = eps; k.wd = wd; k.bc1 = 1.f; k.rsqrt_bc2 = 1.f;
-  k.grad_scale = grad_scale; k.lr_scale = lr_scale;
+  AdamwConsts k{};                                              // beta1, wd, lr_scale and the bias corrections: on the device
+  k.beta2 = beta2; k.eps = eps; k.grad_scale = grad_scale;
   const dim3 grid(static_cast<unsigned>(blocks));
   if (clip)
-    launch_dyn_update<true>(rule, hyper, grid, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
+    launch_dyn_update<true>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
   else
-    launch_dyn_update<false>(rule, hyper, grid, st, p, g, m, v, chunk_lr, n_chunks, k, static_cast<const AdamwDyn*>(dyn));
-  return check_cuda(cudaGetLastError(), hyper != nullptr ? "optim_step_dyn" : clip ? "adamw_arena_dyn_clip" : "adamw_arena_dyn");
+    launch_dyn_update<false>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
+  return check_cuda(cudaGetLastError(), "mf_optim_step_dyn");
 }
 
 // ---------------------------------------------------------------- focal loss backward (layers/focal_loss.py:35-55)

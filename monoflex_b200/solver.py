@@ -6,18 +6,19 @@ step - and DDP all-reduces 280 gradient tensors (83.8 MB) in its own buckets.
 
 Here every trainable tensor lives in ONE flat fp32 arena (``ParamArena``): ``p.data`` and ``p.grad`` become views of the
 parameter / gradient arenas, each tensor padded to ``mf_adamw_chunk()`` elements so a per-chunk lr table can stand in for
-the param groups. ``FusedAdamW.step()`` is then a single hand-written kernel launch (``mf_adamw_step``, 28 B/parameter),
-``zero_grad()`` one memset and the gradient all-reduce a few large chunk-aligned buckets of the same arena
-(``allreduce_grads``; NCCL SUM, the 1/world_size of the mean is folded into the AdamW kernel's ``grad_scale``).
+the param groups. ``FusedAdamW.step()`` is then one guarded, clipping, CUDA-graph-capturable step (``mf_optim_step_dyn``:
+a finite or sum-of-squares scan of the gradient arena, a one-CTA prepare and one hand-written update pass of
+28 B/parameter), ``zero_grad()`` one memset and the gradient all-reduce a few large chunk-aligned buckets of the same
+arena (``allreduce_grads``; NCCL SUM, the 1/world_size of the mean is folded into the update kernel's ``grad_scale``).
+The step count and the hyper-parameters a schedule moves every step (lr multiplier, beta1, weight decay) live on the
+device, the latter in a small block the host rewrites in place before each launch or graph replay.
 
 ``FusedAdamW`` subclasses ``torch.optim.Optimizer`` so the reference's ``LambdaLR`` / ``CosineWarmupLR`` schedulers and
 ``state_dict()`` checkpointing (utils/check_point.py) keep working: ``param_groups`` has the reference's one-group-per-
 tensor layout and ``state[p]`` exposes ``step / exp_avg / exp_avg_sq`` (views of the moment arenas).
 There is no CPU fallback: ``step()`` raises if the arena is not on a CUDA device.
 
-The reference's other ``SOLVER.OPTIMIZER`` values run on the same arena and the same guarded, clipping, capturable step
-(``mf_optim_step_dyn``: one update pass, 28 B/parameter), with the hyper-parameters a schedule moves every step (lr
-multiplier, beta1, weight decay) in a small device block the host rewrites in place before each launch or graph replay:
+The reference's other ``SOLVER.OPTIMIZER`` values run on the same arena and the same step, with another update rule:
 
 * ``'adam'`` -> ``FusedAdam``: ``torch.optim.Adam`` (coupled L2 weight decay, ``g + wd * p``) over the same groups as
   ``'adamw'``; its ``state_dict`` loads into ``torch.optim.Adam`` and back.
@@ -127,16 +128,23 @@ def allreduce_grads(arena, bucket_bytes=32 << 20, group=None, async_op=False):
 
 class FusedAdamW(torch.optim.Optimizer):
     """torch.optim.AdamW(model_params, lr, betas=(0.9, 0.99), weight_decay) (solver/__init__.py:36-37) with the update of
-    ALL tensors in one kernel launch over a ParamArena."""
+    ALL tensors in one kernel launch over a ParamArena.
 
-    _rule = None            # None: the mf_adamw_step* entry points; MF_OPTIM_* rule of mf_optim_step_dyn in the subclasses
+    `step()` keeps the step count on the device and guards the update with a finite scan of the gradient arena (a
+    non-finite gradient skips the update, `skipped_steps()` counts them), so a whole training step can be captured in one
+    CUDA graph.
+
+    Device hyper-parameter block (`_hyper`, float64 {lr multiplier, beta1, weight decay, 0}): refreshed in place by
+    `_lr_table()`, which `step()` calls and the captured Trainer calls before each replay. When every updated tensor's group
+    has the same lr, the chunk table holds 1 (0 / -1 for skipped / decay-only tensors) and the lr itself is the multiplier,
+    so a schedule that moves one lr for all groups rewrites 8 bytes, not the table."""
+
+    _rule = 0                       # MF_OPTIM_ADAMW: p * (1 - lr * wd), then Adam
+    _unused_decays = False          # mark_unused tensors: skipped entirely (torch's AdamW skips grad None)
 
     def __init__(self, params, lr=3e-4, betas=(0.9, 0.99), eps=1e-8, weight_decay=1e-5, symmetric_group=None,
-                 capturable=True, check_finite=True, outside_params=()):
-        """capturable (default): `step()` keeps the step count on the device and guards the update with a finite scan of the
-        gradient arena (`mf_adamw_step_dyn`: a non-finite gradient skips the update, `skipped_steps()` counts them), so a
-        whole training step can be captured in one CUDA graph; capturable=False is the host-scalar `mf_adamw_step` launch.
-        symmetric_group: a torch.distributed process group (NCCL, one rank per GPU of ONE NVLink domain). When given,
+                 outside_params=()):
+        """symmetric_group: a torch.distributed process group (NCCL, one rank per GPU of ONE NVLink domain). When given,
         the parameter and gradient arenas are allocated in symmetric (peer-mapped) memory and `step_exchange()` replaces
         `allreduce_grads(); step(grad_scale=1/world)` by the fused reduce-scatter + AdamW + all-gather kernel.
         outside_params: trainable tensors in no param group. They get arena storage (so zero_grad, the all-reduce and the
@@ -145,7 +153,6 @@ class FusedAdamW(torch.optim.Optimizer):
         # expects in every param group, so a checkpoint written here loads into the reference's optimiser and vice versa
         super().__init__(params, dict(lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, amsgrad=False, maximize=False,
                                       foreach=None, capturable=False, differentiable=False, fused=None))
-        self.capturable, self.check_finite = bool(capturable), bool(check_finite)
         self.n_grouped = sum(len(g["params"]) for g in self.param_groups)
         tensors = [p for g in self.param_groups for p in g["params"]] + list(outside_params)
         if len({id(p) for p in tensors}) != len(tensors):
@@ -179,7 +186,9 @@ class FusedAdamW(torch.optim.Optimizer):
         dev = self.arena.params.device
         self._state4 = torch.zeros(4, dtype=torch.int64, device=dev)      # [step, found-non-finite, skipped steps, -]
         self._dyn16 = torch.zeros(4, dtype=torch.float32, device=dev)
-        # per-CTA sums of squares of the clipping scan (mf_adamw_step_dyn_clip), allocated once so step() stays capturable
+        self._hyper = torch.zeros(4, dtype=torch.float64, device=dev)
+        self._hyper_key = None
+        # per-CTA sums of squares of the clipping scan, allocated once so step() stays capturable
         self._norm_partials = torch.empty((self.arena.n_chunks + 1) // 2, dtype=torch.float64, device=dev)
         self.last_grad_norm = torch.full((), float("nan"), dtype=torch.float32, device=dev)
         self._bind_state()
@@ -210,6 +219,7 @@ class FusedAdamW(torch.optim.Optimizer):
         self._state4[0] = self.step_count
         self._bind_state()
         self._lr_key = None
+        self._hyper_key = None
 
     def zero_grad(self, set_to_none=False):
         """one memset of the gradient arena; p.grad stays a view of it (set_to_none is ignored on purpose)."""
@@ -219,19 +229,39 @@ class FusedAdamW(torch.optim.Optimizer):
         """the param group of each arena tensor, None for outside_params"""
         return [g for g in self.param_groups for _ in g["params"]] + [None] * (len(self.arena.tensors) - self.n_grouped)
 
-    def _lr_table(self):
-        lrs = tuple(0.0 if (skip or g is None) else g["lr"] for (g, skip) in zip(self._group_of_tensor(), self._skip))
-        self._upload_table(lrs)
-        return self._chunk_lr
+    def _weight_decay(self):
+        wds = {g["weight_decay"] for g in self.param_groups}
+        if len(wds) != 1:
+            raise NotImplementedError("%s: weight_decay must be the same for every group" % type(self).__name__)
+        return float(wds.pop())
 
-    def _upload_table(self, lrs):
-        if lrs != self._lr_key:
-            table = self.arena.chunk_table(lrs).to(self.arena.params.device)
+    def _lr_table(self):
+        groups = self._group_of_tensor()
+        betas = {tuple(g["betas"]) for g in self.param_groups}
+        if len(betas) != 1 or tuple(betas)[0][1] != self.defaults["betas"][1]:
+            raise NotImplementedError("%s: every group needs the same betas, and beta2 stays %r"
+                                      % (type(self).__name__, self.defaults["betas"][1]))
+        beta1 = float(tuple(betas)[0][0])
+        unused = -1.0 if self._unused_decays else 0.0
+        active = {float(g["lr"]) for g, skip in zip(groups, self._skip) if g is not None and (not skip or self._unused_decays)}
+        if len(active) == 1:                  # one shared lr: it goes to the device block, the table holds its sign pattern
+            mult = active.pop()
+            vals = tuple(0.0 if g is None else (unused if skip else 1.0) for g, skip in zip(groups, self._skip))
+        else:
+            mult = 1.0
+            vals = tuple(0.0 if g is None else (unused * g["lr"] if skip else g["lr"]) for g, skip in zip(groups, self._skip))
+        if vals != self._lr_key:
+            table = self.arena.chunk_table(vals).to(self.arena.params.device)
             if self._chunk_lr is None or self._chunk_lr.shape != table.shape:
                 self._chunk_lr = table
             else:
                 self._chunk_lr.copy_(table)               # in place: a captured graph keeps reading the same buffer
-            self._lr_key = lrs
+            self._lr_key = vals
+        key = (mult, beta1, self._weight_decay())
+        if key != self._hyper_key:
+            self._hyper.copy_(torch.tensor(key + (0.0,), dtype=torch.float64))   # in place, like the table
+            self._hyper_key = key
+        return self._chunk_lr
 
     def mark_unused(self, names, model):
         """Parameters the forward never uses (e.g. the outer `project` of DLA's two-level trees, dla_dcn.py:249) get grad None
@@ -261,8 +291,6 @@ class FusedAdamW(torch.optim.Optimizer):
         if not self.arena.params.is_cuda:
             raise RuntimeError("FusedAdamW.step: parameters are not on a CUDA device (there is no CPU path)")
         clip = max_grad_norm is not None and float(max_grad_norm) > 0
-        if clip and not self.capturable:
-            raise NotImplementedError("FusedAdamW.step: max_grad_norm needs the device-side step (capturable=True)")
         from . import _lib
         lib = _lib.load()
         if lib.mf_adamw_chunk() != self.arena.chunk:
@@ -275,39 +303,13 @@ class FusedAdamW(torch.optim.Optimizer):
                                    "(use optimizer.zero_grad(), not set_to_none)")
         table = self._lr_table()
         self.step_count += 1
-        b1, b2 = self.defaults["betas"]
-        if self._rule is not None:
-            if self.step_count == 1 and int(self._state4[0].item()) != 0:
-                raise RuntimeError("%s: device step counter out of sync" % type(self).__name__)
-            _lib.call("mf_optim_step_dyn", self._rule, self.arena.params.data_ptr(), self.arena.grads.data_ptr(),
-                      self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks,
-                      self._hyper.data_ptr(), b2, self.defaults["eps"], float(grad_scale), self._state4.data_ptr(),
-                      self._dyn16.data_ptr(), 1 if self.check_finite else 0, float(max_grad_norm) if clip else 0.0,
-                      self._norm_partials.data_ptr(), self.last_grad_norm.data_ptr(), torch.cuda.current_stream().cuda_stream)
-            self._step_t += 1
-            for p in self.arena.tensors:
-                torch.autograd.graph.increment_version(p)
-            return None
-        if self.capturable:
-            if self.step_count == 1 and int(self._state4[0].item()) != 0:
-                raise RuntimeError("FusedAdamW: device step counter out of sync")
-            args = (self.arena.params.data_ptr(), self.arena.grads.data_ptr(), self.exp_avg.data_ptr(),
-                    self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1, b2, self.defaults["eps"],
-                    self.defaults["weight_decay"], float(grad_scale), 1.0, self._state4.data_ptr(), self._dyn16.data_ptr(),
-                    1 if self.check_finite else 0)
-            if clip:
-                _lib.call("mf_adamw_step_dyn_clip", *args, float(max_grad_norm), self._norm_partials.data_ptr(),
-                          self.last_grad_norm.data_ptr(), torch.cuda.current_stream().cuda_stream)
-            else:
-                _lib.call("mf_adamw_step_dyn", *args, torch.cuda.current_stream().cuda_stream)
-            self._step_t += 1
-            for p in self.arena.tensors:
-                torch.autograd.graph.increment_version(p)
-            return None
-        _lib.call("mf_adamw_step", self.arena.params.data_ptr(), self.arena.grads.data_ptr(), self.exp_avg.data_ptr(),
-                  self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1, b2, self.defaults["eps"],
-                  self.defaults["weight_decay"], self.step_count, float(grad_scale), 1.0,
-                  torch.cuda.current_stream().cuda_stream)
+        if self.step_count == 1 and int(self._state4[0].item()) != 0:
+            raise RuntimeError("%s: device step counter out of sync" % type(self).__name__)
+        _lib.call("mf_optim_step_dyn", self._rule, self.arena.params.data_ptr(), self.arena.grads.data_ptr(),
+                  self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks,
+                  self._hyper.data_ptr(), self.defaults["betas"][1], self.defaults["eps"], float(grad_scale),
+                  self._state4.data_ptr(), self._dyn16.data_ptr(), float(max_grad_norm) if clip else 0.0,
+                  self._norm_partials.data_ptr(), self.last_grad_norm.data_ptr(), torch.cuda.current_stream().cuda_stream)
         self._step_t += 1
         for p in self.arena.tensors:            # cached kernel plans key on parameter versions (engine.fingerprint)
             torch.autograd.graph.increment_version(p)
@@ -325,9 +327,9 @@ def _fused_exchange_step(self, use_multicast=True):
     hp, hg, _ = self._symm
     world, rank = hp.world_size, hp.rank
     table = self._lr_table()
+    mult, b1, wd = self._hyper_key            # the p2p kernel reads no hyper block: the lr multiplier is its lr_scale
     self.step_count += 1
-    b1, b2 = self.defaults["betas"]
-    pp = (ctypes.c_ulonglong * world)(*[int(x) for x in hp.buffer_ptrs])
+    pp =(ctypes.c_ulonglong * world)(*[int(x) for x in hp.buffer_ptrs])
     gp = (ctypes.c_ulonglong * world)(*[int(x) for x in hg.buffer_ptrs])
     mc_p = int(hp.multicast_ptr or 0) if use_multicast else 0     # 0 when the fabric / driver has no NVLS multicast
     mc_g = int(hg.multicast_ptr or 0) if use_multicast else 0
@@ -335,8 +337,8 @@ def _fused_exchange_step(self, use_multicast=True):
         mc_p = mc_g = 0
     hg.barrier(channel=0)                       # every rank's backward has finished writing its gradient arena
     _lib.call("mf_adamw_step_p2p", ctypes.addressof(pp), ctypes.addressof(gp), world, rank, mc_p, mc_g,
-              self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1, b2,
-              self.defaults["eps"], self.defaults["weight_decay"], self.step_count, 1.0,
+              self.exp_avg.data_ptr(), self.exp_avg_sq.data_ptr(), table.data_ptr(), self.arena.n_chunks, b1,
+              self.defaults["betas"][1], self.defaults["eps"], wd, self.step_count, mult,
               torch.cuda.current_stream().cuda_stream)
     hp.barrier(channel=1)                       # every shard of the new parameters has landed in every arena
     self._step_t += 1
@@ -352,57 +354,15 @@ class FusedAdam(FusedAdamW):
     """torch.optim.Adam(params, lr, betas, weight_decay) (the reference's 'adam', solver/__init__.py:33-34) over a
     ParamArena, in the guarded capturable step of FusedAdamW: weight decay is coupled L2 (`g <- g + wd * p`, after any
     clipping), tensors marked unused (grad None in the reference) are not touched at all. `state_dict()` has
-    torch.optim.Adam's layout and loads into it and back.
-
-    Device hyper-parameter block (`_hyper`, float64 {lr multiplier, beta1, weight decay, 0}): refreshed in place by
-    `_lr_table()`, which `step()` calls and the captured Trainer calls before each replay. When every updated tensor's group
-    has the same lr, the chunk table holds 1 (0 / -1 for skipped / decay-only tensors) and the lr itself is the multiplier,
-    so a schedule that moves one lr for all groups rewrites 8 bytes, not the table."""
+    torch.optim.Adam's layout and loads into it and back."""
 
     _rule = 1                       # MF_OPTIM_ADAM
-    _unused_decays = False          # mark_unused tensors: skipped entirely (torch's Adam skips grad None)
 
-    def __init__(self, params, lr=1e-3, betas=(0.9, 0.99), eps=1e-8, weight_decay=0.0, check_finite=True,
-                 outside_params=()):
-        super().__init__(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, capturable=True,
-                         check_finite=check_finite, outside_params=outside_params)
+    def __init__(self, params, lr=1e-3, betas=(0.9, 0.99), eps=1e-8, weight_decay=0.0, outside_params=()):
+        super().__init__(params, lr=lr, betas=betas, eps=eps, weight_decay=weight_decay, outside_params=outside_params)
         self.defaults["decoupled_weight_decay"] = False            # torch.optim.Adam's group key (torch >= 2.6)
         for g in self.param_groups:
             g.setdefault("decoupled_weight_decay", False)
-        self._hyper = torch.zeros(4, dtype=torch.float64, device=self.arena.params.device)
-        self._hyper_key = None
-
-    def _weight_decay(self):
-        wds = {g["weight_decay"] for g in self.param_groups}
-        if len(wds) != 1:
-            raise NotImplementedError("%s: weight_decay must be the same for every group" % type(self).__name__)
-        return float(wds.pop())
-
-    def _lr_table(self):
-        groups = self._group_of_tensor()
-        betas = {tuple(g["betas"]) for g in self.param_groups}
-        if len(betas) != 1 or tuple(betas)[0][1] != self.defaults["betas"][1]:
-            raise NotImplementedError("%s: every group needs the same betas, and beta2 stays %r"
-                                      % (type(self).__name__, self.defaults["betas"][1]))
-        beta1 = float(tuple(betas)[0][0])
-        unused = -1.0 if self._unused_decays else 0.0
-        active = {float(g["lr"]) for g, skip in zip(groups, self._skip) if g is not None and (not skip or self._unused_decays)}
-        if len(active) == 1:                  # one shared lr: it goes to the device block, the table holds its sign pattern
-            mult = active.pop()
-            vals = tuple(0.0 if g is None else (unused if skip else 1.0) for g, skip in zip(groups, self._skip))
-        else:
-            mult = 1.0
-            vals = tuple(0.0 if g is None else (unused * g["lr"] if skip else g["lr"]) for g, skip in zip(groups, self._skip))
-        self._upload_table(vals)
-        key = (mult, beta1, self._weight_decay())
-        if key != self._hyper_key:
-            self._hyper.copy_(torch.tensor(key + (0.0,), dtype=torch.float64))   # in place, like the table
-            self._hyper_key = key
-        return self._chunk_lr
-
-    def load_state_dict(self, state_dict):
-        super().load_state_dict(state_dict)
-        self._hyper_key = None
 
     def step_exchange(self, use_multicast=True):
         raise NotImplementedError("%s: the fused peer-memory exchange runs AdamW only" % type(self).__name__)

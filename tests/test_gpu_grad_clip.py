@@ -1,4 +1,4 @@
-"""-m gpu: gradient-norm clipping on the device (FusedAdamW.step(max_grad_norm=...), mf_adamw_step_dyn_clip) against
+"""-m gpu: gradient-norm clipping on the device (FusedAdamW.step(max_grad_norm=...), mf_optim_step_dyn) against
 torch.nn.utils.clip_grad_norm_ + torch.optim.AdamW, and the captured Trainer with the reference's SOLVER.GRAD_NORM_CLIP."""
 import os
 import subprocess

@@ -274,7 +274,7 @@ def _lr_state(opt):
     if inner._chunk_lr is None:
         return lrs, moms, None, None
     a, table = inner.arena, inner._chunk_lr.cpu().numpy()
-    mult, beta1 = inner._hyper.cpu().tolist()[:2] if hasattr(inner, "_hyper") else (1.0, None)
+    mult, beta1 = inner._hyper.cpu().tolist()[:2]
     eff = [abs(float(table[o // a.chunk] * np.float32(mult))) for o in a.offsets[:inner.n_grouped]]
     return lrs, moms, eff, beta1
 
@@ -319,7 +319,7 @@ def test_captured_trainer_matches_eager(case, clip):
         ha, hb = _lr_state(ta.optimizer), _lr_state(tb.optimizer)
         assert ha == hb, i                  # the schedules moved the same way; both steps read the same table / block ...
         assert hb[2] == _expected_device_lrs(tb.optimizer, before[0]), i     # ... holding the lrs of the step just taken
-        assert hb[3] in (None, before[1][0]), (i, hb[3], before[1])         # ... and its beta1
+        assert hb[3] == before[1][0], (i, hb[3], before[1])                 # ... and its beta1
         if clip:
             assert float(ob.last_grad_norm) > cfg.SOLVER.GRAD_NORM_CLIP or i < 2, (i, float(ob.last_grad_norm))
         ta_tot, tb_tot = sum(la[k] for k in la if k.endswith("_loss")), sum(lb[k] for k in lb if k.endswith("_loss"))

@@ -1,5 +1,4 @@
-"""CPU: argument checks of the clipping AdamW entry point (mf_adamw_step_dyn_clip), which fail before any launch."""
-import ctypes
+"""CPU: argument checks of the optimiser step (mf_optim_step_dyn), which fail before any launch."""
 import os
 
 import pytest
@@ -17,10 +16,26 @@ def lib():
     return _lib.load()
 
 
-def test_clip_needs_partials_and_norm_output(lib):
-    dummy = 16                                                         # never dereferenced: the call fails first
-    for partials, norm_out in ((None, dummy), (dummy, None)):
-        rc = lib.mf_adamw_step_dyn_clip(dummy, dummy, dummy, dummy, dummy, 4, 0.9, 0.99, 1e-8, 1e-5, 1.0, 1.0, dummy, dummy, 1,
-                                        1.0, partials, norm_out, None)
-        assert rc != 0
+DUMMY = 16                                                             # never dereferenced: the call fails first
+
+
+def _step(lib, rule=0, hyper=DUMMY, max_norm=0.0, partials=DUMMY, norm_out=DUMMY):
+    return lib.mf_optim_step_dyn(rule, DUMMY, DUMMY, DUMMY, DUMMY, DUMMY, 4, hyper, 0.99, 1e-8, 1.0, DUMMY, DUMMY, max_norm,
+                                 partials, norm_out, None)
+
+
+def test_optim_step_clip_needs_partials_and_norm_output(lib):
+    for partials, norm_out in ((None, DUMMY), (DUMMY, None)):
+        assert _step(lib, max_norm=1.0, partials=partials, norm_out=norm_out) != 0
         assert b"partials buffer and total_norm_out" in lib.mf_last_error()
+
+
+def test_step_needs_hyper_block(lib):
+    assert _step(lib, hyper=None) != 0
+    assert b"hyper (device double[4]) is NULL" in lib.mf_last_error()
+
+
+@pytest.mark.parametrize("rule", [-1, 2])
+def test_step_refuses_unknown_rule(lib, rule):
+    assert _step(lib, rule=rule) != 0
+    assert ("rule %d" % rule).encode() in lib.mf_last_error()
