@@ -348,6 +348,24 @@ int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, flo
                       long long n_chunks, const double* hyper, float beta2, float eps, float grad_scale, long long* state4,
                       void* dyn16, float max_norm, double* partials, float* total_norm_out, void* stream);
 
+/* Dynamic loss scale (torch.amp.GradScaler's rule) kept in device memory: scale = device float, growth_tracker = device
+ * int, both read and written by the kernels only, so a captured training step follows them.
+ * mf_unscale_accumulate: for each of `count` triples (HOST arrays dst_ptrs / src_ptrs of device fp32 addresses, numels),
+ *   dst[i] += src[i] * inv_scale (one fma, like torch._foreach_add_(dst, src, alpha=inv_scale)), or dst[i] = src[i] *
+ *   inv_scale where assign[i] != 0 (assign: HOST array or NULL = accumulate everywhere), inv_scale = float(1.0 /
+ *   double(*scale)) as GradScaler computes it. One launch for up to mf_unscale_max_tensors() triples; empty triples are
+ *   skipped; the arrays are read before the call returns.
+ * mf_loss_scale_update: torch._amp_update_scale_ on the skip flag in dyn16 (the scratch of the mf_optim_step_dyn call just
+ *   enqueued on the same stream: a non-finite gradient arena or clipping norm): on a skip scale *= backoff_factor and
+ *   growth_tracker = 0; otherwise growth_tracker += 1 and, when it reaches growth_interval, scale *= growth_factor (kept
+ *   if finite) and growth_tracker = 0. The products are taken in double and rounded to float, as torch does. Needs
+ *   growth_factor > 1, 0 < backoff_factor < 1, growth_interval >= 1. One single-thread launch. */
+int mf_unscale_max_tensors(void);
+int mf_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs, const long long* numels,
+                          const unsigned char* assign, int count, const float* scale, void* stream);
+int mf_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor, double backoff_factor,
+                         int growth_interval, void* stream);
+
 /* DDP gradient all-reduce (tools/plain_train_net.py:100-104) FUSED with the AdamW step for world > 1: one kernel over
  * peer-mapped memory. param_ptrs / grad_ptrs: HOST arrays [world] of device addresses of every rank's parameter / gradient
  * arena as mapped into THIS process (symmetric memory / CUDA IPC); mc_params / mc_grads: NVLS multicast addresses of the

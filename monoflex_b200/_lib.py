@@ -79,6 +79,9 @@ SIGNATURES = {
     "mf_adamw_step_p2p": [_P, _P, _I, _I, ctypes.c_ulonglong, ctypes.c_ulonglong, _P, _P, _P, _LL, ctypes.c_double, _F, _F,
                           _F, _LL, _F, _P],
     "mf_optim_step_dyn": [_I, _P, _P, _P, _P, _P, _LL, _P, _F, _F, _F, _P, _P, _F, _P, _P, _P],
+    "mf_unscale_max_tensors": [],
+    "mf_unscale_accumulate": [_P, _P, _P, _P, _I, _P, _P],
+    "mf_loss_scale_update": [_P, _P, _P, ctypes.c_double, ctypes.c_double, _I, _P],
     "mf_preprocess_images_u8": [_P, _P, _P, _I, _I, _I, _P, _P, _I, _P, _P],
     "mf_draw_heatmaps": [_P, _I, _I, _I, _I, _I, _P, _P],
     "mf_encode_targets": [_P, _P, _P, _P, _I, _I, _I, _I] + [_P] * 14,

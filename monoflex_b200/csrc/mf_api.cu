@@ -496,6 +496,16 @@ int mf_optim_step_dyn(int rule, float* params, float* grads, float* exp_avg, flo
   return launch_adamw_arena_dyn(rule, params, grads, exp_avg, exp_avg_sq, chunk_lr, n_chunks, hyper, beta2, eps, grad_scale,
                                 state4, dyn16, max_norm, partials, total_norm_out, MF_STREAM(stream));
 }
+int mf_unscale_max_tensors(void) { return MF_UNSCALE_MAX_TENSORS; }
+int mf_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs, const long long* numels,
+                          const unsigned char* assign, int count, const float* scale, void* stream) {
+  return launch_unscale_accumulate(dst_ptrs, src_ptrs, numels, assign, count, scale, MF_STREAM(stream));
+}
+int mf_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor, double backoff_factor,
+                         int growth_interval, void* stream) {
+  return launch_loss_scale_update(dyn16, scale, growth_tracker, growth_factor, backoff_factor, growth_interval,
+                                  MF_STREAM(stream));
+}
 int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
                       unsigned long long mc_params, unsigned long long mc_grads, float* exp_avg, float* exp_avg_sq,
                       const float* chunk_lr, long long n_chunks, double beta1, float beta2, float eps, float weight_decay,

@@ -71,6 +71,12 @@ int launch_focal_loss_backward(const float* pred, const float* tgt, long long n,
 int launch_adamw_arena_dyn(int rule, float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
                            const double* hyper, float beta2, float eps, float grad_scale, long long* state4, void* dyn16,
                            float max_norm, double* partials, float* total_norm_out, cudaStream_t st);
+#define MF_UNSCALE_MAX_TENSORS 1024   /* (dst, src, n) triples of one mf_unscale_accumulate launch (by-value kernel params) */
+int launch_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs,
+                              const long long* numels, const unsigned char* assign, int count, const float* scale,
+                              cudaStream_t st);
+int launch_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor,
+                             double backoff_factor, int growth_interval, cudaStream_t st);
 // OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
 enum {
   MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,

@@ -342,6 +342,140 @@ int launch_adamw_arena_dyn(int rule, float* p, float* g, float* m, float* v, con
   return check_cuda(cudaGetLastError(), "mf_optim_step_dyn");
 }
 
+// ---------------------------------------------------------------- dynamic loss scale (torch.amp.GradScaler's rule)
+// The scale is device state (float scale, int growth_tracker), so a captured training step reads and updates it without
+// the host. Two kernels:
+//   * unscale_accumulate_kernel: dst_i += src_i * inv_scale over a list of (dst, src, n) triples in ONE launch (the
+//     backward tape's ~280 parameter gradients into p.grad), inv_scale = float(1.0 / double(scale)) - GradScaler's
+//     scale.double().reciprocal().float(). The product-add is one fma like torch._foreach_add_(dst, src, alpha) (exact
+//     for a power-of-two scale either way). A triple flagged `assign` is dst_i = src_i * inv_scale (p.grad None).
+//   * loss_scale_update_kernel (1 thread): torch._amp_update_scale_ on the skip flag the optimiser's prepare kernel
+//     published in AdamwDyn (a non-finite gradient arena or clipping norm): backoff on a skip, growth after
+//     growth_interval clean steps unless the grown scale is not finite.
+struct UnscaleList {
+  const float* src[MF_UNSCALE_MAX_TENSORS];
+  float* dst[MF_UNSCALE_MAX_TENSORS];
+  int n[MF_UNSCALE_MAX_TENSORS];
+  int tile0[MF_UNSCALE_MAX_TENSORS + 1];       // first tile of tensor i; tile0[count] = the grid
+  unsigned char assign[MF_UNSCALE_MAX_TENSORS];
+  int count;
+};
+constexpr int UNSCALE_TILE = 4096;              // elements per CTA: 256 threads x 4 float4
+
+__global__ void __launch_bounds__(256) unscale_accumulate_kernel(const __grid_constant__ UnscaleList L,
+                                                                 const float* __restrict__ scale) {
+  const float inv = static_cast<float>(1.0 / static_cast<double>(__ldg(scale)));
+  const int tile = blockIdx.x;
+  int lo = 0, hi = L.count - 1;                 // the tensor whose tiles cover this CTA: largest i with tile0[i] <= tile
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (L.tile0[mid] <= tile) lo = mid; else hi = mid - 1;
+  }
+  const int t = lo;
+  const long long base = static_cast<long long>(tile - L.tile0[t]) * UNSCALE_TILE;
+  const int n = L.n[t];
+  const float* __restrict__ src = L.src[t];
+  float* __restrict__ dst = L.dst[t];
+  const bool assign = L.assign[t] != 0;
+  const int end = static_cast<int>(min(static_cast<long long>(n), base + UNSCALE_TILE));
+  const bool vec = ((reinterpret_cast<unsigned long long>(src) | reinterpret_cast<unsigned long long>(dst)) & 15) == 0;
+  if (vec) {
+    const int v_end = end & ~3;
+    for (int i = static_cast<int>(base) + 4 * threadIdx.x; i < v_end; i += 4 * 256) {
+      const float4 s = __ldcs(reinterpret_cast<const float4*>(src + i));
+      float4 d;
+      if (assign) {
+        d.x = s.x * inv; d.y = s.y * inv; d.z = s.z * inv; d.w = s.w * inv;
+      } else {
+        d = *reinterpret_cast<const float4*>(dst + i);
+        d.x = __fmaf_rn(s.x, inv, d.x); d.y = __fmaf_rn(s.y, inv, d.y);
+        d.z = __fmaf_rn(s.z, inv, d.z); d.w = __fmaf_rn(s.w, inv, d.w);
+      }
+      *reinterpret_cast<float4*>(dst + i) = d;
+    }
+    for (int i = v_end + threadIdx.x; i < end; i += 256)
+      dst[i] = assign ? src[i] * inv : __fmaf_rn(src[i], inv, dst[i]);
+  } else {
+    for (int i = static_cast<int>(base) + threadIdx.x; i < end; i += 256)
+      dst[i] = assign ? src[i] * inv : __fmaf_rn(src[i], inv, dst[i]);
+  }
+}
+
+int launch_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs,
+                              const long long* numels, const unsigned char* assign, int count, const float* scale,
+                              cudaStream_t st) {
+  if (count < 0 || count > MF_UNSCALE_MAX_TENSORS) {
+    set_error("mf_unscale_accumulate: %d tensors (0 .. %d in one launch)", count, MF_UNSCALE_MAX_TENSORS);
+    return -1;
+  }
+  if (count > 0 && (dst_ptrs == nullptr || src_ptrs == nullptr || numels == nullptr)) {
+    set_error("mf_unscale_accumulate: dst_ptrs, src_ptrs and numels are host arrays of count entries, not NULL");
+    return -1;
+  }
+  if (scale == nullptr) { set_error("mf_unscale_accumulate: scale (device float) is NULL"); return -1; }
+  UnscaleList L;
+  long long tiles = 0;
+  int k = 0;
+  for (int i = 0; i < count; ++i) {
+    if (numels[i] < 0 || numels[i] > 0x7fffffffLL) {
+      set_error("mf_unscale_accumulate: tensor %d has %lld elements (0 .. 2^31 - 1)", i, numels[i]);
+      return -1;
+    }
+    if (numels[i] == 0) continue;
+    if (dst_ptrs[i] == 0 || src_ptrs[i] == 0) {
+      set_error("mf_unscale_accumulate: tensor %d has a NULL dst or src", i);
+      return -1;
+    }
+    L.dst[k] = reinterpret_cast<float*>(dst_ptrs[i]);
+    L.src[k] = reinterpret_cast<const float*>(src_ptrs[i]);
+    L.n[k] = static_cast<int>(numels[i]);
+    L.assign[k] = (assign != nullptr && assign[i]) ? 1 : 0;
+    L.tile0[k] = static_cast<int>(tiles);
+    tiles += (numels[i] + UNSCALE_TILE - 1) / UNSCALE_TILE;
+    ++k;
+  }
+  if (k == 0) return 0;
+  if (tiles > 0x7fffffffLL) { set_error("mf_unscale_accumulate: %lld tiles exceed one grid", tiles); return -1; }
+  L.tile0[k] = static_cast<int>(tiles);
+  L.count = k;
+  (void)launch_k(unscale_accumulate_kernel, dim3(static_cast<unsigned>(tiles)), dim3(256), 0, st, L, scale);
+  return check_cuda(cudaGetLastError(), "mf_unscale_accumulate");
+}
+
+__global__ void loss_scale_update_kernel(const AdamwDyn* __restrict__ dyn, float* scale, int* growth_tracker,
+                                         double growth_factor, double backoff_factor, int growth_interval) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  if (dyn->skip) {
+    *scale = static_cast<float>(static_cast<double>(*scale) * backoff_factor);
+    *growth_tracker = 0;
+  } else {
+    const int successful = *growth_tracker + 1;
+    if (successful == growth_interval) {
+      const float grown = static_cast<float>(static_cast<double>(*scale) * growth_factor);
+      if (isfinite(grown)) *scale = grown;            // never grow past float32's range to inf
+      *growth_tracker = 0;
+    } else {
+      *growth_tracker = successful;
+    }
+  }
+}
+
+int launch_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor,
+                             double backoff_factor, int growth_interval, cudaStream_t st) {
+  if (dyn16 == nullptr || scale == nullptr || growth_tracker == nullptr) {
+    set_error("mf_loss_scale_update: dyn16, scale and growth_tracker are device pointers, not NULL");
+    return -1;
+  }
+  if (!(growth_factor > 1.0) || !(backoff_factor > 0.0 && backoff_factor < 1.0) || growth_interval < 1) {
+    set_error("mf_loss_scale_update: needs growth_factor > 1, 0 < backoff_factor < 1, growth_interval >= 1 "
+              "(got %g, %g, %d)", growth_factor, backoff_factor, growth_interval);
+    return -1;
+  }
+  (void)launch_k(loss_scale_update_kernel, dim3(1), dim3(32), 0, st, static_cast<const AdamwDyn*>(dyn16), scale,
+                 growth_tracker, growth_factor, backoff_factor, growth_interval);
+  return check_cuda(cudaGetLastError(), "mf_loss_scale_update");
+}
+
 // ---------------------------------------------------------------- focal loss backward (layers/focal_loss.py:35-55)
 // L = -sum_{t==1} log(p)(1-p)^2 - sum_{0<=t<1} log(1-p) p^2 (1-t)^4
 // dL/dp = -( (1-p)^2 / p - 2 (1-p) log p )                          at t == 1

@@ -50,7 +50,11 @@ class KeypointDetector(nn.Module):
         self.set_precision(engine.default_precision())
         # fp16 gradient flow of the backward tape: dL/dcls, dL/dreg are multiplied by `loss_scale` before they enter the
         # tape and every parameter gradient is divided by it again before it is accumulated into p.grad (fp32)
-        self.loss_scale = float(os.environ.get("MF_LOSS_SCALE", "128"))
+        # MF_LOSS_SCALE=dynamic selects a loss_scale.DynamicLossScale in the Trainer; the static value then stays 128 and
+        # is not used. loss_scaler: a DynamicLossScale (device scale, GradScaler's rule) or None for the static scale.
+        env_scale = os.environ.get("MF_LOSS_SCALE", "128")
+        self.loss_scale = 128.0 if env_scale.strip().lower() == "dynamic" else float(env_scale)
+        self.loss_scaler = None
         self._anchor = None
 
     def set_precision(self, mode):
@@ -98,7 +102,13 @@ class KeypointDetector(nn.Module):
     def _tape_backward(self, g_cls, g_reg):
         """dL/dcls, dL/dreg -> accumulate dL/dp into p.grad for every parameter the forward used (the backward tape)."""
         from ..tape import backbone_backward, predictor_backward
-        pred_mod, S = self.heads.predictor, self.loss_scale
+        pred_mod, S, scaler = self.heads.predictor, self.loss_scale, self.loss_scaler
+        if scaler is not None:
+            if scaler.optimizer is None:
+                raise RuntimeError("model.loss_scaler is set, but no fused optimiser updates it: a dynamic loss scale needs "
+                                   "solver.FusedAdamW / FusedAdam / FusedOneCycleAdam .step(loss_scaler=...) after every "
+                                   "backward (Trainer(loss_scale='dynamic') does this; by hand: loss_scaler.attach(optimizer))")
+            S = scaler.scale                 # 0-d device tensor: the seeding multiply reads the current scale on the GPU
         plan_h, plan_b = pred_mod.last_plan, self.backbone.last_plan
         if g_cls is None:
             g_cls = torch.zeros_like(plan_h.cls)
@@ -109,16 +119,24 @@ class KeypointDetector(nn.Module):
         params = getattr(self, "_param_by_name", None)
         if params is None:
             params = self._param_by_name = dict(self.named_parameters())
-        inv = 1.0 / S
+        inv = None if scaler is not None else 1.0 / S
         used = set()
-        acc_dst, acc_src = [], []
+        acc_dst, acc_src, acc_assign = [], [], []
         for prefix, grads in (("heads.predictor.", hgrads), ("backbone.", bgrads)):
             for name, g in grads.items():
                 p = params[prefix + name]
                 used.add(prefix + name)
                 if not p.requires_grad:
                     continue
-                if p.grad is None:
+                if scaler is not None:       # every p.grad in the one unscale launch below; a first gradient is assigned
+                    assign = p.grad is None
+                    if assign:
+                        p.grad = torch.empty_like(p)
+                    acc_dst.append(p.grad)
+                    acc_assign.append(assign)
+                    g = g.view_as(p)
+                    acc_src.append(g if g.is_contiguous() and g.dtype == p.grad.dtype else g.contiguous().to(p.grad.dtype))
+                elif p.grad is None:
                     p.grad = (g * inv).view_as(p)
                 else:
                     acc_dst.append(p.grad)
@@ -126,7 +144,9 @@ class KeypointDetector(nn.Module):
                     # the multi-tensor kernel needs dense operands; ONE strided gradient would send the whole list down the
                     # per-tensor slow path (285 tiny add kernels per step in the ncu launch list)
                     acc_src.append(g if g.is_contiguous() and g.dtype == p.grad.dtype else g.contiguous().to(p.grad.dtype))
-        if acc_dst:                          # one multi-tensor kernel instead of ~280 tiny adds (p.grad += g / loss_scale)
+        if scaler is not None:               # p.grad += g * inv_scale, inv_scale read from the device scale, one launch
+            scaler.unscale_accumulate(acc_dst, acc_src, acc_assign)
+        elif acc_dst:                        # one multi-tensor kernel instead of ~280 tiny adds (p.grad += g / loss_scale)
             torch._foreach_add_(acc_dst, acc_src, alpha=inv)
         self.last_grad_names = used          # parameters outside the forward graph (the reference leaves their .grad None)
 

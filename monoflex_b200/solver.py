@@ -278,14 +278,25 @@ class FusedAdamW(torch.optim.Optimizer):
         """number of optimiser steps skipped because the gradient arena held a non-finite value (host sync)"""
         return int(self._state4[2].item())
 
+    def state_dict(self):
+        """torch.optim's layout. `step` is the number of updates APPLIED: on a CUDA arena it is read from the device
+        counter (one host read), which leaves out the steps the finite guard skipped - the count the bias corrections
+        used, and what torch's AdamW under GradScaler counts. The host `step_count` is brought in line with it."""
+        if self.arena.params.is_cuda and self._symm is None:       # the peer-memory exchange counts on the host only
+            self.step_count = int(self._state4[0].item())
+            self._step_t.fill_(float(self.step_count))
+        return super().state_dict()
+
     @torch.no_grad()
-    def step(self, closure=None, grad_scale=1.0, max_grad_norm=None):
+    def step(self, closure=None, grad_scale=1.0, max_grad_norm=None, loss_scaler=None):
         """One AdamW update of the whole arena on `grad_scale * grads`.
         max_grad_norm > 0: `torch.nn.utils.clip_grad_norm_(params, max_grad_norm)` first, on the device and inside the same
         three launches (capturable): the norm of `grad_scale * grads` goes to `last_grad_norm` (a 0-d device tensor, the
         value clip_grad_norm_ returns; read it without a sync), the gradient arena is left clipped like p.grad after
         clip_grad_norm_ (still the SUM when grad_scale = 1/world), and a non-finite norm skips the step like any non-finite
-        gradient. None or <= 0 (the reference's GRAD_NORM_CLIP = -1): no clipping, `last_grad_norm` is not written."""
+        gradient. None or <= 0 (the reference's GRAD_NORM_CLIP = -1): no clipping, `last_grad_norm` is not written.
+        loss_scaler: a loss_scale.DynamicLossScale; its scale is then updated on the device by GradScaler's rule from this
+        step's skip decision (one more single-thread launch, no host read)."""
         if closure is not None:
             raise NotImplementedError("FusedAdamW: closures are not used by the reference trainer")
         if not self.arena.params.is_cuda:
@@ -295,6 +306,12 @@ class FusedAdamW(torch.optim.Optimizer):
         lib = _lib.load()
         if lib.mf_adamw_chunk() != self.arena.chunk:
             raise RuntimeError("FusedAdamW: arena chunk %d != library chunk %d" % (self.arena.chunk, lib.mf_adamw_chunk()))
+        if loss_scaler is not None:
+            if loss_scaler.optimizer is not self:
+                loss_scaler.attach(self)
+            if loss_scaler.scale.device != self.arena.params.device:
+                raise ValueError("%s.step: the loss scale lives on %s, the arena on %s" % (
+                    type(self).__name__, loss_scaler.scale.device, self.arena.params.device))
         gbase, pbase = self.arena.grads.data_ptr(), self.arena.params.data_ptr()
         for p, o in zip(self.arena.tensors, self.arena.offsets):   # a caller that replaced .grad / .data breaks the arena
             g = p.grad                                              # contract: fail loudly instead of updating stale memory
@@ -310,6 +327,8 @@ class FusedAdamW(torch.optim.Optimizer):
                   self._hyper.data_ptr(), self.defaults["betas"][1], self.defaults["eps"], float(grad_scale),
                   self._state4.data_ptr(), self._dyn16.data_ptr(), float(max_grad_norm) if clip else 0.0,
                   self._norm_partials.data_ptr(), self.last_grad_norm.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        if loss_scaler is not None:
+            loss_scaler.update(self._dyn16)
         self._step_t += 1
         for p in self.arena.tensors:            # cached kernel plans key on parameter versions (engine.fingerprint)
             torch.autograd.graph.increment_version(p)
@@ -487,9 +506,9 @@ class FusedOneCycleAdam(object):
     def zero_grad(self, set_to_none=False):
         self.opt.zero_grad()
 
-    def step(self, closure=None, grad_scale=1.0, max_grad_norm=None):
+    def step(self, closure=None, grad_scale=1.0, max_grad_norm=None, loss_scaler=None):
         self._set("weight_decay", 0)               # true_wd: the decay is outside Adam
-        return self.opt.step(closure, grad_scale=grad_scale, max_grad_norm=max_grad_norm)
+        return self.opt.step(closure, grad_scale=grad_scale, max_grad_norm=max_grad_norm, loss_scaler=loss_scaler)
 
     def state_dict(self):
         return self.opt.state_dict()

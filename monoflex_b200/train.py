@@ -35,10 +35,18 @@ step just taken; 'adam_onecycle' with LR_WARMUP raises (the reference asserts a 
 plain adamw / LambdaLR case keeps calling `scheduler.step()` without an index. The captured step refreshes the optimiser's
 device lr table and hyper-parameter block (lr, beta1 and weight decay a schedule moves) before every replay, so the
 one-GPU update stays inside the graph for every optimiser.
+
+`loss_scale`: a float is the static loss scale of the fp16 backward (`model.loss_scale`, default 128 or MF_LOSS_SCALE);
+"dynamic" (or MF_LOSS_SCALE=dynamic) or a `loss_scale.DynamicLossScale` turns on the dynamic scale: `model.loss_scaler`
+seeds the backward with the device scale, unscales into p.grad on the device, and every optimiser step (eager or
+captured, after the NCCL all-reduce on several GPUs, so every rank keeps the same scale) updates it by GradScaler's rule
+from the finite guard's skip decision. `trainer.scaler` is the DynamicLossScale, None for a static scale. Not available
+with `symmetric_group` (the peer-memory exchange kernel has no finite guard).
 """
 import torch
 import torch.distributed as dist
 
+from . import loss_scale as _loss_scale
 from . import solver
 from .targets import EncodedTargets
 
@@ -63,14 +71,21 @@ class Trainer(object):
             raise NotImplementedError("GRAD_NORM_CLIP > 0 with symmetric_group: the fused peer-memory exchange (step_exchange) "
                                       "has no cross-rank gradient norm between its reduce and its update; use the NCCL "
                                       "exchange (no symmetric_group) or use_cuda_graph=False")
+        static_scale, self.scaler = _loss_scale.resolve(loss_scale)
+        if self.scaler is not None and symmetric_group is not None:
+            raise NotImplementedError("a dynamic loss scale with symmetric_group: the fused peer-memory exchange kernel has "
+                                      "no finite guard to update the scale from; use the NCCL exchange (no symmetric_group)")
         self.model = model.train()
-        if loss_scale is not None:
-            model.loss_scale = float(loss_scale)
+        if static_scale is not None:
+            model.loss_scale = static_scale
         self.cfg = cfg
         self.group = process_group
         self.bucket_bytes = bucket_bytes
         self.optimizer = solver.build_optimizer(model, cfg, symmetric_group=symmetric_group)
         self._arena_opt = getattr(self.optimizer, "opt", self.optimizer)    # FusedOneCycleAdam wraps its arena optimiser
+        if self.scaler is not None:
+            self.scaler.attach(self._arena_opt)
+        model.loss_scaler = self.scaler
         self.scheduler, self.warmup_scheduler = solver.build_scheduler(self.optimizer, cfg.SOLVER)
         # indexed stepping of do_train (engine/trainer.py:123-126) with a warm-up or one-cycle schedule
         self._indexed_schedule = onecycle or self.warmup_scheduler is not None
@@ -125,7 +140,8 @@ class Trainer(object):
         else:
             if world > 1:
                 solver.allreduce_grads(opt.arena, self.bucket_bytes, self.group)
-            opt.step(grad_scale=1.0 / world, max_grad_norm=max_grad_norm)   # clips the rank mean, as DDP + clip_grad_norm_
+            opt.step(grad_scale=1.0 / world, max_grad_norm=max_grad_norm,   # clips the rank mean, as DDP + clip_grad_norm_
+                     loss_scaler=self.scaler)
 
     # ------------------------------------------------------------------ captured step
     def _capture(self, images, targets):
@@ -148,7 +164,7 @@ class Trainer(object):
                 opt.zero_grad()
                 losses.backward()
                 if g["update_inside"]:
-                    self.optimizer.step(grad_scale=1.0, max_grad_norm=self.grad_norm_clip)
+                    self.optimizer.step(grad_scale=1.0, max_grad_norm=self.grad_norm_clip, loss_scaler=self.scaler)
         finally:
             pred._targets_preloaded = False
         if g["update_inside"]:                 # capture only records: undo the host-side bookkeeping of the captured step()
