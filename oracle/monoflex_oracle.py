@@ -121,10 +121,11 @@ def dcn_columns(x, offset, mask, k=3, pad=1, dil=1):
     """modulated_deformable_im2col (src/cpu/dcn_v2_im2col_cpu.cpp:27-56,127-196), stride 1, dg=1.
     Returns columns [B, C, k*k, H*W] (reference layout [B, C*k*k, H*W] viewed)."""
     B, C, H, W = x.shape
-    ys = torch.arange(H, dtype=torch.float32).view(1, 1, H, 1)
-    xs = torch.arange(W, dtype=torch.float32).view(1, 1, 1, W)
-    ki = torch.arange(k * k) // k
-    kj = torch.arange(k * k) % k
+    dev = x.device
+    ys = torch.arange(H, dtype=torch.float32, device=dev).view(1, 1, H, 1)
+    xs = torch.arange(W, dtype=torch.float32, device=dev).view(1, 1, 1, W)
+    ki = torch.arange(k * k, device=dev) // k
+    kj = torch.arange(k * k, device=dev) % k
     off = offset.view(B, k * k, 2, H, W)
     h_im = (ys - pad) + (ki.view(1, -1, 1, 1) * dil).float() + off[:, :, 0]   # h_in + i*dil + offset_h  (:176)
     w_im = (xs - pad) + (kj.view(1, -1, 1, 1) * dil).float() + off[:, :, 1]
