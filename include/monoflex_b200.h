@@ -242,7 +242,8 @@ int mf_dcn_col2im_nhwc_f16(const void* x, int x_ld, const float* offmask, int om
 
 /* Training-mode nn.BatchNorm2d(momentum 0.1) / InPlaceABN over NHWC fp16 rows (dla_dcn.py:76-79, detector_predictor.py:50,74;
  * eval mode is folded into the conv epilogues instead). x = raw conv output [M, x_ld], C channels (multiple of 8).
- * forward: batch mean / biased variance (deterministic two-level reduction), running-stat update like torch (unbiased
+ * forward: batch mean / biased variance (deterministic two-level reduction of x - x[row 0], so that a channel's mean does
+ *   not cancel its variance away), running-stat update like torch (unbiased
  *   variance, skipped when running_mean is NULL), y = act(x * scale + shift [+ res]); act 0 none / 1 ReLU / 2 leaky 0.01;
  *   abs_gamma = 1 uses |gamma| + eps (InPlaceABN). Outputs mean, rstd, scale, shift [C] are kept for the backward call.
  * backward: g = dy * act'(y); dgamma = sum g * xhat, dbeta = sum g; dx = scale * (g - mean(g) - xhat * mean(g * xhat));
@@ -261,7 +262,8 @@ int mf_bn_train_backward(const void* x, int x_ld, const void* dy, int dy_ld, con
  * train-mode BatchNorm kernels split around the exchange. `sums` is a DEVICE double [2][C] buffer: *_stats writes the local
  * per-channel sums (forward: sum x, sum x^2; backward: sum g, sum g*xhat, plus the LOCAL dgamma / dbeta that DDP averages like any
  * gradient), the host all-reduces it (SUM, NCCL, same stream), *_apply normalises with `count` = the global number of elements per
- * channel. workspace: mf_bn_train_workspace(M, C) bytes. With one rank the pair equals mf_bn_train_forward / _backward. */
+ * channel. workspace: mf_bn_train_workspace(M, C) bytes. With one rank the pair equals mf_bn_train_forward / _backward
+ * to rounding (its forward sums x, not x - x[row 0]: the first rows of the ranks differ). */
 int mf_bn_sync_forward_stats(const void* x, int x_ld, long long M, int C, float* workspace, double* sums, void* stream);
 int mf_bn_sync_forward_apply(const void* x, int x_ld, long long M, int C, const double* sums, double count, const float* gamma,
                              const float* beta, float eps, float momentum, int abs_gamma, float* running_mean, float* running_var,

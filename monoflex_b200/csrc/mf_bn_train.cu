@@ -1,6 +1,7 @@
 // Training-mode BatchNorm2d over NHWC fp16 rows (nn.BatchNorm2d(momentum=0.1) after every conv of the backbone,
 // model/backbone/dla_dcn.py:76-79 etc.; eval mode is folded into the conv epilogue instead). HBM-bound kernels:
-//   forward : bn_partial_kernel     per-CTA fp32 partial sums of x and x^2 per channel (deterministic: fixed row->CTA map)
+//   forward : bn_partial_kernel     per-CTA fp32 partial sums of d and d^2 per channel, d = x - x[row 0] (deterministic:
+//                                   fixed row->CTA map)
 //             bn_finalize_kernel    fixed-order double reduction -> mean, biased var, (scale, shift), running-stat update
 //             bn_apply_kernel       y = act(x * scale + shift [+ residual])                     (one read, one write)
 //   backward: bn_bwd_partial_kernel per-CTA partial sums of g and g * xhat, g = dy * act'(y)
@@ -34,11 +35,15 @@ MF_DEVINL float bn_act_grad(float y, int act) {           // derivative of the a
 
 // thread (cv, r): channel chunk cv (8 channels), row lane r; the CTA walks rows r0 + r, r0 + r + RL, ... of ITS slab.
 // part layout: [ncta][2][C] (sum a, sum b)
+// Forward with pivot != 0: the sums are of d = x - x[row 0], the channel's first value. E[d^2] - E[d]^2 then cancels only
+// as much as the spread of the channel allows, not its mean: summed as E[x^2] - E[x]^2 in fp32, the variance was off by
+// ~2^-24 (mean/std)^2 of itself, and a constant channel kept a variance of rounding noise instead of 0. The SyncBatchNorm
+// halves pass pivot = 0: their sums are added across ranks, whose first rows differ.
 template <bool BWD>
 __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restrict__ x, int x_ld, const __half* __restrict__ dy,
                                                          int dy_ld, const __half* __restrict__ y, int y_ld,
                                                          const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                         long long M, int C, int act, long long rows_per_cta,
+                                                         long long M, int C, int act, long long rows_per_cta, int pivot,
                                                          float* __restrict__ part) {
   extern __shared__ float sm[];                            // [RL][2][C]
   const int CV = C / 8, RL = blockDim.x / CV;
@@ -50,6 +55,11 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
   if (BWD) {
 #pragma unroll
     for (int e = 0; e < 8; ++e) { mu[e] = mean[cv * 8 + e]; rs[e] = rstd[cv * 8 + e]; }
+  } else if (pivot) {
+    bn_unpack8(__ldg(reinterpret_cast<const uint4*>(x + cv * 8)), mu);
+  } else {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) mu[e] = 0.f;
   }
   const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
   const long long r1 = r0 + rows_per_cta < M ? r0 + rows_per_cta : M;
@@ -66,8 +76,6 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
         if (BWD) {
           gq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(dy + rc * dy_ld + cv * 8)) : make_uint4(0u, 0u, 0u, 0u);
           yq[u] = __ldg(reinterpret_cast<const uint4*>(y + rc * y_ld + cv * 8));
-        } else if (!ok) {
-          xq[u] = make_uint4(0u, 0u, 0u, 0u);
         }
       }
 #pragma unroll
@@ -75,8 +83,13 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
         float xv[8];
         bn_unpack8(xq[u], xv);
         if (!BWD) {
+          const bool ok = row + static_cast<long long>(u) * RL < r1;    // rows past the slab add nothing
 #pragma unroll
-          for (int e = 0; e < 8; ++e) { a[e] += xv[e]; b[e] += xv[e] * xv[e]; }
+          for (int e = 0; e < 8; ++e) {
+            const float d = ok ? xv[e] - mu[e] : 0.f;
+            a[e] += d;
+            b[e] += d * d;
+          }
         } else {
           float gv[8], yv[8];
           bn_unpack8(gq[u], gv);
@@ -111,17 +124,19 @@ MF_DEVINL double bn_warp_sum(const float* __restrict__ part, int ncta, int C, in
 }
 
 // forward finalize: one WARP per channel (a single thread walking ~1000 partials was 22 us of pure latency per layer)
-__global__ void bn_finalize_kernel(const float* __restrict__ part, int ncta, int C, long long M, const float* __restrict__ gamma,
-                                   const float* __restrict__ beta, float eps, float momentum, int abs_gamma,
-                                   float* __restrict__ running_mean, float* __restrict__ running_var,
+// x: the rows whose first row bn_partial_kernel took as the pivot
+__global__ void bn_finalize_kernel(const float* __restrict__ part, int ncta, int C, long long M, const __half* __restrict__ x,
+                                   const float* __restrict__ gamma, const float* __restrict__ beta, float eps, float momentum,
+                                   int abs_gamma, float* __restrict__ running_mean, float* __restrict__ running_var,
                                    float* __restrict__ mean_out, float* __restrict__ rstd_out, float* __restrict__ scale,
                                    float* __restrict__ shift) {
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (c >= C) return;
   const double s = bn_warp_sum(part, ncta, C, 0, c, lane), ss = bn_warp_sum(part, ncta, C, 1, c, lane);
   if (lane != 0) return;
-  const double mean = s / static_cast<double>(M);
-  double var = ss / static_cast<double>(M) - mean * mean;
+  const double md = s / static_cast<double>(M);           // mean of d = x - pivot
+  double var = ss / static_cast<double>(M) - md * md;
+  const double mean = static_cast<double>(__half2float(x[c])) + md;
   if (var < 0.0) var = 0.0;
   const float rstd = static_cast<float>(1.0 / sqrt(var + static_cast<double>(eps)));
   float g = gamma[c];
@@ -303,9 +318,9 @@ int launch_bn_train_forward(const __half* x, int x_ld, long long M, int C, const
   if (sm > 64 * 1024) { set_error("bn_train_forward: shared memory"); return -1; }
   (void)launch_k(bn_partial_kernel<false>, dim3(ncta), dim3(th), sm, st, x, x_ld, static_cast<const __half*>(nullptr), 0,
                  static_cast<const __half*>(nullptr), 0, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), M,
-                 C, 0, rpc, workspace);
-  bn_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, M, gamma, beta, eps, momentum, abs_gamma, running_mean,
-                                                      running_var, mean, rstd, scale, shift);
+                 C, 0, rpc, 1, workspace);
+  bn_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, M, x, gamma, beta, eps, momentum, abs_gamma,
+                                                      running_mean, running_var, mean, rstd, scale, shift);
   const long long n = M * (C / 8);
   (void)launch_k(bn_apply_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_ld,
                  static_cast<const float*>(scale), static_cast<const float*>(shift), res, res_ld, act, y, y_ld, M, C);
@@ -324,7 +339,7 @@ int launch_bn_train_backward(const __half* x, int x_ld, const __half* dy, int dy
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_train_backward: C=%d too wide", C); return -1; }
   float* sums = workspace + static_cast<size_t>(ncta) * 2 * C;        // [2][C] after the partials
   (void)launch_k(bn_partial_kernel<true>, dim3(ncta), dim3(th), sm, st, x, x_ld, dy, dy_ld, y, y_ld, mean, rstd, M, C, act, rpc,
-                 workspace);
+                 0, workspace);
   bn_bwd_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, dgamma, dbeta, sums, sums + C);
   const long long n = M * (C / 8);
   (void)launch_k(bn_bwd_apply_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_ld, dy, dy_ld, y, y_ld,
@@ -347,7 +362,7 @@ int launch_bn_sync_forward_stats(const __half* x, int x_ld, long long M, int C, 
   }
   (void)launch_k(bn_partial_kernel<false>, dim3(ncta), dim3(th), sm, st, x, x_ld, static_cast<const __half*>(nullptr), 0,
                  static_cast<const __half*>(nullptr), 0, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), M,
-                 C, 0, rpc, workspace);
+                 C, 0, rpc, 0, workspace);
   bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, sums);
   return check_cuda(cudaGetLastError(), "bn_sync_forward_stats");
 }
@@ -371,7 +386,7 @@ int launch_bn_sync_backward_stats(const __half* x, int x_ld, const __half* dy, i
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_sync_backward_stats: C=%d too wide", C); return -1; }
   (void)launch_k(bn_partial_kernel<true>, dim3(ncta), dim3(th), sm, st, x, x_ld, dy, dy_ld, y, y_ld, mean, rstd, M, C, act, rpc,
-                 workspace);
+                 0, workspace);
   bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, sums);
   bn_bwd_sums_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, nullptr, nullptr, dgamma, dbeta);      // local parameter gradients
   return check_cuda(cudaGetLastError(), "bn_sync_backward_stats");

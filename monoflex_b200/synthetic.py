@@ -357,14 +357,15 @@ def make_train_targets(batch, seed=5, out_w=320, out_h=96, max_objs=MAX_OBJECTS,
     return out
 
 
-def make_train_param_lists(fields):
+def make_train_param_lists(fields, out_w=320, out_h=96):
     """ParamsList objects (is_train=True) as the reference's collate hands them to model(images, targets)
-    (data/collate_batch.py); field names of kitti.py:496-521."""
+    (data/collate_batch.py); field names of kitti.py:496-521. The edge indices are those of an (out_w x 4) x (out_h x 4)
+    padded image, the geometry make_train_targets was given."""
     from .structures import Calibration, ParamsList
-    idx, n, img_size = edge_indices()
+    idx, n, img_size = edge_indices(out_w, out_h)
     res = []
     for f in fields:
-        t = ParamsList((1280, 384), is_train=True)
+        t = ParamsList((out_w * 4, out_h * 4), is_train=True)
         for k, v in f.items():
             t.add_field("2d_bboxes" if k == "bboxes" else k, torch.from_numpy(np.ascontiguousarray(v)))
         t.add_field("calib", Calibration(KITTI_P2))

@@ -83,10 +83,16 @@ LAUNCHES = {
 # ------------------------------------------------------------------------------------------------ recording the plan
 class Op(object):
     """one recorded plan-builder call: its kind, bound arguments, returned Act, [first, end) launch range and, for a DCN,
-    the fp32 [M, 32] offset/mask rows it keeps"""
+    the fp32 [M, 32] offset/mask rows it keeps; `subs` are the recorded calls it made itself, `kept` the tensors it added
+    to plan.keep and `saved` its Plan.bn_saved entries (train plans)"""
 
-    def __init__(self, plan, kind, args, y, first, end, om):
+    def __init__(self, plan, kind, args, y, first, end, om, subs=(), kept=(), saved=()):
         self.plan, self.kind, self.args, self.y, self.first, self.end, self.om = plan, kind, args, y, first, end, om
+        self.subs, self.kept, self.saved = list(subs), list(kept), list(saved)
+
+    def sub(self, kind):
+        """the first recorded call of `kind` this op made itself"""
+        return next(o for o in self.subs if o.kind == kind)
 
     @property
     def x(self):
@@ -99,9 +105,11 @@ class Op(object):
         return [a for a in (self.x, self.args.get(extra)) if a is not None]
 
 
-def record(monkeypatch):
-    """wrap the plan builder's op emitters; returns the list the wrapped calls are appended to"""
-    ops, depth = [], [0]
+def record(monkeypatch, kinds=RECORDED):
+    """wrap the plan builder's op emitters `kinds`; returns the list the outermost wrapped calls are appended to (the
+    calls they make themselves go to their `subs`)"""
+    ops = []
+    frames = [ops]                        # the list the call being recorded is appended to, innermost last
 
     def wrap(kind, fn):
         sig = inspect.signature(fn)
@@ -109,31 +117,34 @@ def record(monkeypatch):
         def recorded(self, *args, **kw):
             bound = sig.bind(self, *args, **kw)
             bound.apply_defaults()
-            first, keep0 = len(self.ops), len(self.keep)
-            depth[0] += 1
+            first, keep0, saved0 = len(self.ops), len(self.keep), len(self.bn_saved)
+            frames.append([])
             try:
                 y = fn(self, *args, **kw)
             finally:
-                depth[0] -= 1
-            if depth[0] == 0:
-                a = dict(bound.arguments)
-                del a["self"]
-                ops.append(Op(self, kind, a, y, first, len(self.ops), self.keep[keep0] if kind == "dcn" else None))
+                subs = frames.pop()
+            a = dict(bound.arguments)
+            del a["self"]
+            frames[-1].append(Op(self, kind, a, y, first, len(self.ops), self.keep[keep0] if kind == "dcn" else None,
+                                 subs, self.keep[keep0:], self.bn_saved[saved0:]))
             return y
         return recorded
 
-    for kind in RECORDED:
+    for kind in kinds:
         monkeypatch.setattr(engine.Plan, kind, wrap(kind, getattr(engine.Plan, kind)))
     return ops
 
 
-def check_coverage(ops, names, precision):
-    """the recorded launch ranges tile [0, len(names)) and each emits exactly the launches of its kind -> problems"""
+def check_coverage(ops, names, precision, launches=None):
+    """the recorded launch ranges tile [0, len(names)) and each emits exactly the launches of its kind -> problems.
+    `launches` (default LAUNCHES): (kind, precision) -> the launch names, or a function of the op giving them"""
     bad, pos = [], 0
     for op in sorted(ops, key=lambda o: o.first):
         if op.first != pos:
             bad.append("launches %d..%d: %s" % (pos, op.first, names[pos:op.first]))
-        want = LAUNCHES.get((op.kind, precision))
+        want = (LAUNCHES if launches is None else launches).get((op.kind, precision))
+        if callable(want):
+            want = want(op)
         if want is None or tuple(names[op.first:op.end]) != want:
             bad.append("%s at %d: %s" % (op.kind, op.first, names[op.first:op.end]))
         pos = max(pos, op.end)
@@ -210,9 +221,15 @@ def param64(w, kind="fp32"):
     return w.double()
 
 
-def conv_ref(x, w, stride, pad, bn, act, residual=None, weights="fp32"):
-    """eval-mode conv + BatchNorm (+ residual) + activation in float64"""
-    y = F.conv2d(x, param64(w, weights).to(x.device), None, stride, pad)
+def conv_ref(x, w, stride, pad, bn, act, residual=None, weights="fp32", bias=None):
+    """eval-mode conv (+ bias) + BatchNorm (+ residual) + activation in float64; bn=None: no normalisation (the raw
+    convolutions of train plans). A Conv1d weight [O, I, k] runs as [O, I, 1, k] over a [B, I, 1, L] input."""
+    w = param64(w, weights).to(x.device)
+    if w.dim() == 3:
+        w = w.unsqueeze(2)
+    y = F.conv2d(x, w, None if bias is None else bias.detach().double().to(x.device), stride, pad)
+    if bn is None:
+        return activate(y if residual is None else y + residual, act)
     s, t = bn_fold(bn)
     y = y * s.to(y.device).view(1, -1, 1, 1) + t.to(y.device).view(1, -1, 1, 1)
     if residual is not None:
@@ -229,7 +246,8 @@ def offset_mask_ref(x, om_conv, weights="fp32"):
 def dcn_ref(x, dcn_mod, bn, off, mask, fp16=False, weights="fp32"):
     """DCNv2 gather + contract + BatchNorm + ReLU on the given offsets/masks. Strict: the oracle's dcn_v2_forward in float64
     (float32 offsets keep the sampling positions and bilinear weights in float32, as the reference computes them). Fast:
-    the blend of the fp16 input in float32, rounded to fp16 as the kernel stores it, fp16 weights."""
+    the blend of the fp16 input in float32, rounded to fp16 as the kernel stores it, fp16 weights. bn=None: the raw
+    output (gather + contract + bias) a train plan normalises with batch statistics."""
     w, b = dcn_mod.weight.detach(), dcn_mod.bias.detach().double().to(x.device)
     if fp16:
         B, C, H, W = x.shape
@@ -237,6 +255,8 @@ def dcn_ref(x, dcn_mod, bn, off, mask, fp16=False, weights="fp32"):
         out = (torch.matmul(param64(w, "fp16").to(x.device).reshape(w.shape[0], -1), cols) + b.view(1, -1, 1)).view(B, -1, H, W)
     else:
         out = mo.dcn_v2_forward(x, param64(w, weights).to(x.device), b, off, mask)
+    if bn is None:
+        return out
     s, t = bn_fold(bn)
     return F.relu(out * s.to(x.device).view(1, -1, 1, 1) + t.to(x.device).view(1, -1, 1, 1))
 
