@@ -166,9 +166,6 @@ int mf_dcn_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, const
 /* images [B,C<=8,H,W] fp32 NCHW (engine/trainer.py:106, engine/inference.py:29) -> NHWC fp16 with 8 channels */
 int mf_pack_image(const float* x_nchw, void* y_nhwc8, int B, int C, int H, int W, void* stream);
 int mf_nchw_f32_to_nhwc_f16(const float* x, void* y, int B, int C, int HW, int y_ld, void* stream);
-int mf_nhwc_f16_to_nchw_f32(const void* x, float* y, int B, int C, int HW, int x_ld, void* stream);
-/* offset [B,18,H,W] + mask [B,9,H,W] (reference _ext layout) -> [B*HW, 32] fp32 rows */
-int mf_pack_offmask(const float* offset, const float* mask, float* y, int B, int HW, void* stream);
 /* nn.MaxPool2d(2) of Tree.downsample (dla_dcn.py:238) */
 int mf_maxpool2_nhwc_f16(const void* x, void* y, int B, int H, int W, int C, int x_ld, int y_ld, void* stream);
 /* depthwise ConvTranspose2d(k=2f, stride f, pad f/2) + skip add (IDAUp.forward dla_dcn.py:419-425).

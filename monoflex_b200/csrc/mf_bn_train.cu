@@ -9,7 +9,7 @@
 //             bn_bwd_apply_kernel   dx = scale * (g - mean(g) - xhat * mean(g * xhat))
 // x is the raw conv output, y the activated output kept from the forward (its sign gives the ReLU / leaky mask).
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -277,7 +277,7 @@ __global__ void bn_bwd_sums_kernel(const double* __restrict__ sums, int C, float
   if (dgamma != nullptr) { dbeta[c] = s; dgamma[c] = sx; }
 }
 
-// ------------------------------------------------------------------------------------------------ launchers
+// ------------------------------------------------------------------------------------------------ launch geometry
 static int bn_grid(long long M, int C, long long& rows_per_cta, int& threads, size_t& smem) {
   const int CV = C / 8;
   threads = 256;
@@ -295,17 +295,25 @@ static int bn_grid(long long M, int C, long long& rows_per_cta, int& threads, si
   rows_per_cta = (rows_per_cta + group - 1) / group * group;
   return static_cast<int>((M + rows_per_cta - 1) / rows_per_cta);
 }
-size_t bn_train_workspace_floats(long long M, int C) {
+
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+size_t mf_bn_train_workspace(long long M, int C) {
   long long rpc; int th; size_t sm;
   const int ncta = bn_grid(M, C, rpc, th, sm);
-  return ncta < 0 ? 0 : static_cast<size_t>(ncta) * 2 * C + 2 * static_cast<size_t>(C);
+  return sizeof(float) * (ncta < 0 ? 0 : static_cast<size_t>(ncta) * 2 * C + 2 * static_cast<size_t>(C));
 }
 
-int launch_bn_train_forward(const __half* x, int x_ld, long long M, int C, const float* gamma, const float* beta, float eps,
-                            float momentum, int abs_gamma, float* running_mean, float* running_var, const __half* res,
-                            int res_ld, int act, __half* y, int y_ld, float* mean, float* rstd, float* scale, float* shift,
-                            float* workspace, cudaStream_t st) {
+int mf_bn_train_forward(const void* x, int x_ld, long long M, int C, const float* gamma, const float* beta, float eps,
+                        float momentum, int abs_gamma, float* running_mean, float* running_var, const void* res, int res_ld,
+                        int act, void* y, int y_ld, float* mean, float* rstd, float* scale, float* shift, float* workspace,
+                        void* stream) {
   if (C % 8 || x_ld % 8 || y_ld % 8 || (res && res_ld % 8) || C > 2048 || M < 1) { set_error("bn_train_forward: bad shape (C=%d)", C); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
   long long rpc; int th; size_t sm;
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0) { set_error("bn_train_forward: C=%d too wide", C); return -1; }
@@ -319,7 +327,7 @@ int launch_bn_train_forward(const __half* x, int x_ld, long long M, int C, const
   (void)launch_k(bn_partial_kernel<false>, dim3(ncta), dim3(th), sm, st, x, x_ld, static_cast<const __half*>(nullptr), 0,
                  static_cast<const __half*>(nullptr), 0, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), M,
                  C, 0, rpc, 1, workspace);
-  bn_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, M, x, gamma, beta, eps, momentum, abs_gamma,
+  bn_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, M, static_cast<const __half*>(x), gamma, beta, eps, momentum, abs_gamma,
                                                       running_mean, running_var, mean, rstd, scale, shift);
   const long long n = M * (C / 8);
   (void)launch_k(bn_apply_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_ld,
@@ -327,13 +335,14 @@ int launch_bn_train_forward(const __half* x, int x_ld, long long M, int C, const
   return check_cuda(cudaGetLastError(), "bn_train_forward");
 }
 
-int launch_bn_train_backward(const __half* x, int x_ld, const __half* dy, int dy_ld, const __half* y, int y_ld, long long M, int C,
-                             const float* mean, const float* rstd, const float* scale, int act, __half* dx, int dx_ld,
-                             __half* dres, int dres_ld, float* dgamma, float* dbeta, float* workspace, cudaStream_t st) {
+int mf_bn_train_backward(const void* x, int x_ld, const void* dy, int dy_ld, const void* y, int y_ld, long long M, int C,
+                         const float* mean, const float* rstd, const float* scale, int act, void* dx, int dx_ld, void* dres,
+                         int dres_ld, float* dgamma, float* dbeta, float* workspace, void* stream) {
   if (C % 8 || x_ld % 8 || dy_ld % 8 || y_ld % 8 || dx_ld % 8 || (dres && dres_ld % 8) || C > 2048 || M < 1) {
     set_error("bn_train_backward: bad shape (C=%d)", C);
     return -1;
   }
+  const cudaStream_t st = MF_STREAM(stream);
   long long rpc; int th; size_t sm;
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_train_backward: C=%d too wide", C); return -1; }
@@ -348,9 +357,10 @@ int launch_bn_train_backward(const __half* x, int x_ld, const __half* dy, int dy
   return check_cuda(cudaGetLastError(), "bn_train_backward");
 }
 
-// ---- SyncBatchNorm halves (see above). sums: double [2][C] device buffer the host all-reduces between the two calls.
-int launch_bn_sync_forward_stats(const __half* x, int x_ld, long long M, int C, float* workspace, double* sums, cudaStream_t st) {
+// SyncBatchNorm halves (see above). sums: double [2][C] device buffer the host all-reduces between the two calls.
+int mf_bn_sync_forward_stats(const void* x, int x_ld, long long M, int C, float* workspace, double* sums, void* stream) {
   if (C % 8 || x_ld % 8 || C > 2048 || M < 1) { set_error("bn_sync_forward_stats: bad shape (C=%d)", C); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
   long long rpc; int th; size_t sm;
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_sync_forward_stats: C=%d too wide", C); return -1; }
@@ -366,11 +376,13 @@ int launch_bn_sync_forward_stats(const __half* x, int x_ld, long long M, int C, 
   bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, sums);
   return check_cuda(cudaGetLastError(), "bn_sync_forward_stats");
 }
-int launch_bn_sync_forward_apply(const __half* x, int x_ld, long long M, int C, const double* sums, double count, const float* gamma,
-                                 const float* beta, float eps, float momentum, int abs_gamma, float* running_mean,
-                                 float* running_var, const __half* res, int res_ld, int act, __half* y, int y_ld, float* mean,
-                                 float* rstd, float* scale, float* shift, cudaStream_t st) {
+
+int mf_bn_sync_forward_apply(const void* x, int x_ld, long long M, int C, const double* sums, double count, const float* gamma,
+                             const float* beta, float eps, float momentum, int abs_gamma, float* running_mean, float* running_var,
+                             const void* res, int res_ld, int act, void* y, int y_ld, float* mean, float* rstd, float* scale,
+                             float* shift, void* stream) {
   if (C % 8 || x_ld % 8 || y_ld % 8 || (res && res_ld % 8) || count < 1.0) { set_error("bn_sync_forward_apply: bad shape"); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
   bn_finalize_sums_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, count, gamma, beta, eps, momentum, abs_gamma, running_mean,
                                                            running_var, mean, rstd, scale, shift);
   const long long n = M * (C / 8);
@@ -378,10 +390,12 @@ int launch_bn_sync_forward_apply(const __half* x, int x_ld, long long M, int C, 
                  static_cast<const float*>(scale), static_cast<const float*>(shift), res, res_ld, act, y, y_ld, M, C);
   return check_cuda(cudaGetLastError(), "bn_sync_forward_apply");
 }
-int launch_bn_sync_backward_stats(const __half* x, int x_ld, const __half* dy, int dy_ld, const __half* y, int y_ld, long long M,
-                                  int C, const float* mean, const float* rstd, int act, float* workspace, double* sums,
-                                  float* dgamma, float* dbeta, cudaStream_t st) {
+
+int mf_bn_sync_backward_stats(const void* x, int x_ld, const void* dy, int dy_ld, const void* y, int y_ld, long long M, int C,
+                              const float* mean, const float* rstd, int act, float* workspace, double* sums, float* dgamma,
+                              float* dbeta, void* stream) {
   if (C % 8 || x_ld % 8 || dy_ld % 8 || y_ld % 8 || C > 2048 || M < 1) { set_error("bn_sync_backward_stats: bad shape"); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
   long long rpc; int th; size_t sm;
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_sync_backward_stats: C=%d too wide", C); return -1; }
@@ -391,13 +405,15 @@ int launch_bn_sync_backward_stats(const __half* x, int x_ld, const __half* dy, i
   bn_bwd_sums_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, nullptr, nullptr, dgamma, dbeta);      // local parameter gradients
   return check_cuda(cudaGetLastError(), "bn_sync_backward_stats");
 }
-int launch_bn_sync_backward_apply(const __half* x, int x_ld, const __half* dy, int dy_ld, const __half* y, int y_ld, long long M,
-                                  int C, const float* mean, const float* rstd, const float* scale, const double* sums, double count,
-                                  int act, __half* dx, int dx_ld, __half* dres, int dres_ld, float* workspace, cudaStream_t st) {
+
+int mf_bn_sync_backward_apply(const void* x, int x_ld, const void* dy, int dy_ld, const void* y, int y_ld, long long M, int C,
+                              const float* mean, const float* rstd, const float* scale, const double* sums, double count, int act,
+                              void* dx, int dx_ld, void* dres, int dres_ld, float* workspace, void* stream) {
   if (C % 8 || x_ld % 8 || dy_ld % 8 || y_ld % 8 || dx_ld % 8 || (dres && dres_ld % 8) || count < 1.0) {
     set_error("bn_sync_backward_apply: bad shape");
     return -1;
   }
+  const cudaStream_t st = MF_STREAM(stream);
   float* fs = workspace;                                            // [2][C] float copies of the global sums
   bn_bwd_sums_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, fs, fs + C, nullptr, nullptr);
   const long long n = M * (C / 8);
@@ -407,4 +423,4 @@ int launch_bn_sync_backward_apply(const __half* x, int x_ld, const __half* dy, i
   return check_cuda(cudaGetLastError(), "bn_sync_backward_apply");
 }
 
-}  // namespace mf
+}  // extern "C"

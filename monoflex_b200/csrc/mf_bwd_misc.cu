@@ -13,7 +13,7 @@
 //   interleave2x2       dX[b, 2i+py, 2j+px] = part[py][px][b, i, j]: recombines the four parity sub-convolutions of a
 //                       stride-2 convolution's data gradient (monoflex_b200/backward.py::conv2d_dgrad_stride2).
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -63,14 +63,6 @@ __global__ void __launch_bounds__(256) maxpool2_bwd_kernel(const __half* __restr
   }
 #pragma unroll
   for (int q = 0; q < 4; ++q) *reinterpret_cast<uint4*>(dx + rows[q] * dx_ld + cv * 8) = bm_pack8(o[q]);
-}
-int launch_maxpool2_bwd(const __half* x, const __half* dy, __half* dx, int B, int H, int W, int C, int x_ld, int dy_ld,
-                        int dx_ld, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || dy_ld % 8 || dx_ld % 8 || H % 2 || W % 2) { set_error("maxpool2_bwd: bad shape"); return -1; }
-  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
-  (void)launch_k(maxpool2_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, dy, dx, B, H, W, C, x_ld,
-                 dy_ld, dx_ld);
-  return check_cuda(cudaGetLastError(), "maxpool2_bwd");
 }
 
 // ---------------------------------------------------------------- depth-wise ConvTranspose2d backward: data
@@ -192,32 +184,7 @@ static int upsample_slabs(long long npix, long long& per) {
   per = (npix + ns - 1) / ns;
   return static_cast<int>((npix + per - 1) / per);
 }
-size_t upsample_bwd_workspace_floats(int B, int Hi, int Wi, int C, int f) {
-  long long per;
-  const int ns = upsample_slabs(static_cast<long long>(B) * Hi * Wi, per);
-  return static_cast<size_t>(ns) * 4 * f * f * C;
-}
 // w / dw: fp32 [k*k, C] tap-major (the layout mf_upsample_add_nhwc_f16 takes)
-int launch_upsample_bwd(const __half* x, const float* w, const __half* dy, __half* dx, float* dw, int B, int Hi, int Wi, int C,
-                        int f, int x_ld, int dy_ld, int dx_ld, float* workspace, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || dy_ld % 8 || dx_ld % 8 || f < 1 || f > 8) { set_error("upsample_bwd: bad shape"); return -1; }
-  const long long npix = static_cast<long long>(B) * Hi * Wi;
-  if (dx != nullptr) {
-    const long long n = npix * (C / 8);
-    (void)launch_k(upsample_bwd_dx_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, dy, w, dx, B, Hi, Wi, C,
-                   f, dy_ld, dx_ld);
-  }
-  if (dw != nullptr) {
-    long long per;
-    const int ns = upsample_slabs(npix, per);
-    const int taps = 4 * f * f, CV = C / 8;
-    (void)launch_k(upsample_bwd_dw_kernel, dim3((CV + 7) / 8, ns, (taps + UPW_TAPS - 1) / UPW_TAPS), dim3(256), 0, st, x, dy,
-                   workspace, B, Hi, Wi, C, f, x_ld, dy_ld, per);
-    const long long n = static_cast<long long>(taps) * C;
-    slab_reduce_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(workspace, dw, n, ns);
-  }
-  return check_cuda(cudaGetLastError(), "upsample_bwd");
-}
 
 // ---------------------------------------------------------------- sigmoid_hm backward (fp32, any layout)
 __global__ void sigmoid_clamp_bwd_kernel(const float* __restrict__ y, const float* __restrict__ dy, float* __restrict__ dx,
@@ -226,10 +193,6 @@ __global__ void sigmoid_clamp_bwd_kernel(const float* __restrict__ y, const floa
   if (i >= n) return;
   const float s = y[i];
   dx[i] = (s > 1e-4f && s < 1.f - 1e-4f) ? dy[i] * s * (1.f - s) : 0.f;      // where the clamp bound, the gradient is cut
-}
-int launch_sigmoid_clamp_bwd(const float* y, const float* dy, float* dx, long long n, cudaStream_t st) {
-  (void)launch_k(sigmoid_clamp_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, y, dy, dx, n);
-  return check_cuda(cudaGetLastError(), "sigmoid_clamp_bwd");
 }
 
 // ---------------------------------------------------------------- column sum of an [M, C] fp16 matrix
@@ -266,21 +229,6 @@ static int colsum_grid(long long M, long long& rpc) {
   if (n < 1) n = 1;
   rpc = (M + n - 1) / n;
   return static_cast<int>((M + rpc - 1) / rpc);
-}
-size_t column_sum_workspace_floats(long long M, int C) {
-  long long rpc;
-  return static_cast<size_t>(colsum_grid(M, rpc)) * C;
-}
-int launch_column_sum(const __half* x, int x_ld, long long M, int C, float* out, float* workspace, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || C > 2048 || M < 1) { set_error("column_sum: bad shape"); return -1; }
-  long long rpc;
-  const int ncta = colsum_grid(M, rpc);
-  const int RL = 256 / (C / 8);
-  if (RL < 1) { set_error("column_sum: C too wide"); return -1; }
-  (void)launch_k(column_sum_partial_kernel, dim3(ncta), dim3(256), static_cast<size_t>(RL) * C * sizeof(float), st, x, x_ld, M, C,
-                 rpc, workspace);
-  slab_reduce_kernel<<<(C + 255) / 256, 256, 0, st>>>(workspace, out, C, ncta);
-  return check_cuda(cudaGetLastError(), "column_sum");
 }
 
 // ---------------------------------------------------------------- edge-fusion gather backward
@@ -320,13 +268,6 @@ __global__ void edge_gather_bwd_kernel(const __half* __restrict__ d_ea, const __
 #pragma unroll
     for (int h = 0; h < 4; ++h) atomicAdd(dst + h, __floats2half2_rn(g[2 * h] * wts[q], g[2 * h + 1] * wts[q]));
   }
-}
-int launch_edge_gather_bwd(const __half* d_ea, const __half* d_eb, int ch_a, int ch_b, const long long* edge_idx, __half* d_feat,
-                           int feat_ld, int B, int H, int W, int K, int out_w, int out_h, cudaStream_t st) {
-  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
-  (void)launch_k(edge_gather_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, d_ea, d_eb, ch_a, ch_b,
-                 edge_idx, d_feat, feat_ld, B, H, W, K, out_w, out_h);
-  return check_cuda(cudaGetLastError(), "edge_gather_bwd");
 }
 
 // ---------------------------------------------------------------- edge_head_add backward (detector_predictor.py:155-158)
@@ -400,17 +341,6 @@ __global__ void __launch_bounds__(256) edge_head_add_bwd_kernel(const __half* __
     if (s != 0.f) atomicAdd(dbias + threadIdx.x, s);
   }
 }
-int launch_edge_head_add_bwd(const __half* t, const float* w, int n_out, const long long* edge_idx, const long long* edge_len,
-                             const float* d_out, int out_ctot, int out_ch0, __half* d_t, float* dw, float* dbias, int B, int K,
-                             int H, int W, cudaStream_t st) {
-  if (check_cuda(cudaMemsetAsync(dw, 0, sizeof(float) * n_out * 256, st), "edge_head_add_bwd memset")) return -1;
-  if (check_cuda(cudaMemsetAsync(dbias, 0, sizeof(float) * n_out, st), "edge_head_add_bwd memset")) return -1;
-  if (n_out < 1 || n_out > 4) { set_error("edge_head_add_bwd: n_out %d (1..4 supported)", n_out); return -1; }
-  const int blocks = (B * K + 63) / 64;                          // 8 warps x 8 positions per CTA
-  (void)launch_k(edge_head_add_bwd_kernel<4>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, t, w, n_out,
-                 edge_idx, edge_len, d_out, out_ctot, out_ch0, d_t, dw, dbias, B, K, H, W);
-  return check_cuda(cudaGetLastError(), "edge_head_add_bwd");
-}
 
 // ---------------------------------------------------------------- dst[r, 0:C] += src[r, 0:C] (gradient accumulation)
 __global__ void __launch_bounds__(256) add_rows_kernel(__half* __restrict__ dst, int dst_ld, const __half* __restrict__ src,
@@ -426,12 +356,6 @@ __global__ void __launch_bounds__(256) add_rows_kernel(__half* __restrict__ dst,
 #pragma unroll
   for (int e = 0; e < 8; ++e) a[e] += b[e];
   *reinterpret_cast<uint4*>(dst + row * dst_ld + cv * 8) = bm_pack8(a);
-}
-int launch_add_rows(__half* dst, int dst_ld, const __half* src, int src_ld, long long M, int C, cudaStream_t st) {
-  if (C % 8 || dst_ld % 8 || src_ld % 8) { set_error("add_rows: bad shape"); return -1; }
-  const long long n = M * (C / 8);
-  (void)launch_k(add_rows_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, dst, dst_ld, src, src_ld, M, C);
-  return check_cuda(cudaGetLastError(), "add_rows");
 }
 
 // ---------------------------------------------------------------- 2x2 parity interleave
@@ -456,13 +380,110 @@ __global__ void __launch_bounds__(256) interleave2x2_kernel(const __half* __rest
   *reinterpret_cast<uint4*>(out + (base + 2 * Wh) * out_ld + cv * 8) = __ldg(reinterpret_cast<const uint4*>(p10 + src));
   *reinterpret_cast<uint4*>(out + (base + 2 * Wh + 1) * out_ld + cv * 8) = __ldg(reinterpret_cast<const uint4*>(p11 + src));
 }
-int launch_interleave2x2(const __half* p00, const __half* p01, const __half* p10, const __half* p11, int part_ld, __half* out,
-                         int out_ld, int B, int Hh, int Wh, int C, cudaStream_t st) {
+
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_maxpool2_bwd_nhwc_f16(const void* x, const void* dy, void* dx, int B, int H, int W, int C, int x_ld, int dy_ld, int dx_ld,
+                             void* stream) {
+  if (C % 8 || x_ld % 8 || dy_ld % 8 || dx_ld % 8 || H % 2 || W % 2) { set_error("maxpool2_bwd: bad shape"); return -1; }
+  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
+  (void)launch_k(maxpool2_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), x, dy, dx, B,
+                 H, W, C, x_ld, dy_ld, dx_ld);
+  return check_cuda(cudaGetLastError(), "maxpool2_bwd");
+}
+
+size_t mf_upsample_bwd_workspace(int B, int Hi, int Wi, int C, int f) {
+  long long per;
+  const int ns = upsample_slabs(static_cast<long long>(B) * Hi * Wi, per);
+  return sizeof(float) * (static_cast<size_t>(ns) * 4 * f * f * C);
+}
+
+int mf_upsample_bwd_nhwc_f16(const void* x, const float* w_taps, const void* dy, void* dx, float* dw_taps, int B, int Hi, int Wi,
+                             int C, int f, int x_ld, int dy_ld, int dx_ld, float* workspace, void* stream) {
+  if (C % 8 || x_ld % 8 || dy_ld % 8 || dx_ld % 8 || f < 1 || f > 8) { set_error("upsample_bwd: bad shape"); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
+  const long long npix = static_cast<long long>(B) * Hi * Wi;
+  if (dx != nullptr) {
+    const long long n = npix * (C / 8);
+    (void)launch_k(upsample_bwd_dx_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, dy, w_taps, dx, B, Hi,
+                   Wi, C, f, dy_ld, dx_ld);
+  }
+  if (dw_taps != nullptr) {
+    long long per;
+    const int ns = upsample_slabs(npix, per);
+    const int taps = 4 * f * f, CV = C / 8;
+    (void)launch_k(upsample_bwd_dw_kernel, dim3((CV + 7) / 8, ns, (taps + UPW_TAPS - 1) / UPW_TAPS), dim3(256), 0, st, x, dy,
+                   workspace, B, Hi, Wi, C, f, x_ld, dy_ld, per);
+    const long long n = static_cast<long long>(taps) * C;
+    slab_reduce_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(workspace, dw_taps, n, ns);
+  }
+  return check_cuda(cudaGetLastError(), "upsample_bwd");
+}
+
+int mf_sigmoid_clamp_bwd(const float* y, const float* dy, float* dx, long long n, void* stream) {
+  (void)launch_k(sigmoid_clamp_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), y, dy, dx,
+                 n);
+  return check_cuda(cudaGetLastError(), "sigmoid_clamp_bwd");
+}
+
+size_t mf_column_sum_workspace(long long M, int C) {
+  long long rpc;
+  return sizeof(float) * (static_cast<size_t>(colsum_grid(M, rpc)) * C);
+}
+
+int mf_column_sum_nhwc_f16(const void* x, int x_ld, long long M, int C, float* out, float* workspace, void* stream) {
+  if (C % 8 || x_ld % 8 || C > 2048 || M < 1) { set_error("column_sum: bad shape"); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
+  long long rpc;
+  const int ncta = colsum_grid(M, rpc);
+  const int RL = 256 / (C / 8);
+  if (RL < 1) { set_error("column_sum: C too wide"); return -1; }
+  (void)launch_k(column_sum_partial_kernel, dim3(ncta), dim3(256), static_cast<size_t>(RL) * C * sizeof(float), st, x, x_ld, M, C,
+                 rpc, workspace);
+  slab_reduce_kernel<<<(C + 255) / 256, 256, 0, st>>>(workspace, out, C, ncta);
+  return check_cuda(cudaGetLastError(), "column_sum");
+}
+
+int mf_edge_gather_bwd(const void* d_ea, const void* d_eb, int ch_a, int ch_b, const long long* edge_idx, void* d_feat, int feat_ld,
+                       int B, int H, int W, int K, int out_w, int out_h, void* stream) {
+  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
+  (void)launch_k(edge_gather_bwd_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), d_ea, d_eb,
+                 ch_a, ch_b, edge_idx, d_feat, feat_ld, B, H, W, K, out_w, out_h);
+  return check_cuda(cudaGetLastError(), "edge_gather_bwd");
+}
+
+int mf_edge_head_add_bwd(const void* t, const float* w, int n_out, const long long* edge_idx, const long long* edge_len,
+                         const float* d_out, int out_ctot, int out_ch0, void* d_t, float* dw, float* dbias, int B, int K, int H,
+                         int W, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (check_cuda(cudaMemsetAsync(dw, 0, sizeof(float) * n_out * 256, st), "edge_head_add_bwd memset")) return -1;
+  if (check_cuda(cudaMemsetAsync(dbias, 0, sizeof(float) * n_out, st), "edge_head_add_bwd memset")) return -1;
+  if (n_out < 1 || n_out > 4) { set_error("edge_head_add_bwd: n_out %d (1..4 supported)", n_out); return -1; }
+  const int blocks = (B * K + 63) / 64;                          // 8 warps x 8 positions per CTA
+  (void)launch_k(edge_head_add_bwd_kernel<4>, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, t, w, n_out,
+                 edge_idx, edge_len, d_out, out_ctot, out_ch0, d_t, dw, dbias, B, K, H, W);
+  return check_cuda(cudaGetLastError(), "edge_head_add_bwd");
+}
+
+int mf_add_rows_f16(void* dst, int dst_ld, const void* src, int src_ld, long long M, int C, void* stream) {
+  if (C % 8 || dst_ld % 8 || src_ld % 8) { set_error("add_rows: bad shape"); return -1; }
+  const long long n = M * (C / 8);
+  (void)launch_k(add_rows_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), dst, dst_ld, src,
+                 src_ld, M, C);
+  return check_cuda(cudaGetLastError(), "add_rows");
+}
+
+int mf_interleave2x2_nhwc_f16(const void* p00, const void* p01, const void* p10, const void* p11, int part_ld, void* out, int out_ld,
+                              int B, int Hh, int Wh, int C, void* stream) {
   if (C % 8 || part_ld % 8 || out_ld % 8) { set_error("interleave2x2: bad shape"); return -1; }
   const long long n = static_cast<long long>(B) * Hh * Wh * (C / 8);
-  (void)launch_k(interleave2x2_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, p00, p01, p10, p11, part_ld,
-                 out, out_ld, B, Hh, Wh, C);
+  (void)launch_k(interleave2x2_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), p00, p01, p10,
+                 p11, part_ld, out, out_ld, B, Hh, Wh, C);
   return check_cuda(cudaGetLastError(), "interleave2x2");
 }
 
-}  // namespace mf
+}  // extern "C"

@@ -14,6 +14,9 @@ namespace mf {
 void set_error(const char* fmt, ...);
 int check_cuda(cudaError_t e, const char* what);
 
+// the C ABI passes the caller's cudaStream_t as void*
+#define MF_STREAM(s) reinterpret_cast<cudaStream_t>(s)
+
 // kernel<<<grid, block, smem, st>>>(args...) through cudaLaunchKernelEx, converting each argument to the kernel's parameter type
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {

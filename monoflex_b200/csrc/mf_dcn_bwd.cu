@@ -10,7 +10,7 @@
 //                     epilogue (ACT_OFFMASK), so its backward wants the pre-activation gradient. One row [32] fp32 per pixel:
 //                     18 offset gradients (dy, dx interleaved per tap), 9 mask pre-activation gradients, 5 zeros.
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -154,16 +154,25 @@ __global__ void __launch_bounds__(256) dcn_col2im_kernel(const __half* __restric
   }
 }
 
-int launch_dcn_sample_cols(const __half* x, int x_ld, const float* om, int om_ld, __half* cols, int B, int H, int W, int C,
-                           cudaStream_t st) {
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_dcn_sample_cols_nhwc_f16(const void* x, int x_ld, const float* om, int om_ld, void* cols, int B, int H, int W, int C,
+                                void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
   if (C % 8 || x_ld % 8 || om_ld < 27) { set_error("dcn_sample_cols: bad shape"); return -1; }
   const long long n = static_cast<long long>(B) * H * W * 9 * (C / 8);
   (void)launch_k(dcn_sample_cols_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_ld, om, om_ld, cols,
                  B, H, W, C);
   return check_cuda(cudaGetLastError(), "dcn_sample_cols");
 }
-int launch_dcn_col2im(const __half* x, int x_ld, const float* om, int om_ld, const __half* gcol, __half* dx, int dx_ld, float* dom,
-                      int B, int H, int W, int C, cudaStream_t st) {
+
+int mf_dcn_col2im_nhwc_f16(const void* x, int x_ld, const float* om, int om_ld, const void* gcol, void* dx, int dx_ld,
+                           float* dom, int B, int H, int W, int C, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
   if (C % 8 || x_ld % 8 || dx_ld % 8 || om_ld < 27) { set_error("dcn_col2im: bad shape"); return -1; }
   const int CV = C / 8;
   int L = 1;
@@ -175,4 +184,4 @@ int launch_dcn_col2im(const __half* x, int x_ld, const float* om, int om_ld, con
   return check_cuda(cudaGetLastError(), "dcn_col2im");
 }
 
-}  // namespace mf
+}  // extern "C"

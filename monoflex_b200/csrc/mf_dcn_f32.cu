@@ -16,7 +16,7 @@
 //                 partial sums per split go to the workspace and are reduced in a fixed order (deterministic);
 //             k4: bias gradient, one block per output channel.
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -345,7 +345,7 @@ __global__ void __launch_bounds__(256) dcn_f32_bias_grad_kernel(const float* __r
   }
 }
 
-// ------------------------------------------------------------------------------------------------ launchers
+// ------------------------------------------------------------------------------------------------ host helpers
 static int make_geom(DcnGeom& g, int B, int C, int H, int W, int Co, int kh, int kw, int sh, int sw, int ph, int pw, int dh,
                      int dw, int dg, const char* who) {
   if (dg < 1 || C % dg != 0) { set_error("%s: channels %d not divisible by deformable_group %d", who, C, dg); return -1; }
@@ -371,32 +371,41 @@ static int wgrad_splits(const DcnGeom& g) {
   return static_cast<int>(S);
 }
 
-int launch_dcn_v2_forward_f32(const float* x, const float* w, const float* bias, const float* off, const float* mask,
-                              float* y, int B, int Cin, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph,
-                              int pw, int dh, int dw, int dg, cudaStream_t st) {
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_dcn_v2_forward(const float* x, const float* w, const float* bias, const float* off, const float* mask, float* y,
+                      int B, int Cin, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh,
+                      int dw, int dg, void* workspace, size_t ws_bytes, void* stream) {
+  (void)workspace; (void)ws_bytes;
   DcnGeom g;
   if (make_geom(g, B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, "mf_dcn_v2_forward")) return -1;
   const long long HoWo = static_cast<long long>(g.Ho) * g.Wo;
   dim3 grid(static_cast<unsigned>((HoWo + TN - 1) / TN), static_cast<unsigned>((Cout + TM - 1) / TM), static_cast<unsigned>(B));
-  dcn_f32_forward_kernel<<<grid, 256, 0, st>>>(x, w, bias, off, mask, y, g);
+  dcn_f32_forward_kernel<<<grid, 256, 0, MF_STREAM(stream)>>>(x, w, bias, off, mask, y, g);
   return check_cuda(cudaGetLastError(), "dcn_v2_forward_f32");
 }
 
-size_t dcn_v2_backward_f32_workspace(int B, int Cin, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
-                                     int dh, int dw, int dg) {
+size_t mf_dcn_v2_backward_workspace(int B, int Cin, int H, int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw,
+                                    int dh, int dw, int dg) {
   DcnGeom g;
   if (make_geom(g, B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, "mf_dcn_v2_backward_workspace")) return 0;
   const size_t CT = static_cast<size_t>(Cin) * kh * kw, HoWo = static_cast<size_t>(g.Ho) * g.Wo;
   return sizeof(float) * (static_cast<size_t>(B) * CT * HoWo + static_cast<size_t>(wgrad_splits(g)) * Cout * CT);
 }
 
-int launch_dcn_v2_backward_f32(const float* x, const float* w, const float* off, const float* mask, const float* dy,
-                               float* gx, float* goff, float* gmask, float* gw, float* gb, int B, int Cin, int H, int W,
-                               int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int dg,
-                               void* workspace, size_t ws_bytes, cudaStream_t st) {
+int mf_dcn_v2_backward(const float* x, const float* w, const float* bias, const float* off, const float* mask,
+                       const float* dy, float* gx, float* goff, float* gmask, float* gw, float* gb, int B, int Cin, int H,
+                       int W, int Cout, int kh, int kw, int sh, int sw, int ph, int pw, int dh, int dw, int dg,
+                       void* workspace, size_t ws_bytes, void* stream) {
+  (void)bias;
+  const cudaStream_t st = MF_STREAM(stream);
   DcnGeom g;
   if (make_geom(g, B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg, "mf_dcn_v2_backward")) return -1;
-  const size_t need = dcn_v2_backward_f32_workspace(B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
+  const size_t need = mf_dcn_v2_backward_workspace(B, Cin, H, W, Cout, kh, kw, sh, sw, ph, pw, dh, dw, dg);
   if (workspace == nullptr || ws_bytes < need) {
     set_error("mf_dcn_v2_backward: workspace of %zu bytes required (got %zu); query mf_dcn_v2_backward_workspace()", need,
               ws_bytes);
@@ -421,4 +430,14 @@ int launch_dcn_v2_backward_f32(const float* x, const float* w, const float* off,
   return check_cuda(cudaGetLastError(), "dcn_v2_backward_f32");
 }
 
-}  // namespace mf
+// dcn_v2_psroi_pooling_forward / _backward of the reference's _ext: MonoFlex never instantiates them
+int mf_dcn_v2_psroi_pooling_forward(void) {
+  set_error("dcn_v2_psroi_pooling_forward: not built (dead code for MonoFlex, SURVEY 2.2 K6)");
+  return -2;
+}
+int mf_dcn_v2_psroi_pooling_backward(void) {
+  set_error("dcn_v2_psroi_pooling_backward: not built (dead code for MonoFlex, SURVEY 2.2 K6)");
+  return -2;
+}
+
+}  // extern "C"

@@ -9,10 +9,17 @@
 // Stage 2: one CTA per image merges C*K candidates, gathers the 50 regression channels of each survivor and decodes.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 #include <math_constants.h>
 
 namespace mf {
+
+// OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
+enum {
+  MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,
+  MF_DEPTH_KEYPOINTS_AVG = 5, MF_DEPTH_KEYPOINTS_CENTER = 6, MF_DEPTH_KEYPOINTS_02 = 7, MF_DEPTH_KEYPOINTS_13 = 8,
+  MF_DEPTH_MODES = 9
+};
 
 #define MF_DECODE_SLABS 8
 static constexpr int S1_THREADS = 1024;
@@ -244,11 +251,6 @@ __global__ void nms_hm_kernel(const float* __restrict__ hm, float* __restrict__ 
     }
   out[i] = (mx == v) ? v : v * 0.f;                   // heat * 0 keeps the sign of a negative pixel, like the reference
 }
-int launch_nms_hm(const float* hm, float* out, int planes, int H, int W, cudaStream_t st) {
-  const long long n = static_cast<long long>(planes) * H * W;
-  (void)launch_k(nms_hm_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, hm, out, H, W, n);
-  return check_cuda(cudaGetLastError(), "nms_hm");
-}
 
 struct DecodeParams {
   const float* s1_score;  // [B, C, K]
@@ -270,7 +272,7 @@ struct DecodeParams {
   float* pois;            // [B, K, R]
   float* result;          // [B, K, 14]
   int* count;             // [B]
-  // OUTPUT_DEPTH estimator (MF_DEPTH_* in mf_launch.h) and, for the oracle, the ground truth of every image:
+  // OUTPUT_DEPTH estimator (MF_DEPTH_* above) and, for the oracle, the ground truth of every image:
   // gt [B, G, 7] = (valid, class, x1, y1, x2, y2, z)
   int depth_mode;
   const float* gt;
@@ -507,11 +509,23 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   r[6] = dh; r[7] = dw; r[8] = dl; r[9] = lx; r[10] = ly; r[11] = depth; r[12] = roty; r[13] = conf;
 }
 
-int launch_decode(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
-                  const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                  int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores, long long* inds,
-                  float* clses, float* ys, float* xs, float* pois, float* result, int* count, float* depth_err,
-                  float* proj, int* min_unc, cudaStream_t st) {
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_nms_hm(const float* hm, float* out, int planes, int H, int W, void* stream) {
+  const long long n = static_cast<long long>(planes) * H * W;
+  (void)launch_k(nms_hm_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), hm, out, H, W, n);
+  return check_cuda(cudaGetLastError(), "nms_hm");
+}
+
+int mf_decode_detections(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
+                         const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
+                         int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores,
+                         long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
+                         float* depth_err, float* proj, int* min_unc, void* stream) {
   if (depth_mode < 0 || depth_mode >= MF_DEPTH_MODES) {
     set_error("decode: depth_mode %d is not one of the %d OUTPUT_DEPTH estimators", depth_mode, MF_DEPTH_MODES);
     return -1;
@@ -561,7 +575,7 @@ int launch_decode(const float* heat, const float* reg, const float* calib, const
       return -1;
     s1_attr = s1_smem;
   }
-  (void)launch_k(nms_topk_stage1_kernel, dim3(B * C * S), dim3(S1_THREADS), s1_smem, st, heat, H, W, K, apply_sigmoid, S, s1_score, s1_idx);
+  (void)launch_k(nms_topk_stage1_kernel, dim3(B * C * S), dim3(S1_THREADS), s1_smem, MF_STREAM(stream), heat, H, W, K, apply_sigmoid, S, s1_score, s1_idx);
   if (check_cuda(cudaGetLastError(), "nms_topk_stage1")) return -1;
   DecodeParams p;
   p.s1_score = s1_score; p.s1_idx = s1_idx; p.reg = reg; p.calib = calib; p.pad = pad; p.size = size;
@@ -569,8 +583,8 @@ int launch_decode(const float* heat, const float* reg, const float* calib, const
   p.scores = scores; p.inds = inds; p.clses = clses; p.ys = ys; p.xs = xs; p.pois = pois; p.result = result;
   p.count = count;
   p.depth_mode = depth_mode; p.gt = gt; p.G = G; p.depth_err = depth_err; p.proj = proj; p.min_unc = min_unc;
-  (void)launch_k(topk_decode_stage2_kernel, dim3(B), dim3(S2_THREADS), 0, st, p);
+  (void)launch_k(topk_decode_stage2_kernel, dim3(B), dim3(S2_THREADS), 0, MF_STREAM(stream), p);
   return check_cuda(cudaGetLastError(), "topk_decode_stage2");
 }
 
-}  // namespace mf
+}  // extern "C"

@@ -1,7 +1,7 @@
 // HBM-bound layout / pooling / up-sampling / edge-fusion kernels: coalesced 16-byte vector accesses on NHWC fp16.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -31,14 +31,8 @@ __global__ void pack_image_kernel(const float* __restrict__ x, __half* __restric
   for (int c = 0; c < 8; ++c) f[c] = c < C ? __ldg(x + (b * C + c) * HW + pix) : 0.f;
   *reinterpret_cast<uint4*>(y + i * 8) = pack8(f);
 }
-int launch_pack_image(const float* x, __half* y, int B, int C, int H, int W, cudaStream_t st) {
-  if (C > 8) { set_error("pack_image: C=%d > 8", C); return -1; }
-  const long long n = static_cast<long long>(B) * H * W;
-  (void)launch_k(pack_image_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, C, static_cast<long long>(H) * W);
-  return check_cuda(cudaGetLastError(), "pack_image");
-}
 
-// ---------------------------------------------------------------- generic NCHW fp32 <-> NHWC fp16 (tile transpose)
+// ---------------------------------------------------------------- generic NCHW fp32 -> NHWC fp16 (tile transpose)
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __half* __restrict__ y, int C, int HW, int y_ld) {
   __shared__ float tile[32][33];
   const int b = blockIdx.z, p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
@@ -51,48 +45,6 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __half* __restr
     const int pp = p0 + i, c = c0 + threadIdx.x;
     if (pp < HW && c < C) y[(static_cast<long long>(b) * HW + pp) * y_ld + c] = __float2half_rn(tile[threadIdx.x][i]);
   }
-}
-int launch_nchw_to_nhwc(const float* x, __half* y, int B, int C, int HW, int y_ld, cudaStream_t st) {
-  dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  (void)launch_k(nchw_to_nhwc_kernel, dim3(grid), dim3(block), 0, st, x, y, C, HW, y_ld);
-  return check_cuda(cudaGetLastError(), "nchw_to_nhwc");
-}
-__global__ void nhwc_to_nchw_kernel(const __half* __restrict__ x, float* __restrict__ y, int C, int HW, int x_ld) {
-  __shared__ float tile[32][33];
-  const int b = blockIdx.z, p0 = blockIdx.x * 32, c0 = blockIdx.y * 32;
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int pp = p0 + i, c = c0 + threadIdx.x;
-    tile[i][threadIdx.x] = (pp < HW && c < C) ? __half2float(x[(static_cast<long long>(b) * HW + pp) * x_ld + c]) : 0.f;
-  }
-  __syncthreads();
-  for (int i = threadIdx.y; i < 32; i += blockDim.y) {
-    const int c = c0 + i, pp = p0 + threadIdx.x;
-    if (c < C && pp < HW) y[(static_cast<long long>(b) * C + c) * HW + pp] = tile[threadIdx.x][i];
-  }
-}
-int launch_nhwc_to_nchw(const __half* x, float* y, int B, int C, int HW, int x_ld, cudaStream_t st) {
-  dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
-  (void)launch_k(nhwc_to_nchw_kernel, dim3(grid), dim3(block), 0, st, x, y, C, HW, x_ld);
-  return check_cuda(cudaGetLastError(), "nhwc_to_nchw");
-}
-
-// offset [B,18,H,W] + mask [B,9,H,W] (fp32 NCHW, reference _ext layout) -> [B*H*W, 32] fp32 rows
-__global__ void pack_offmask_kernel(const float* __restrict__ off, const float* __restrict__ mask, float* __restrict__ y,
-                                    int B, int HW) {
-  const long long i = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i >= static_cast<long long>(B) * HW * 32) return;
-  const int ch = static_cast<int>(i & 31);
-  const long long m = i >> 5;
-  const long long b = m / HW, pix = m - b * HW;
-  float v = 0.f;
-  if (ch < 18) v = off[(b * 18 + ch) * HW + pix];
-  else if (ch < 27) v = mask[(b * 9 + (ch - 18)) * HW + pix];
-  y[i] = v;
-}
-int launch_pack_offmask(const float* off, const float* mask, float* y, int B, int HW, cudaStream_t st) {
-  const long long n = static_cast<long long>(B) * HW * 32;
-  (void)launch_k(pack_offmask_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, off, mask, y, B, HW);
-  return check_cuda(cudaGetLastError(), "pack_offmask");
 }
 
 // ---------------------------------------------------------------- MaxPool2d(2) NHWC fp16 (dla_dcn.py:238)
@@ -121,12 +73,6 @@ __global__ void maxpool2_kernel(const __half* __restrict__ x, __half* __restrict
 #pragma unroll
   for (int e = 0; e < 4; ++e) ho[e] = __hmax2(__hmax2(ha[e], hb[e]), __hmax2(hc[e], hd[e]));
   *reinterpret_cast<uint4*>(y + pix * y_ld + cv * 8) = o;
-}
-int launch_maxpool2(const __half* x, __half* y, int B, int H, int W, int C, int x_ld, int y_ld, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || y_ld % 8 || H % 2 || W % 2) { set_error("maxpool2: bad shape"); return -1; }
-  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
-  (void)launch_k(maxpool2_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, H, W, C, x_ld, y_ld);
-  return check_cuda(cudaGetLastError(), "maxpool2");
 }
 
 // ---------------------------------------------------------------- depthwise ConvTranspose2d(k=2f, s=f, p=f/2) + skip add
@@ -243,20 +189,6 @@ upsample2_add_kernel(const __half* __restrict__ x, const float* __restrict__ w, 
     }
   }
 }
-int launch_upsample_add(const __half* x, const float* w, const __half* skip, __half* y, int B, int Hi, int Wi, int C,
-                        int f, int x_ld, int skip_ld, int y_ld, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || y_ld % 8 || (skip && skip_ld % 8) || f < 1) { set_error("upsample_add: bad shape"); return -1; }
-  if (f == 2) {
-    const long long n2 = static_cast<long long>(B) * (Hi + 1) * (Wi + 1) * (C / 8);
-    (void)launch_k(upsample2_add_kernel, dim3(static_cast<unsigned>((n2 + 255) / 256)), dim3(256), 0, st, x, w, skip, y, B, Hi, Wi, C, x_ld, skip_ld,
-                                                                                 y_ld);
-    return check_cuda(cudaGetLastError(), "upsample2_add");
-  }
-  const long long n = static_cast<long long>(B) * Hi * f * Wi * f * (C / 8);
-  (void)launch_k(upsample_add_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, w, skip, y, B, Hi, Wi, C, f, x_ld,
-                                                                               skip_ld, y_ld);
-  return check_cuda(cudaGetLastError(), "upsample_add");
-}
 
 // ---------------------------------------------------------------- edge fusion gather (detector_predictor.py:137-147)
 // F.grid_sample(bilinear, zeros padding, align_corners=True) of two 256-channel slices of the head feature map at the
@@ -304,13 +236,6 @@ __global__ void edge_gather_kernel(const __half* __restrict__ feat, int feat_ld,
   __half* dst = (which ? eb : ea) + (static_cast<long long>(b) * (K + 2) + pos) * 256 + cv * 8;
   *reinterpret_cast<uint4*>(dst) = pack8(acc);
 }
-int launch_edge_gather(const __half* feat, int feat_ld, int ch_a, int ch_b, const long long* edge_idx, __half* ea,
-                       __half* eb, int B, int H, int W, int K, int out_w, int out_h, cudaStream_t st) {
-  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
-  (void)launch_k(edge_gather_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, feat, feat_ld, ch_a, ch_b, edge_idx, ea, eb,
-                                                                              B, H, W, K, out_w, out_h);
-  return check_cuda(cudaGetLastError(), "edge_gather");
-}
 
 // byte mask [B*H*W] of the pixels edge_gather_kernel reads (the up-to-4 bilinear corners of every border position, computed
 // with the same fp32 round trip), so that the fused head stores hidden activations for those pixels only.
@@ -332,12 +257,6 @@ __global__ void edge_mask_kernel(const long long* __restrict__ edge_idx, unsigne
       const int yy = y0 + dy, xx = x0 + dx;
       if (yy >= 0 && yy < H && xx >= 0 && xx < W) mb[yy * W + xx] = 1;
     }
-}
-int launch_edge_mask(const long long* edge_idx, unsigned char* mask, int B, int K, int H, int W, int out_w, int out_h,
-                     cudaStream_t st) {
-  if (check_cuda(cudaMemsetAsync(mask, 0, static_cast<size_t>(B) * H * W, st), "edge_mask memset")) return -1;
-  (void)launch_k(edge_mask_kernel, dim3((B * K + 255) / 256), dim3(256), 0, st, edge_idx, mask, B, H, W, K, out_w, out_h);
-  return check_cuda(cudaGetLastError(), "edge_mask");
 }
 
 // final Conv1d(256 -> n_out, k=1) of one truncation branch + indexed add into an NCHW fp32 map
@@ -362,14 +281,6 @@ __global__ void edge_head_add_kernel(const __half* __restrict__ t, const float* 
     if (lane == 0) out[((static_cast<long long>(b) * out_ctot + out_ch0 + o) * H + ey) * W + ex] += s + bias[o];
   }
 }
-int launch_edge_head_add(const __half* t, const float* w, const float* bias, int n_out, const long long* edge_idx,
-                         const long long* edge_len, float* out, int out_ctot, int out_ch0, int B, int K, int H, int W,
-                         cudaStream_t st) {
-  const long long threads = static_cast<long long>(B) * K * 32;
-  (void)launch_k(edge_head_add_kernel, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, st, t, w, bias, n_out, edge_idx, edge_len,
-                                                                                     out, out_ctot, out_ch0, B, K, H, W);
-  return check_cuda(cudaGetLastError(), "edge_head_add");
-}
 
 // sigmoid_hm (model/layers/utils.py:39-43): x = clamp(sigmoid(x), 1e-4, 1-1e-4), in place
 __global__ void sigmoid_clamp_kernel(float* __restrict__ x, long long n) {
@@ -377,10 +288,6 @@ __global__ void sigmoid_clamp_kernel(float* __restrict__ x, long long n) {
   if (i >= n) return;
   const float s = 1.f / (1.f + expf(-x[i]));
   x[i] = fminf(fmaxf(s, 1e-4f), 1.f - 1e-4f);
-}
-int launch_sigmoid_clamp(float* x, long long n, cudaStream_t st) {
-  (void)launch_k(sigmoid_clamp_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, n);
-  return check_cuda(cudaGetLastError(), "sigmoid_clamp");
 }
 
 // ---------------------------------------------------------------- penalty-reduced focal loss (layers/focal_loss.py:35-55)
@@ -428,3 +335,81 @@ int launch_focal_loss(const float* pred, const float* tgt, long long n, float* o
 }
 
 }  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_pack_image(const float* x_nchw, void* y_nhwc8, int B, int C, int H, int W, void* stream) {
+  if (C > 8) { set_error("pack_image: C=%d > 8", C); return -1; }
+  const long long n = static_cast<long long>(B) * H * W;
+  (void)launch_k(pack_image_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), x_nchw, y_nhwc8,
+                 B, C, static_cast<long long>(H) * W);
+  return check_cuda(cudaGetLastError(), "pack_image");
+}
+
+int mf_nchw_f32_to_nhwc_f16(const float* x, void* y, int B, int C, int HW, int y_ld, void* stream) {
+  dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
+  (void)launch_k(nchw_to_nhwc_kernel, dim3(grid), dim3(block), 0, MF_STREAM(stream), x, y, C, HW, y_ld);
+  return check_cuda(cudaGetLastError(), "nchw_to_nhwc");
+}
+
+int mf_maxpool2_nhwc_f16(const void* x, void* y, int B, int H, int W, int C, int x_ld, int y_ld, void* stream) {
+  if (C % 8 || x_ld % 8 || y_ld % 8 || H % 2 || W % 2) { set_error("maxpool2: bad shape"); return -1; }
+  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
+  (void)launch_k(maxpool2_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), x, y, B, H, W, C,
+                 x_ld, y_ld);
+  return check_cuda(cudaGetLastError(), "maxpool2");
+}
+
+int mf_upsample_add_nhwc_f16(const void* x, const float* w_taps, const void* skip, void* y, int B, int Hi, int Wi, int C,
+                             int f, int x_ld, int skip_ld, int y_ld, void* stream) {
+  if (C % 8 || x_ld % 8 || y_ld % 8 || (skip && skip_ld % 8) || f < 1) { set_error("upsample_add: bad shape"); return -1; }
+  const cudaStream_t st = MF_STREAM(stream);
+  if (f == 2) {
+    const long long n2 = static_cast<long long>(B) * (Hi + 1) * (Wi + 1) * (C / 8);
+    (void)launch_k(upsample2_add_kernel, dim3(static_cast<unsigned>((n2 + 255) / 256)), dim3(256), 0, st, x, w_taps, skip, y, B, Hi,
+                   Wi, C, x_ld, skip_ld, y_ld);
+    return check_cuda(cudaGetLastError(), "upsample2_add");
+  }
+  const long long n = static_cast<long long>(B) * Hi * f * Wi * f * (C / 8);
+  (void)launch_k(upsample_add_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, w_taps, skip, y, B, Hi, Wi,
+                 C, f, x_ld, skip_ld, y_ld);
+  return check_cuda(cudaGetLastError(), "upsample_add");
+}
+
+int mf_edge_gather(const void* feat, int feat_ld, int ch_a, int ch_b, const long long* edge_idx, void* ea, void* eb, int B,
+                   int H, int W, int K, int out_w, int out_h, void* stream) {
+  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
+  (void)launch_k(edge_gather_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), feat, feat_ld,
+                 ch_a, ch_b, edge_idx, ea, eb, B, H, W, K, out_w, out_h);
+  return check_cuda(cudaGetLastError(), "edge_gather");
+}
+
+int mf_edge_mask(const long long* edge_idx, unsigned char* mask, int B, int K, int H, int W, int out_w, int out_h,
+                 void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (check_cuda(cudaMemsetAsync(mask, 0, static_cast<size_t>(B) * H * W, st), "edge_mask memset")) return -1;
+  (void)launch_k(edge_mask_kernel, dim3((B * K + 255) / 256), dim3(256), 0, st, edge_idx, mask, B, H, W, K, out_w, out_h);
+  return check_cuda(cudaGetLastError(), "edge_mask");
+}
+
+int mf_edge_head_add(const void* t, const float* w, const float* bias, int n_out, const long long* edge_idx,
+                     const long long* edge_len, float* out, int out_ctot, int out_ch0, int B, int K, int H, int W,
+                     void* stream) {
+  const long long threads = static_cast<long long>(B) * K * 32;
+  (void)launch_k(edge_head_add_kernel, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, MF_STREAM(stream), t, w,
+                 bias, n_out, edge_idx, edge_len, out, out_ctot, out_ch0, B, K, H, W);
+  return check_cuda(cudaGetLastError(), "edge_head_add");
+}
+
+int mf_sigmoid_clamp(float* x, long long n, void* stream) {
+  (void)launch_k(sigmoid_clamp_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream), x, n);
+  return check_cuda(cudaGetLastError(), "sigmoid_clamp");
+}
+
+int mf_focal_loss_forward(const float* pred, const float* target, long long n, float* out2, void* stream) {
+  return launch_focal_loss(pred, target, n, out2, MF_STREAM(stream));
+}
+
+}  // extern "C"

@@ -12,6 +12,7 @@
 //               and after the second one adds the 1x1 bias and writes the fp32 NCHW `cls` / `reg` channels of that branch.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
 #include <cstring>
 
 namespace mf {
@@ -211,13 +212,18 @@ static void* driver_fn(const char* name) {
   return ptr;
 }
 
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
 // x: features [B*H*W, x_ld] fp16 (Cin channels used); w3: packed 3x3 weights [nbranch*256, 9*Cin]; w2: packed 1x1 weights
 // [nbranch*32, 256]; hid: [M, hid_ld] fp16 buffer receiving the hidden activations of the branches with hid_col >= 0 at the
 // pixels hid_mask flags.
-int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* w3, const __half* w2,
-                      const float* scale, const float* shift, const float* bias2, int nbranch, float* const* out,
-                      const int* out_ctot, const int* out_nch, const int* hid_col, __half* hid, int hid_ld,
-                      const unsigned char* hid_mask, cudaStream_t st) {
+int mf_head_fused(const void* x, int x_ld, int B, int H, int W, int Cin, const void* w3, const void* w2, const float* scale,
+                  const float* shift, const float* bias2, int nbranch, void* const* out, const int* out_ctot, const int* out_nch,
+                  const int* hid_col, void* hid, int hid_ld, const unsigned char* hid_mask, void* stream) {
   static PFN_encTiledH enc = reinterpret_cast<PFN_encTiledH>(driver_fn("cuTensorMapEncodeTiled"));
   static PFN_encIm2colH enc2 = reinterpret_cast<PFN_encIm2colH>(driver_fn("cuTensorMapEncodeIm2col"));
   if (!enc || !enc2) { set_error("head_fused: tensor-map driver entry points unavailable"); return -1; }
@@ -232,9 +238,9 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
   memset(&p, 0, sizeof(p));
   p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.M = B * H * W; p.nkb = 9 * Cin / 64; p.nbranch = nbranch;
   p.scale = scale; p.shift = shift; p.bias2 = bias2;
-  p.hid = hid; p.hid_ld = hid_ld; p.hid_mask = hid_mask;
+  p.hid = static_cast<__half*>(hid); p.hid_ld = hid_ld; p.hid_mask = hid_mask;
   for (int i = 0; i < nbranch; ++i) {
-    p.out[i] = out[i]; p.out_ctot[i] = out_ctot[i]; p.out_nch[i] = out_nch[i]; p.hid_col[i] = hid_col[i];
+    p.out[i] = static_cast<float*>(out[i]); p.out_ctot[i] = out_ctot[i]; p.out_nch[i] = out_nch[i]; p.hid_col[i] = hid_col[i];
     if (out_nch[i] > 32) { set_error("head_fused: branch %d has %d > 32 output channels", i, out_nch[i]); return -1; }
   }
   CUtensorMap tx, tw, tw2;
@@ -243,7 +249,7 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     cuuint64_t gstr[3] = {static_cast<cuuint64_t>(x_ld) * 2, static_cast<cuuint64_t>(x_ld) * 2 * W, static_cast<cuuint64_t>(x_ld) * 2 * W * H};
     int lower[2] = {-1, -1}, upper[2] = {-1, -1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    if (enc2(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(x), gdim, gstr, lower, upper, 64, HBM, estr,
+    if (enc2(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), gdim, gstr, lower, upper, 64, HBM, estr,
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) { set_error("head_fused: im2col map failed"); return -1; }
   }
@@ -270,7 +276,7 @@ int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, c
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const int ntm = (p.M + HBM - 1) / HBM;
   const int grid = ntm < nsm ? ntm : nsm;
-  return check_cuda(launch_k(head_fused_kernel, dim3(grid), dim3(H_THREADS), H_SMEM, st, tx, tw, tw2, p), "head_fused launch");
+  return check_cuda(launch_k(head_fused_kernel, dim3(grid), dim3(H_THREADS), H_SMEM, MF_STREAM(stream), tx, tw, tw2, p), "head_fused launch");
 }
 
-}  // namespace mf
+}  // extern "C"

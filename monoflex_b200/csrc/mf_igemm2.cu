@@ -26,6 +26,7 @@
 // the ring. At 64 columns a gathered A element feeds only 64 x 3 MACs, so the gather bounds the kernel, not the tensor pipe.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -1005,20 +1006,12 @@ __global__ void head2_reduce_kernel(const float* __restrict__ part, const float*
                          : reg + (static_cast<long long>(b) * nreg + (ch - ncls)) * HW + pix;
   *reinterpret_cast<float4*>(dst) = s;
 }
-int launch_head2_reduce(const float* part, const float* bias, float* cls, float* reg, int B, int ncls, int nreg, int HW,
-                        cudaStream_t st) {
-  if (HW % 4 != 0) { set_error("head2_reduce: H*W must be a multiple of 4"); return -1; }
-  const long long n4 = static_cast<long long>(B) * (ncls + nreg) * HW / 4;
-  (void)launch_k(head2_reduce_kernel, dim3(static_cast<unsigned>((n4 + 255) / 256)), dim3(256), 0, st, part, bias, cls, reg, B, ncls,
-                 nreg, HW);
-  return check_cuda(cudaGetLastError(), "head2_reduce");
-}
 
 int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, int mode, cudaStream_t st) {
   PFN_encodeTiled2 enc = encode_fn();
   if (!enc) return -1;
   // HEAD2 tiles: 128 columns (a 256-column tile would need 128 accumulator registers per consumer thread)
-  const int bn = p.h2_w != nullptr ? 128 : igemm_block_n(p.Cout);
+  const int bn = p.h2_w != nullptr ? 128 : mf_conv_block_n(p.Cout);
   const bool store_ok = p.out_mode == OUT_F16_NHWC && bn >= 64 && (reinterpret_cast<uintptr_t>(p.y) & 15) == 0 && p.y_ld % 8 == 0;
   if (p.act == ACT_OFFMASK) { set_error("igemm2: the offset/mask convolution runs in mf_offset_conv.cu"); return -1; }
   if (n_pad % bn != 0 || k_pad % BK != 0 || k_pad < p.nkb * BK) {
@@ -1149,3 +1142,17 @@ int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, 
 }
 
 }  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_head2_reduce(const float* part, const float* bias, float* cls, float* reg, int B, int ncls, int nreg, int HW, void* stream) {
+  if (HW % 4 != 0) { set_error("head2_reduce: H*W must be a multiple of 4"); return -1; }
+  const long long n4 = static_cast<long long>(B) * (ncls + nreg) * HW / 4;
+  (void)launch_k(head2_reduce_kernel, dim3(static_cast<unsigned>((n4 + 255) / 256)), dim3(256), 0, MF_STREAM(stream), part, bias,
+                 cls, reg, B, ncls, nreg, HW);
+  return check_cuda(cudaGetLastError(), "head2_reduce");
+}
+
+}  // extern "C"

@@ -11,7 +11,8 @@
 //                          |dy| <= ry, sigma = (2 r + 1) / 6 per axis, evaluated in double and rounded to fp32 like numpy's
 //                          float64 -> float32 store. One thread per heat-map element, <= 40 objects per image.
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -42,15 +43,6 @@ __global__ void __launch_bounds__(256) preprocess_u8_kernel(const unsigned char*
     const int oc = k.to_bgr ? 2 - c : c;
     out[(static_cast<long long>(b) * 3 + oc) * HW + pix] = t;
   }
-}
-int launch_preprocess_u8(const unsigned char* const* src, const int* hw, const int* flip, int B, int H, int W,
-                         const float* mean3, const float* std3, int to_bgr, float* out, cudaStream_t st) {
-  NormConsts k;
-  for (int c = 0; c < 3; ++c) { k.mean[c] = mean3[c]; k.stdv[c] = std3[c]; }
-  k.to_bgr = to_bgr;
-  const long long n = static_cast<long long>(B) * H * W;
-  (void)launch_k(preprocess_u8_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, src, hw, flip, B, H, W, k, out);
-  return check_cuda(cudaGetLastError(), "preprocess_u8");
 }
 
 // obj: int32 [B][max_objs][6] = (valid, cls, cx, cy, rx, ry); hm: fp32 [B][ncls][H][W]
@@ -86,3 +78,24 @@ int launch_draw_heatmap(const int* obj, int B, int max_objs, int ncls, int H, in
 }
 
 }  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_preprocess_images_u8(const void* const* src, const int* hw, const int* flip, int B, int H, int W, const float* mean3,
+                            const float* std3, int to_bgr, float* out, void* stream) {
+  NormConsts k;
+  for (int c = 0; c < 3; ++c) { k.mean[c] = mean3[c]; k.stdv[c] = std3[c]; }
+  k.to_bgr = to_bgr;
+  const long long n = static_cast<long long>(B) * H * W;
+  (void)launch_k(preprocess_u8_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, MF_STREAM(stream),
+                 reinterpret_cast<const unsigned char* const*>(src), hw, flip, B, H, W, k, out);
+  return check_cuda(cudaGetLastError(), "preprocess_u8");
+}
+
+int mf_draw_heatmaps(const int* obj6, int B, int max_objs, int ncls, int H, int W, float* hm, void* stream) {
+  return launch_draw_heatmap(obj6, B, max_objs, ncls, H, W, hm, MF_STREAM(stream));
+}
+
+}  // extern "C"

@@ -2,6 +2,7 @@
 // grid-stride, over [N, 8, 3] float32 corner tables. The IoU itself is mf_iou3d.cuh, shared with the fused loss.
 #include "mf_common.cuh"
 #include "mf_iou3d.cuh"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 namespace {
@@ -38,7 +39,7 @@ int mf_iou3d_corners(const float* pred, const float* target, long long n, float*
   }
   const long long blocks = (n + 255) / 256;
   (void)mf::launch_k(mf::iou3d_corners_kernel, dim3(static_cast<unsigned>(blocks < 4096 ? blocks : 4096)), dim3(256), 0,
-                     reinterpret_cast<cudaStream_t>(stream), pred, target, n, out);
+                     MF_STREAM(stream), pred, target, n, out);
   return mf::check_cuda(cudaGetLastError(), "iou3d_corners");
 }
 

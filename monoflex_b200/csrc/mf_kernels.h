@@ -1,4 +1,5 @@
-// Internal launcher declarations shared by the .cu files of libmonoflex_b200.so (not part of the public C ABI).
+// Internal declarations shared by the .cu files of libmonoflex_b200.so (not part of the public C ABI, which is
+// include/monoflex_b200.h): the implicit-GEMM parameters and the launchers one file calls in another.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -59,24 +60,17 @@ struct IgemmParams {
   const unsigned char* h2_mask;
 };
 
-int igemm_block_n(int cout);
-int launch_conv_wgrad_narrow(const __half* x, int x_ld, int B, int H, int W, const __half* dy, int dy_ld, int k, float* dw,
-                             cudaStream_t st);
-int launch_head2_reduce(const float* part, const float* bias, float* cls, float* reg, int B, int ncls, int nreg, int HW,
-                        cudaStream_t st);
 int launch_igemm2(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, int mode, cudaStream_t st);
-int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar, const __half* wp, int n_pad, int k_pad,
-                     int kh, int kw, int stride, int pad, int Cout, const float* scale, const float* shift, int act,
-                     int out_planar, int out_npar, __half* y, int y_ld, cudaStream_t st, int in_mode = 0, int split_out = 0,
-                     int y_lo = 0);
-int launch_head_fused(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* w3, const __half* w2,
-                      const float* scale, const float* shift, const float* bias2, int nbranch, float* const* out,
-                      const int* out_ctot, const int* out_nch, const int* hid_col, __half* hid, int hid_ld,
-                      const unsigned char* hid_mask, cudaStream_t st);
-int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* dy, int dy_ld, int Cout, int kh,
-                      int kw, int stride, int pad_h, int pad_w, float* dw, cudaStream_t st);
 int launch_offset_conv(const __half* x, int x_ld, int x_lo, int B, int H, int W, int Cin, const __half* wp, int n_pad, int k_pad,
                        const float* scale, const float* shift, float* y, int y_ld, bool pair, cudaStream_t st);
 int launch_simt_gemm(const IgemmParams& p, const __half* wp, int n_pad, int k_pad, int mode, cudaStream_t st);
+int launch_conv_wgrad_narrow(const __half* x, int x_ld, int B, int H, int W, const __half* dy, int dy_ld, int k, float* dw,
+                             cudaStream_t st);
+int launch_draw_heatmap(const int* obj, int B, int max_objs, int ncls, int H, int W, float* hm, cudaStream_t st);
+int launch_focal_loss(const float* pred, const float* tgt, long long n, float* out2, cudaStream_t st);
+int launch_focal_loss_backward(const float* pred, const float* tgt, long long n, const float* scale, float* grad,
+                               cudaStream_t st);
+
+#define MF_LOSS_OBJ_COLS 64   /* floats per (image, object slot) row of the packed label table (mf_loss.cu, mf_targets.cu) */
 
 }  // namespace mf

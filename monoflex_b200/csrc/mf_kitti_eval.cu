@@ -500,14 +500,14 @@ size_t mf_kitti_eval_workspace(int n_gt, int n_dt, int ncls) {
 int mf_kitti_pack_results(const float* rows, int n, double* out, void* stream) {
   if (n < 0) { set_error("mf_kitti_pack_results: n = %d", n); return -1; }
   if (n == 0) return 0;
-  pack_results_kernel<<<(n + 127) / 128, 128, 0, static_cast<cudaStream_t>(stream)>>>(rows, n, out);
+  pack_results_kernel<<<(n + 127) / 128, 128, 0, MF_STREAM(stream)>>>(rows, n, out);
   return check_cuda(cudaGetLastError(), "kitti_pack_results");
 }
 
 int mf_kitti_eval_overlaps(const double* gt, const int* gt_off, const double* dt, const int* dt_off,
                            const long long* pair_off, int n_img, long long n_pair, double* overlaps, void* stream) {
   if (n_img < 1 || n_pair < 0) { set_error("mf_kitti_eval_overlaps: %d images, %lld pairs", n_img, n_pair); return -1; }
-  overlaps_kernel<<<n_img, 128, 0, static_cast<cudaStream_t>(stream)>>>(gt, gt_off, dt, dt_off, pair_off, n_pair, overlaps);
+  overlaps_kernel<<<n_img, 128, 0, MF_STREAM(stream)>>>(gt, gt_off, dt, dt_off, pair_off, n_pair, overlaps);
   return check_cuda(cudaGetLastError(), "kitti_eval_overlaps");
 }
 
@@ -527,7 +527,7 @@ int mf_kitti_eval_statistics(const double* gt, const int* gt_off, const double* 
     set_error("mf_kitti_eval_statistics: workspace of %zu bytes, %zu needed", ws_bytes, L.total);
     return -1;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  cudaStream_t st = MF_STREAM(stream);
   char* ws = static_cast<char*>(workspace);
   StatArgs a;
   a.gt = gt; a.gt_off = gt_off; a.dt = dt; a.dt_off = dt_off; a.pair_off = pair_off; a.ov = overlaps;
@@ -568,9 +568,9 @@ int mf_kitti_eval_ap(const void* workspace, int n_gt, int n_dt, int ncls, double
   if (ncls < 1 || ncls > MAX_CLS || workspace == nullptr) { set_error("mf_kitti_eval_ap: %d classes", ncls); return -1; }
   const Layout L = layout(n_gt, n_dt, ncls);
   const char* ws = static_cast<const char*>(workspace);
-  ap_kernel<<<1, 18 * ncls, 0, static_cast<cudaStream_t>(stream)>>>(reinterpret_cast<const double*>(ws + L.pr),
-                                                                      reinterpret_cast<const int*>(ws + L.nthr),
-                                                                      reinterpret_cast<const int*>(ws + L.aos), ncls, out);
+  ap_kernel<<<1, 18 * ncls, 0, MF_STREAM(stream)>>>(reinterpret_cast<const double*>(ws + L.pr),
+                                                     reinterpret_cast<const int*>(ws + L.nthr),
+                                                     reinterpret_cast<const int*>(ws + L.aos), ncls, out);
   return check_cuda(cudaGetLastError(), "kitti_eval_ap");
 }
 

@@ -18,7 +18,10 @@
 
 #include "mf_common.cuh"
 #include "mf_iou3d.cuh"
-#include "mf_launch.h"
+#include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
+
+#define MF_LOSS_WS_FLOATS 96  /* floats of the loss workspace: 24 fixed slots + f_u of up to 64 images */
 
 namespace mf {
 
@@ -413,7 +416,7 @@ __global__ void __launch_bounds__(128) loss_backward_kernel(const float* __restr
 
 __global__ void loss_hm_scale_kernel(float* ws, const float* gw) { ws[WS_HMG] = ws[WS_HM] * gw[0]; }
 
-// ------------------------------------------------------------------------------------------------ launchers
+// ------------------------------------------------------------------------------------------------ host helpers
 static int fill_cfg(LossCfg& c, const float* weights11, const float* dim_mean9, int B, int M, int H, int W, int C) {
   if (C != 50) { set_error("loss: the regression map must have the 50 channels of runs/monoflex.yaml:27-28 (got %d)", C); return -1; }
   if (B < 1 || B > 64 || M < 1) { set_error("loss: batch %d (1..64) / max objects %d not supported", B, M); return -1; }
@@ -426,9 +429,18 @@ static int fill_cfg(LossCfg& c, const float* weights11, const float* dim_mean9, 
   return 0;
 }
 
-int launch_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
-                        const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                        float* out48, float* ws96, cudaStream_t st) {
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_loss_obj_cols(void) { return MF_LOSS_OBJ_COLS; }
+
+int mf_loss_forward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
+                    const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
+                    float* out48, float* ws96, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
   LossCfg c;
   if (fill_cfg(c, weights11, dim_mean9, B, M, H, W, C)) return -1;
   float* focal2 = ws96 + 20;                                               // [20] loss sum, [21] num_pos
@@ -438,9 +450,10 @@ int launch_loss_forward(const float* pred_cls, const float* hm, const float* pre
   return check_cuda(cudaGetLastError(), "loss_forward");
 }
 
-int launch_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
-                         const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
-                         const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, cudaStream_t st) {
+int mf_loss_backward(const float* pred_cls, const float* hm, const float* pred_reg, const float* obj, const float* img,
+                     const float* weights11, const float* dim_mean9, int B, int ncls, int M, int H, int W, int C,
+                     const float* ws96, const float* grad_losses11, float* grad_cls, float* grad_reg, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
   LossCfg c;
   if (fill_cfg(c, weights11, dim_mean9, B, M, H, W, C)) return -1;
   const long long n_reg = static_cast<long long>(B) * C * H * W, n_cls = static_cast<long long>(B) * ncls * H * W;
@@ -459,4 +472,4 @@ int launch_loss_backward(const float* pred_cls, const float* hm, const float* pr
   return 0;
 }
 
-}  // namespace mf
+}  // extern "C"

@@ -24,6 +24,7 @@
 //     fp32 (first half + second half) before scale/shift.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
 #include <cstring>
 
 namespace mf {
@@ -274,7 +275,7 @@ static int rows_conv_launch(int grid, int smem, cudaStream_t st, const CUtensorM
 //              from the lo planes: rows [0, Cout) = [W_hi ; W_hi], rows [Cout, 2 Cout) = [W_lo ; 0].
 // So every A operand is read by ONE MMA (N = 2 Cout): the same three products A_hi W_hi + A_lo W_hi + A_hi W_lo over the
 // same resident row segments.
-int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar, const __half* wp, int n_pad, int k_pad,
+static int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar, const __half* wp, int n_pad, int k_pad,
                      int kh, int kw, int stride, int pad, int Cout, const float* scale, const float* shift, int act,
                      int out_planar, int out_npar, __half* y, int y_ld, cudaStream_t st, int in_mode, int split_out,
                      int y_lo) {
@@ -419,3 +420,25 @@ int launch_rows_conv(const __half* x, int B, int H, int W, int Cin, int in_npar,
 }
 
 }  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_conv2d_rows_f16(const void* x, int B, int H, int W, int Cin, int in_npar, const void* w_packed, int n_pad, int k_pad,
+                       int kh, int kw, int stride, int pad, int Cout, const float* scale, const float* shift, int act,
+                       int out_planar, int out_npar, void* y, int y_ld, void* stream) {
+  return launch_rows_conv(static_cast<const __half*>(x), B, H, W, Cin, in_npar, static_cast<const __half*>(w_packed), n_pad,
+                          k_pad, kh, kw, stride, pad, Cout, scale, shift, act, out_planar, out_npar, static_cast<__half*>(y),
+                          y_ld, MF_STREAM(stream), 0, 0, 0);
+}
+
+int mf_conv2d_rows_f16x2(const void* x, int B, int H, int W, int Cin, int in_npar, int in_mode, const void* w_packed, int n_pad,
+                         int k_pad, int kh, int kw, int stride, int pad, int Cout, const float* scale, const float* shift, int act,
+                         int out_planar, int out_npar, void* y, int y_ld, int y_lo, void* stream) {
+  return launch_rows_conv(static_cast<const __half*>(x), B, H, W, Cin, in_npar, static_cast<const __half*>(w_packed), n_pad,
+                          k_pad, kh, kw, stride, pad, Cout, scale, shift, act, out_planar, out_npar, static_cast<__half*>(y),
+                          y_ld, MF_STREAM(stream), in_mode, 1, y_lo);
+}
+
+}  // extern "C"

@@ -18,7 +18,7 @@
 // descriptor's matrix-base-offset field (bits 49-51) = 0 (v = 0) or (start >> 7) & 7 (v = 1). A wrong variant gives wrong
 // numbers, never an out-of-range address: every row read lies in the 80-row buffer (tests/test_gpu_offset_conv.py).
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -56,11 +56,6 @@ __global__ void __launch_bounds__(256) mn_major_selftest_kernel(const __half* __
     const int row = wg * 64 + 16 * w + (l >> 2) + 8 * ((i >> 1) & 1), col = 8 * (i >> 2) + 2 * (l & 3) + (i & 1);
     d_mn[row * N + col] = d[i];
   }
-}
-
-int launch_mn_major_selftest(const __half* a_km, const __half* b_kn, float* d_mn, cudaStream_t st) {
-  mn_major_selftest_kernel<<<1, 256, 0, st>>>(a_km, b_kn, d_mn);
-  return check_cuda(cudaGetLastError(), "mn_major_selftest");
 }
 
 __global__ void __launch_bounds__(128) sw128_shift_selftest_kernel(const __half* __restrict__ a_rows,
@@ -102,9 +97,22 @@ __global__ void __launch_bounds__(128) sw128_shift_selftest_kernel(const __half*
     }
 }
 
-int launch_sw128_shift_selftest(const __half* a_rows, const __half* b_rows, float* d, cudaStream_t st) {
-  sw128_shift_selftest_kernel<<<1, 128, 0, st>>>(a_rows, b_rows, d);
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_selftest_mn_major(const void* a_km, const void* b_kn, float* d_mn, void* stream) {
+  mn_major_selftest_kernel<<<1, 256, 0, MF_STREAM(stream)>>>(static_cast<const __half*>(a_km), static_cast<const __half*>(b_kn),
+                                                                 d_mn);
+  return check_cuda(cudaGetLastError(), "mn_major_selftest");
+}
+
+int mf_selftest_sw128_shift(const void* a_rows, const void* b_rows, float* d, void* stream) {
+  sw128_shift_selftest_kernel<<<1, 128, 0, MF_STREAM(stream)>>>(static_cast<const __half*>(a_rows),
+                                                                    static_cast<const __half*>(b_rows), d);
   return check_cuda(cudaGetLastError(), "sw128_shift_selftest");
 }
 
-}  // namespace mf
+}  // extern "C"

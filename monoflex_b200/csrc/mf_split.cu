@@ -8,7 +8,7 @@
 // plumbing between those GEMMs: image packing, max-pool, depth-wise up-sampling + add, the edge-fusion gather / final add.
 #include "mf_common.cuh"
 #include "mf_kernels.h"
-#include "mf_launch.h"
+#include "../../include/monoflex_b200.h"
 
 namespace mf {
 
@@ -57,17 +57,6 @@ __global__ void pack_conv_weight_split_kernel(const float* __restrict__ w, int C
   }
   out[i] = r;
 }
-int launch_pack_conv_weight_split(const float* w, int Cout, int Cin, int kh, int kw, int n_pad, int k_pad, __half* out,
-                                  cudaStream_t st) {
-  const int cw = Cin < 64 ? Cin : 64;
-  if (Cin % cw != 0 || 64 % cw != 0 || k_pad < 3 * kh * kw * Cin || n_pad < Cout) {
-    set_error("pack_conv_weight_split: Cin=%d must be a multiple of 64 or one of 8/16/32; k_pad >= 3*taps*Cin", Cin);
-    return -1;
-  }
-  const long long n = static_cast<long long>(n_pad) * k_pad;
-  pack_conv_weight_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, st>>>(w, Cout, Cin, kh * kw, cw, n_pad, k_pad, out);
-  return check_cuda(cudaGetLastError(), "pack_conv_weight_split");
-}
 
 // ---------------------------------------------------------------- image: NCHW fp32 [B,3,H,W] -> [B*H*W, 16] fp16 rows
 // channels [hi(3) | lo(3) | hi(3) | 0 x 7]: the 7x7 stem then is an ORDINARY 16-channel convolution whose per-tap weights are
@@ -93,13 +82,6 @@ __global__ void pack_image_split_kernel(const float* __restrict__ x, __half* __r
   dst[0] = *reinterpret_cast<uint4*>(&o[0]);
   dst[1] = *reinterpret_cast<uint4*>(&o[8]);
 }
-int launch_pack_image_split(const float* x, __half* y, int B, int C, int H, int W, cudaStream_t st) {
-  if (C > 3) { set_error("pack_image_split: C=%d > 3", C); return -1; }
-  const long long n = static_cast<long long>(B) * H * W;
-  (void)launch_k(pack_image_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, C,
-                 static_cast<long long>(H) * W);
-  return check_cuda(cudaGetLastError(), "pack_image_split");
-}
 
 // image -> ONE 16-byte-pixel plane [hi3 | lo3 | 0 0] for the row-segment stem kernel (mf_rows.cu, in_mode 1)
 __global__ void pack_image_pair8_kernel(const float* __restrict__ x, __half* __restrict__ y, int B, int C, long long HW) {
@@ -119,13 +101,6 @@ __global__ void pack_image_pair8_kernel(const float* __restrict__ x, __half* __r
     }
   }
   *reinterpret_cast<uint4*>(y + i * 8) = *reinterpret_cast<uint4*>(&o[0]);
-}
-int launch_pack_image_pair8(const float* x, __half* y, int B, int C, int H, int W, cudaStream_t st) {
-  if (C > 3) { set_error("pack_image_pair8: C=%d > 3", C); return -1; }
-  const long long n = static_cast<long long>(B) * H * W;
-  (void)launch_k(pack_image_pair8_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, C,
-                 static_cast<long long>(H) * W);
-  return check_cuda(cudaGetLastError(), "pack_image_pair8");
 }
 
 // ---------------------------------------------------------------- MaxPool2d(2) on hi/lo rows
@@ -149,14 +124,6 @@ __global__ void maxpool2_split_kernel(const __half* __restrict__ x, int x_lo, __
 #pragma unroll
   for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaxf(a[e], bq[e]), fmaxf(c[e], d[e]));
   st8_split(y + pix * y_ld + cv * 8, y_lo, o);       // hi + lo of one input is exactly representable again: lossless
-}
-int launch_maxpool2_split(const __half* x, int x_lo, __half* y, int y_lo, int B, int H, int W, int C, int x_ld, int y_ld,
-                          cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || y_ld % 8 || x_lo % 8 || y_lo % 8 || H % 2 || W % 2) { set_error("maxpool2_split: bad shape"); return -1; }
-  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
-  (void)launch_k(maxpool2_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_lo, y, y_lo, B, H, W, C,
-                 x_ld, y_ld);
-  return check_cuda(cudaGetLastError(), "maxpool2_split");
 }
 
 // ---------------------------------------------------------------- depthwise ConvTranspose2d(k=2f, s=f, p=f/2) + skip add
@@ -230,17 +197,6 @@ __global__ void upsample_add_split_kernel(const __half* __restrict__ x, int x_lo
   for (int e = 0; e < 8; ++e) acc[e] += up[e];
   st8_split(y + pix * y_ld + cv * 8, y_lo, acc);
 }
-int launch_upsample_add_split(const __half* x, int x_lo, const float* w, const __half* skip, int skip_lo, __half* y, int y_lo,
-                              int B, int Hi, int Wi, int C, int f, int x_ld, int skip_ld, int y_ld, cudaStream_t st) {
-  if (C % 8 || x_ld % 8 || y_ld % 8 || (skip && skip_ld % 8) || x_lo % 8 || y_lo % 8 || (skip && skip_lo % 8) || f < 1) {
-    set_error("upsample_add_split: bad shape");
-    return -1;
-  }
-  const long long n = static_cast<long long>(B) * Hi * f * Wi * f * (C / 8);
-  (void)launch_k(upsample_add_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_lo, w, skip, skip_lo,
-                 y, y_lo, B, Hi, Wi, C, f, x_ld, skip_ld, y_ld);
-  return check_cuda(cudaGetLastError(), "upsample_add_split");
-}
 
 // ---------------------------------------------------------------- edge fusion gather on hi/lo rows (see edge_gather_kernel)
 // outputs ea / eb: [B, K+2, 512] rows = [hi 256 | lo 256]
@@ -286,13 +242,6 @@ __global__ void edge_gather_split_kernel(const __half* __restrict__ feat, int fe
   corner(y1, x1, wy1 * wx1);
   st8_split((which ? eb : ea) + (static_cast<long long>(b) * (K + 2) + pos) * 512 + cv * 8, 256, acc);
 }
-int launch_edge_gather_split(const __half* feat, int feat_ld, int feat_lo, int ch_a, int ch_b, const long long* edge_idx,
-                             __half* ea, __half* eb, int B, int H, int W, int K, int out_w, int out_h, cudaStream_t st) {
-  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
-  (void)launch_k(edge_gather_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, feat, feat_ld, feat_lo, ch_a,
-                 ch_b, edge_idx, ea, eb, B, H, W, K, out_w, out_h);
-  return check_cuda(cudaGetLastError(), "edge_gather_split");
-}
 
 // final Conv1d(256 -> n_out, k=1) + indexed add, input rows [hi 256 | lo 256] with row stride t_ld (see edge_head_add_kernel)
 __global__ void edge_head_add_split_kernel(const __half* __restrict__ t, int t_ld, int t_lo, const float* __restrict__ w,
@@ -315,14 +264,6 @@ __global__ void edge_head_add_split_kernel(const __half* __restrict__ t, int t_l
     if (lane == 0) out[((static_cast<long long>(b) * out_ctot + out_ch0 + o) * H + ey) * W + ex] += s + bias[o];
   }
 }
-int launch_edge_head_add_split(const __half* t, int t_ld, int t_lo, const float* w, const float* bias, int n_out,
-                               const long long* edge_idx, const long long* edge_len, float* out, int out_ctot, int out_ch0, int B,
-                               int K, int H, int W, cudaStream_t st) {
-  const long long threads = static_cast<long long>(B) * K * 32;
-  (void)launch_k(edge_head_add_split_kernel, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, st, t, t_ld, t_lo, w, bias,
-                 n_out, edge_idx, edge_len, out, out_ctot, out_ch0, B, K, H, W);
-  return check_cuda(cudaGetLastError(), "edge_head_add_split");
-}
 
 // hi/lo rows -> fp32 NCHW (tests / feature-map export): y = float(hi) + float(lo)
 __global__ void split_to_nchw_kernel(const __half* __restrict__ x, int x_ld, int x_lo, float* __restrict__ y, int C, int HW) {
@@ -343,10 +284,89 @@ __global__ void split_to_nchw_kernel(const __half* __restrict__ x, int x_ld, int
     if (c < C && pp < HW) y[(static_cast<long long>(b) * C + c) * HW + pp] = tile[threadIdx.x][i];
   }
 }
-int launch_split_to_nchw(const __half* x, int x_ld, int x_lo, float* y, int B, int C, int HW, cudaStream_t st) {
+
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_pack_conv_weight_split(const float* w, int Cout, int Cin, int kh, int kw, int n_pad, int k_pad, void* out, void* stream) {
+  const int cw = Cin < 64 ? Cin : 64;
+  if (Cin % cw != 0 || 64 % cw != 0 || k_pad < 3 * kh * kw * Cin || n_pad < Cout) {
+    set_error("pack_conv_weight_split: Cin=%d must be a multiple of 64 or one of 8/16/32; k_pad >= 3*taps*Cin", Cin);
+    return -1;
+  }
+  const long long n = static_cast<long long>(n_pad) * k_pad;
+  pack_conv_weight_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, MF_STREAM(stream)>>>(w, Cout, Cin, kh * kw, cw, n_pad,
+                                                                                                k_pad, static_cast<__half*>(out));
+  return check_cuda(cudaGetLastError(), "pack_conv_weight_split");
+}
+
+int mf_pack_image_split(const float* x, void* y, int B, int C, int H, int W, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (C > 3) { set_error("pack_image_split: C=%d > 3", C); return -1; }
+  const long long n = static_cast<long long>(B) * H * W;
+  (void)launch_k(pack_image_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, C,
+                 static_cast<long long>(H) * W);
+  return check_cuda(cudaGetLastError(), "pack_image_split");
+}
+
+int mf_pack_image_pair8(const float* x, void* y, int B, int C, int H, int W, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (C > 3) { set_error("pack_image_pair8: C=%d > 3", C); return -1; }
+  const long long n = static_cast<long long>(B) * H * W;
+  (void)launch_k(pack_image_pair8_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, y, B, C,
+                 static_cast<long long>(H) * W);
+  return check_cuda(cudaGetLastError(), "pack_image_pair8");
+}
+
+int mf_maxpool2_split(const void* x, int x_lo, void* y, int y_lo, int B, int H, int W, int C, int x_ld, int y_ld, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (C % 8 || x_ld % 8 || y_ld % 8 || x_lo % 8 || y_lo % 8 || H % 2 || W % 2) { set_error("maxpool2_split: bad shape"); return -1; }
+  const long long n = static_cast<long long>(B) * (H / 2) * (W / 2) * (C / 8);
+  (void)launch_k(maxpool2_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_lo, y, y_lo, B, H, W, C,
+                 x_ld, y_ld);
+  return check_cuda(cudaGetLastError(), "maxpool2_split");
+}
+
+int mf_upsample_add_split(const void* x, int x_lo, const float* w, const void* skip, int skip_lo, void* y, int y_lo, int B,
+                          int Hi, int Wi, int C, int f, int x_ld, int skip_ld, int y_ld, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  if (C % 8 || x_ld % 8 || y_ld % 8 || (skip && skip_ld % 8) || x_lo % 8 || y_lo % 8 || (skip && skip_lo % 8) || f < 1) {
+    set_error("upsample_add_split: bad shape");
+    return -1;
+  }
+  const long long n = static_cast<long long>(B) * Hi * f * Wi * f * (C / 8);
+  (void)launch_k(upsample_add_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_lo, w, skip, skip_lo,
+                 y, y_lo, B, Hi, Wi, C, f, x_ld, skip_ld, y_ld);
+  return check_cuda(cudaGetLastError(), "upsample_add_split");
+}
+
+int mf_edge_gather_split(const void* feat, int feat_ld, int feat_lo, int ch_a, int ch_b, const long long* edge_idx, void* ea,
+                         void* eb, int B, int H, int W, int K, int out_w, int out_h, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  const long long n = static_cast<long long>(B) * (K + 2) * 32 * 2;
+  (void)launch_k(edge_gather_split_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, feat, feat_ld, feat_lo, ch_a,
+                 ch_b, edge_idx, ea, eb, B, H, W, K, out_w, out_h);
+  return check_cuda(cudaGetLastError(), "edge_gather_split");
+}
+
+int mf_edge_head_add_split(const void* t, int t_ld, int t_lo, const float* w, const float* bias, int n_out,
+                           const long long* edge_idx, const long long* edge_len, float* out, int out_ctot, int out_ch0, int B,
+                           int K, int H, int W, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
+  const long long threads = static_cast<long long>(B) * K * 32;
+  (void)launch_k(edge_head_add_split_kernel, dim3(static_cast<unsigned>((threads + 255) / 256)), dim3(256), 0, st, t, t_ld, t_lo, w, bias,
+                 n_out, edge_idx, edge_len, out, out_ctot, out_ch0, B, K, H, W);
+  return check_cuda(cudaGetLastError(), "edge_head_add_split");
+}
+
+int mf_split_to_nchw_f32(const void* x, int x_ld, int x_lo, float* y, int B, int C, int HW, void* stream) {
+  const cudaStream_t st = MF_STREAM(stream);
   dim3 grid((HW + 31) / 32, (C + 31) / 32, B), block(32, 8);
   (void)launch_k(split_to_nchw_kernel, dim3(grid), dim3(block), 0, st, x, x_ld, x_lo, y, C, HW);
   return check_cuda(cudaGetLastError(), "split_to_nchw");
 }
 
-}  // namespace mf
+}  // extern "C"

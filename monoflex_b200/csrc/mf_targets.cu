@@ -14,7 +14,7 @@
 // The reference raises for an edge object with two non-zero radii (kitti.py:457) and for an outside object whose 2D box centre
 // lies outside the image (approx_proj_center returns None); such objects are counted in the status word and left out.
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "mf_kernels.h"
 #include "../../include/monoflex_b200.h"
 #include <math.h>
 
@@ -399,7 +399,7 @@ int mf_encode_targets_views(const double* labels, const double* P2, const int* s
     set_error("mf_encode_targets_views: B=%d M=%d H=%d W=%d (H and W multiples of %d)", B, M, H, W, DOWN);
     return -1;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  cudaStream_t st = MF_STREAM(stream);
   cudaError_t e = cudaMemsetAsync(status, 0, sizeof(int), st);
   if (e != cudaSuccess) return check_cuda(e, "encode_targets status");
   TargetOut o{obj, img, alphas, gt_bboxes, reg_weight, occlusions, truncations, obj6, P2_out, status};
@@ -430,7 +430,7 @@ int mf_encode_edges(const int* sizes, int B, int H, int W, long long* edge_indic
     set_error("mf_encode_edges: B=%d H=%d W=%d (H and W multiples of %d)", B, H, W, DOWN);
     return -1;
   }
-  return launch_edges(sizes, B, H, W, edge_indices, edge_len, reinterpret_cast<cudaStream_t>(stream));
+  return launch_edges(sizes, B, H, W, edge_indices, edge_len, MF_STREAM(stream));
 }
 
 }  // extern "C"

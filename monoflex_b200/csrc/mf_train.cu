@@ -11,7 +11,12 @@
 //  * focal_loss_backward_kernel: d/dpred of FocalLoss.forward (model/layers/focal_loss.py:35-55) scaled by a device
 //    scalar (loss weight / clamp(num_pos, 1), detector_loss.py:276).
 #include "mf_common.cuh"
-#include "mf_launch.h"
+#include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
+
+#define MF_MAX_PEERS 16
+#define MF_ADAMW_CHUNK 512   /* arena granularity (elements) of the per-chunk lr table */
+#define MF_UNSCALE_MAX_TENSORS 1024   /* (dst, src, n) triples of one mf_unscale_accumulate launch (by-value kernel params) */
 
 namespace mf {
 
@@ -122,35 +127,6 @@ static AdamwConsts adamw_consts(double beta1, float beta2, float eps, float wd, 
   k.bc1 = static_cast<float>(bc1); k.rsqrt_bc2 = static_cast<float>(1.0 / sqrt(bc2));
   k.grad_scale = grad_scale; k.lr_scale = lr_scale;
   return k;
-}
-
-int launch_adamw_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
-                     unsigned long long mc_params, unsigned long long mc_grads, float* m, float* v, const float* chunk_lr,
-                     long long n_chunks, double beta1, float beta2, float eps, float wd, long long step, float lr_scale,
-                     cudaStream_t st) {
-  if (world < 1 || world > MF_MAX_PEERS || rank < 0 || rank >= world) {
-    set_error("adamw_p2p: world %d (max %d) / rank %d", world, MF_MAX_PEERS, rank);
-    return -1;
-  }
-  if (step < 1) { set_error("adamw_p2p: step must be >= 1"); return -1; }
-  if ((mc_params == 0) != (mc_grads == 0)) { set_error("adamw_p2p: give both multicast addresses or neither"); return -1; }
-  PeerPtrs peers;
-  for (int r = 0; r < MF_MAX_PEERS; ++r) {
-    peers.p[r] = r < world ? reinterpret_cast<float*>(param_ptrs[r]) : nullptr;
-    peers.g[r] = r < world ? reinterpret_cast<const float*>(grad_ptrs[r]) : nullptr;
-  }
-  const long long base = n_chunks / world, extra = n_chunks % world;      // parallel.shard_range semantics
-  const long long lo = rank * base + (rank < extra ? rank : extra), hi = lo + base + (rank < extra ? 1 : 0);
-  if (hi <= lo) return 0;
-  const long long n_vec = (hi - lo) * (MF_ADAMW_CHUNK / 4);
-  long long blocks = (n_vec + 255) / 256;
-  const long long cap = 132LL * 8 * 4;
-  if (blocks > cap) blocks = cap;
-  const AdamwConsts k = adamw_consts(beta1, beta2, eps, wd, step, 1.f / static_cast<float>(world), lr_scale);
-  adamw_p2p_kernel<<<dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st>>>(
-      peers, world, rank, reinterpret_cast<float*>(mc_params), reinterpret_cast<const float*>(mc_grads), m, v, chunk_lr, lo,
-      hi, k);
-  return check_cuda(cudaGetLastError(), "adamw_p2p");
 }
 
 // ---------------------------------------------------------------- CUDA-graph-safe optimiser step with a finite guard
@@ -304,44 +280,6 @@ static void launch_dyn_update(int rule, dim3 grid, cudaStream_t st, float* p, fl
     (void)launch_k(adamw_arena_dyn_kernel<CLIP, MF_OPTIM_ADAMW>, grid, dim3(256), 0, st, p, g, m, v, chunk_lr, n_chunks, k,
                    dyn, hyper);
 }
-// max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL).
-// hyper: device double[4] {lr_mult, beta1, weight_decay, unused}, never NULL.
-int launch_adamw_arena_dyn(int rule, float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
-                           const double* hyper, float beta2, float eps, float grad_scale, long long* state4, void* dyn16,
-                           float max_norm, double* partials, float* total_norm_out, cudaStream_t st) {
-  if (rule != MF_OPTIM_ADAMW && rule != MF_OPTIM_ADAM) {
-    set_error("mf_optim_step_dyn: rule %d (0 = AdamW, 1 = Adam with L2 weight decay)", rule);
-    return -1;
-  }
-  if (n_chunks <= 0) return 0;
-  const bool clip = max_norm > 0.f;
-  if (clip && (partials == nullptr || total_norm_out == nullptr)) {
-    set_error("mf_optim_step_dyn: max_norm > 0 needs the partials buffer and total_norm_out");
-    return -1;
-  }
-  const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
-  long long blocks = (n_vec + 255) / 256;                       // <= (n_chunks + 1) / 2: the partials the caller provides
-  const long long cap = 132LL * 8 * 4;
-  if (blocks > cap) blocks = cap;
-  AdamwDyn* dyn = static_cast<AdamwDyn*>(dyn16);
-  if (clip) {
-    (void)launch_k(grad_sumsq_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, partials);
-    (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta2, partials,
-                   static_cast<int>(blocks), grad_scale, max_norm, total_norm_out, hyper);
-  } else {
-    (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
-    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta2, hyper);
-  }
-  AdamwConsts k{};                                              // beta1, wd, lr_scale and the bias corrections: on the device
-  k.beta2 = beta2; k.eps = eps; k.grad_scale = grad_scale;
-  const dim3 grid(static_cast<unsigned>(blocks));
-  if (clip)
-    launch_dyn_update<true>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
-  else
-    launch_dyn_update<false>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
-  return check_cuda(cudaGetLastError(), "mf_optim_step_dyn");
-}
-
 // ---------------------------------------------------------------- dynamic loss scale (torch.amp.GradScaler's rule)
 // The scale is device state (float scale, int growth_tracker), so a captured training step reads and updates it without
 // the host. Two kernels:
@@ -401,47 +339,6 @@ __global__ void __launch_bounds__(256) unscale_accumulate_kernel(const __grid_co
   }
 }
 
-int launch_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs,
-                              const long long* numels, const unsigned char* assign, int count, const float* scale,
-                              cudaStream_t st) {
-  if (count < 0 || count > MF_UNSCALE_MAX_TENSORS) {
-    set_error("mf_unscale_accumulate: %d tensors (0 .. %d in one launch)", count, MF_UNSCALE_MAX_TENSORS);
-    return -1;
-  }
-  if (count > 0 && (dst_ptrs == nullptr || src_ptrs == nullptr || numels == nullptr)) {
-    set_error("mf_unscale_accumulate: dst_ptrs, src_ptrs and numels are host arrays of count entries, not NULL");
-    return -1;
-  }
-  if (scale == nullptr) { set_error("mf_unscale_accumulate: scale (device float) is NULL"); return -1; }
-  UnscaleList L;
-  long long tiles = 0;
-  int k = 0;
-  for (int i = 0; i < count; ++i) {
-    if (numels[i] < 0 || numels[i] > 0x7fffffffLL) {
-      set_error("mf_unscale_accumulate: tensor %d has %lld elements (0 .. 2^31 - 1)", i, numels[i]);
-      return -1;
-    }
-    if (numels[i] == 0) continue;
-    if (dst_ptrs[i] == 0 || src_ptrs[i] == 0) {
-      set_error("mf_unscale_accumulate: tensor %d has a NULL dst or src", i);
-      return -1;
-    }
-    L.dst[k] = reinterpret_cast<float*>(dst_ptrs[i]);
-    L.src[k] = reinterpret_cast<const float*>(src_ptrs[i]);
-    L.n[k] = static_cast<int>(numels[i]);
-    L.assign[k] = (assign != nullptr && assign[i]) ? 1 : 0;
-    L.tile0[k] = static_cast<int>(tiles);
-    tiles += (numels[i] + UNSCALE_TILE - 1) / UNSCALE_TILE;
-    ++k;
-  }
-  if (k == 0) return 0;
-  if (tiles > 0x7fffffffLL) { set_error("mf_unscale_accumulate: %lld tiles exceed one grid", tiles); return -1; }
-  L.tile0[k] = static_cast<int>(tiles);
-  L.count = k;
-  (void)launch_k(unscale_accumulate_kernel, dim3(static_cast<unsigned>(tiles)), dim3(256), 0, st, L, scale);
-  return check_cuda(cudaGetLastError(), "mf_unscale_accumulate");
-}
-
 __global__ void loss_scale_update_kernel(const AdamwDyn* __restrict__ dyn, float* scale, int* growth_tracker,
                                          double growth_factor, double backoff_factor, int growth_interval) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
@@ -458,22 +355,6 @@ __global__ void loss_scale_update_kernel(const AdamwDyn* __restrict__ dyn, float
       *growth_tracker = successful;
     }
   }
-}
-
-int launch_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor,
-                             double backoff_factor, int growth_interval, cudaStream_t st) {
-  if (dyn16 == nullptr || scale == nullptr || growth_tracker == nullptr) {
-    set_error("mf_loss_scale_update: dyn16, scale and growth_tracker are device pointers, not NULL");
-    return -1;
-  }
-  if (!(growth_factor > 1.0) || !(backoff_factor > 0.0 && backoff_factor < 1.0) || growth_interval < 1) {
-    set_error("mf_loss_scale_update: needs growth_factor > 1, 0 < backoff_factor < 1, growth_interval >= 1 "
-              "(got %g, %g, %d)", growth_factor, backoff_factor, growth_interval);
-    return -1;
-  }
-  (void)launch_k(loss_scale_update_kernel, dim3(1), dim3(32), 0, st, static_cast<const AdamwDyn*>(dyn16), scale,
-                 growth_tracker, growth_factor, backoff_factor, growth_interval);
-  return check_cuda(cudaGetLastError(), "mf_loss_scale_update");
 }
 
 // ---------------------------------------------------------------- focal loss backward (layers/focal_loss.py:35-55)
@@ -509,3 +390,142 @@ int launch_focal_loss_backward(const float* pred, const float* tgt, long long n,
 }
 
 }  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_adamw_chunk(void) { return MF_ADAMW_CHUNK; }
+int mf_unscale_max_tensors(void) { return MF_UNSCALE_MAX_TENSORS; }
+
+int mf_adamw_step_p2p(const unsigned long long* param_ptrs, const unsigned long long* grad_ptrs, int world, int rank,
+                      unsigned long long mc_params, unsigned long long mc_grads, float* m, float* v, const float* chunk_lr,
+                      long long n_chunks, double beta1, float beta2, float eps, float wd, long long step, float lr_scale,
+                      void* stream) {
+  if (world < 1 || world > MF_MAX_PEERS || rank < 0 || rank >= world) {
+    set_error("adamw_p2p: world %d (max %d) / rank %d", world, MF_MAX_PEERS, rank);
+    return -1;
+  }
+  if (step < 1) { set_error("adamw_p2p: step must be >= 1"); return -1; }
+  if ((mc_params == 0) != (mc_grads == 0)) { set_error("adamw_p2p: give both multicast addresses or neither"); return -1; }
+  PeerPtrs peers;
+  for (int r = 0; r < MF_MAX_PEERS; ++r) {
+    peers.p[r] = r < world ? reinterpret_cast<float*>(param_ptrs[r]) : nullptr;
+    peers.g[r] = r < world ? reinterpret_cast<const float*>(grad_ptrs[r]) : nullptr;
+  }
+  const long long base = n_chunks / world, extra = n_chunks % world;      // parallel.shard_range semantics
+  const long long lo = rank * base + (rank < extra ? rank : extra), hi = lo + base + (rank < extra ? 1 : 0);
+  if (hi <= lo) return 0;
+  const long long n_vec = (hi - lo) * (MF_ADAMW_CHUNK / 4);
+  long long blocks = (n_vec + 255) / 256;
+  const long long cap = 132LL * 8 * 4;
+  if (blocks > cap) blocks = cap;
+  const AdamwConsts k = adamw_consts(beta1, beta2, eps, wd, step, 1.f / static_cast<float>(world), lr_scale);
+  adamw_p2p_kernel<<<dim3(static_cast<unsigned>(blocks)), dim3(256), 0, MF_STREAM(stream)>>>(
+      peers, world, rank, reinterpret_cast<float*>(mc_params), reinterpret_cast<const float*>(mc_grads), m, v, chunk_lr, lo,
+      hi, k);
+  return check_cuda(cudaGetLastError(), "adamw_p2p");
+}
+
+// max_norm <= 0: no clipping (g is only read; partials and total_norm_out are not used and may be NULL).
+// hyper: device double[4] {lr_mult, beta1, weight_decay, unused}, never NULL.
+int mf_optim_step_dyn(int rule, float* p, float* g, float* m, float* v, const float* chunk_lr, long long n_chunks,
+                      const double* hyper, float beta2, float eps, float grad_scale, long long* state4, void* dyn16,
+                      float max_norm, double* partials, float* total_norm_out, void* stream) {
+  if (hyper == nullptr) { set_error("mf_optim_step_dyn: hyper (device double[4]) is NULL"); return -1; }
+  if (rule != MF_OPTIM_ADAMW && rule != MF_OPTIM_ADAM) {
+    set_error("mf_optim_step_dyn: rule %d (0 = AdamW, 1 = Adam with L2 weight decay)", rule);
+    return -1;
+  }
+  if (n_chunks <= 0) return 0;
+  const bool clip = max_norm > 0.f;
+  if (clip && (partials == nullptr || total_norm_out == nullptr)) {
+    set_error("mf_optim_step_dyn: max_norm > 0 needs the partials buffer and total_norm_out");
+    return -1;
+  }
+  const long long n_vec = n_chunks * (MF_ADAMW_CHUNK / 4);
+  long long blocks = (n_vec + 255) / 256;                       // <= (n_chunks + 1) / 2: the partials the caller provides
+  const long long cap = 132LL * 8 * 4;
+  if (blocks > cap) blocks = cap;
+  AdamwDyn* dyn = static_cast<AdamwDyn*>(dyn16);
+  const cudaStream_t st = MF_STREAM(stream);
+  if (clip) {
+    (void)launch_k(grad_sumsq_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, partials);
+    (void)launch_k(adamw_prepare_clip_kernel, dim3(1), dim3(256), 0, st, state4, dyn, beta2, partials,
+                   static_cast<int>(blocks), grad_scale, max_norm, total_norm_out, hyper);
+  } else {
+    (void)launch_k(grad_finite_kernel, dim3(static_cast<unsigned>(blocks)), dim3(256), 0, st, g, n_vec, state4);
+    (void)launch_k(adamw_prepare_kernel, dim3(1), dim3(32), 0, st, state4, dyn, beta2, hyper);
+  }
+  AdamwConsts k{};                                              // beta1, wd, lr_scale and the bias corrections: on the device
+  k.beta2 = beta2; k.eps = eps; k.grad_scale = grad_scale;
+  const dim3 grid(static_cast<unsigned>(blocks));
+  if (clip)
+    launch_dyn_update<true>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
+  else
+    launch_dyn_update<false>(rule, grid, st, p, g, m, v, chunk_lr, n_chunks, k, dyn, hyper);
+  return check_cuda(cudaGetLastError(), "mf_optim_step_dyn");
+}
+
+int mf_unscale_accumulate(const unsigned long long* dst_ptrs, const unsigned long long* src_ptrs, const long long* numels,
+                          const unsigned char* assign, int count, const float* scale, void* stream) {
+  if (count < 0 || count > MF_UNSCALE_MAX_TENSORS) {
+    set_error("mf_unscale_accumulate: %d tensors (0 .. %d in one launch)", count, MF_UNSCALE_MAX_TENSORS);
+    return -1;
+  }
+  if (count > 0 && (dst_ptrs == nullptr || src_ptrs == nullptr || numels == nullptr)) {
+    set_error("mf_unscale_accumulate: dst_ptrs, src_ptrs and numels are host arrays of count entries, not NULL");
+    return -1;
+  }
+  if (scale == nullptr) { set_error("mf_unscale_accumulate: scale (device float) is NULL"); return -1; }
+  UnscaleList L;
+  long long tiles = 0;
+  int k = 0;
+  for (int i = 0; i < count; ++i) {
+    if (numels[i] < 0 || numels[i] > 0x7fffffffLL) {
+      set_error("mf_unscale_accumulate: tensor %d has %lld elements (0 .. 2^31 - 1)", i, numels[i]);
+      return -1;
+    }
+    if (numels[i] == 0) continue;
+    if (dst_ptrs[i] == 0 || src_ptrs[i] == 0) {
+      set_error("mf_unscale_accumulate: tensor %d has a NULL dst or src", i);
+      return -1;
+    }
+    L.dst[k] = reinterpret_cast<float*>(dst_ptrs[i]);
+    L.src[k] = reinterpret_cast<const float*>(src_ptrs[i]);
+    L.n[k] = static_cast<int>(numels[i]);
+    L.assign[k] = (assign != nullptr && assign[i]) ? 1 : 0;
+    L.tile0[k] = static_cast<int>(tiles);
+    tiles += (numels[i] + UNSCALE_TILE - 1) / UNSCALE_TILE;
+    ++k;
+  }
+  if (k == 0) return 0;
+  if (tiles > 0x7fffffffLL) { set_error("mf_unscale_accumulate: %lld tiles exceed one grid", tiles); return -1; }
+  L.tile0[k] = static_cast<int>(tiles);
+  L.count = k;
+  (void)launch_k(unscale_accumulate_kernel, dim3(static_cast<unsigned>(tiles)), dim3(256), 0, MF_STREAM(stream), L, scale);
+  return check_cuda(cudaGetLastError(), "mf_unscale_accumulate");
+}
+
+int mf_loss_scale_update(const void* dyn16, float* scale, int* growth_tracker, double growth_factor, double backoff_factor,
+                         int growth_interval, void* stream) {
+  if (dyn16 == nullptr || scale == nullptr || growth_tracker == nullptr) {
+    set_error("mf_loss_scale_update: dyn16, scale and growth_tracker are device pointers, not NULL");
+    return -1;
+  }
+  if (!(growth_factor > 1.0) || !(backoff_factor > 0.0 && backoff_factor < 1.0) || growth_interval < 1) {
+    set_error("mf_loss_scale_update: needs growth_factor > 1, 0 < backoff_factor < 1, growth_interval >= 1 "
+              "(got %g, %g, %d)", growth_factor, backoff_factor, growth_interval);
+    return -1;
+  }
+  (void)launch_k(loss_scale_update_kernel, dim3(1), dim3(32), 0, MF_STREAM(stream), static_cast<const AdamwDyn*>(dyn16), scale,
+                 growth_tracker, growth_factor, backoff_factor, growth_interval);
+  return check_cuda(cudaGetLastError(), "mf_loss_scale_update");
+}
+
+int mf_focal_loss_backward(const float* pred, const float* target, long long n, const float* scale, float* grad_pred,
+                           void* stream) {
+  return launch_focal_loss_backward(pred, target, n, scale, grad_pred, MF_STREAM(stream));
+}
+
+}  // extern "C"

@@ -13,6 +13,7 @@
 // order across splits is therefore not fixed (like cuDNN's non-deterministic wgrad algorithms).
 #include "mf_common.cuh"
 #include "mf_kernels.h"
+#include "../../include/monoflex_b200.h"
 #include <cstring>
 
 namespace mf {
@@ -195,11 +196,23 @@ static int launch_wgrad_n(int bn, const CUtensorMap& tx, const CUtensorMap& tdy,
   return launch_wgrad_cfg<16, AW, 16>(tx, tdy, p, grid, st);
 }
 
+}  // namespace mf
+
+using namespace mf;
+
+extern "C" {
+
+int mf_conv2d_wgrad_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, const void* dy, int dy_ld, int Cout, int k,
+                             int stride, int pad, float* dw, void* stream) {
+  return mf_conv2d_wgrad_rect_nhwc_f16(x, x_ld, B, H, W, Cin, dy, dy_ld, Cout, k, k, stride, pad, pad, dw, stream);
+}
+
 // x: [B*H*W, x_ld] fp16 NHWC rows; dy: [B*Ho*Wo, dy_ld] fp16 rows; dw: [Cout, Cin, kh, kw] fp32 (overwritten)
-int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, const __half* dy, int dy_ld, int Cout, int kh,
-                      int kw, int stride, int pad_h, int pad_w, float* dw, cudaStream_t st) {
+int mf_conv2d_wgrad_rect_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, const void* dy, int dy_ld, int Cout, int kh,
+                                  int kw, int stride, int pad_h, int pad_w, float* dw, void* stream) {
   static PFN_encTiledW enc = reinterpret_cast<PFN_encTiledW>(wg_driver_fn("cuTensorMapEncodeTiled"));
   static PFN_encIm2colW enc2 = reinterpret_cast<PFN_encIm2colW>(wg_driver_fn("cuTensorMapEncodeIm2col"));
+  const cudaStream_t st = MF_STREAM(stream);
   if (!enc || !enc2) { set_error("conv wgrad: tensor-map driver entry points unavailable"); return -1; }
   const bool cin_ok = Cin == 16 || Cin == 32 || (Cin > 0 && Cin % 64 == 0);
   const bool cout_ok = Cout == 16 || Cout == 32 || (Cout > 0 && Cout % 64 == 0);
@@ -211,7 +224,8 @@ int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, c
   }
   // full-resolution stem layers: all reduction, no tile (mf_wgrad_narrow.cu)
   if (Cin == 16 && Cout == 16 && stride == 1 && kh == kw && (kh == 3 || kh == 7) && pad_h == kh / 2 && pad_w == kh / 2)
-    return launch_conv_wgrad_narrow(x, x_ld, B, H, W, dy, dy_ld, kh, dw, st);
+    return launch_conv_wgrad_narrow(static_cast<const __half*>(x), x_ld, B, H, W, static_cast<const __half*>(dy), dy_ld, kh, dw,
+                                    st);
   const int aw = Cin < 64 ? Cin : 64, bw = Cout < 64 ? Cout : 64;
   WgradParams p;
   memset(&p, 0, sizeof(p));
@@ -242,7 +256,7 @@ int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     int lower[2] = {-pad_w, -pad_h}, upper[2] = {pad_w - (kw - 1), pad_h - (kh - 1)};
     cuuint32_t estr[4] = {1, static_cast<cuuint32_t>(stride), static_cast<cuuint32_t>(stride), 1};
     const CUtensorMapSwizzle swa = aw == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : aw == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-    if (enc2(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<__half*>(x), gdim, gstr, lower, upper, static_cast<cuuint32_t>(aw),
+    if (enc2(&tx, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x), gdim, gstr, lower, upper, static_cast<cuuint32_t>(aw),
              WG_BK, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swa, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) { set_error("conv wgrad: im2col map failed"); return -1; }
   }
@@ -252,7 +266,7 @@ int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, c
     cuuint32_t box[2] = {static_cast<cuuint32_t>(bw), WG_BK};
     cuuint32_t estr[2] = {1, 1};
     const CUtensorMapSwizzle swb = bw == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : bw == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
-    if (enc(&tdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<__half*>(dy), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    if (enc(&tdy, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(dy), gdim, gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
             swb, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS) {
       set_error("conv wgrad: dY map failed");
       return -1;
@@ -266,4 +280,4 @@ int launch_conv_wgrad(const __half* x, int x_ld, int B, int H, int W, int Cin, c
   return launch_wgrad_n<16>(bn, tx, tdy, p, grid, st);
 }
 
-}  // namespace mf
+}  // extern "C"

@@ -1,7 +1,7 @@
 """TEST TOOLING — heat maps that drive the decode kernels (csrc/mf_decode.cu) onto each of their stage-1 paths, slab splits
 and tie rules.
 
-Stage 1 splits every (image, class) plane into S slabs (`slab_count`, a copy of launch_decode's rule) and selects each
+Stage 1 splits every (image, class) plane into S slabs (`slab_count`, a copy of mf_decode_detections' rule) and selects each
 slab's top-K in one of two ways: rank by counting when the slab holds between k_eff = min(K, slab size) and S1_CAND
 strictly positive local maxima ('fast'), otherwise an MSB-first radix select plus a 256-key bitonic sort ('radix').
 The synthetic N(-3, 1.5) logits of synthetic.make_head_logits only ever take the fast path. The families here:
@@ -40,13 +40,13 @@ LO, HI = np.float32(1e-4), np.float32(1 - 1e-4)          # sigmoid_hm's clamp bo
 R = 50
 
 
-# ------------------------------------------------------------------------------------------------ launch_decode's rules
+# -------------------------------------------------------------------------------------- mf_decode_detections' rules
 def _cdiv(a, b):
     return -(-a // b)
 
 
 def slab_count(B, C, H, W, K, nsm=H100_SMS, smem_max=H100_SMEM_OPTIN):
-    """launch_decode's slab rule: the S <= 8 minimising waves x (items per thread + 6) among the splits whose slab (score
+    """mf_decode_detections' slab rule: the S <= 8 minimising waves x (items per thread + 6) among the splits whose slab (score
     keys + staged pixels with the one-row halo) fits the opt-in shared memory and whose C*S*K candidates fit stage 2.
     0 = no split fits."""
     HW = H * W

@@ -1,5 +1,6 @@
 """CPU: the C-ABI library loads without a GPU driver and exports every symbol include/monoflex_b200.h declares; the
-ctypes table in monoflex_b200/_lib.py covers the same set; product modules keep the reference's state_dict keys."""
+ctypes table monoflex_b200/_lib.py derives from the header covers the same set with the right types; csrc/ defines each
+entry point exactly once; product modules keep the reference's state_dict keys."""
 import ctypes
 import os
 import re
@@ -35,6 +36,49 @@ def test_library_exports_every_declared_symbol(lib):
 def test_ctypes_table_matches_header():
     from monoflex_b200 import _lib
     assert sorted(list(_lib.SIGNATURES) + ["mf_last_error"]) == header_symbols()
+
+
+def test_derived_bindings_cover_header():
+    """The prototypes parsed from the header include every symbol this independent name scan finds."""
+    from monoflex_b200 import _lib
+    assert sorted(_lib._PROTOTYPES) == header_symbols()
+
+
+def test_derived_ctypes_types():
+    from monoflex_b200 import _lib
+    sig, proto = _lib.SIGNATURES, _lib._PROTOTYPES
+    assert sig["mf_bn_sync_forward_apply"][5] is ctypes.c_double
+    assert sig["mf_loss_scale_update"][3:5] == [ctypes.c_double, ctypes.c_double]
+    assert sig["mf_adamw_step_p2p"][4:6] == [ctypes.c_ulonglong, ctypes.c_ulonglong]
+    assert sig["mf_kitti_eval_statistics"][14] is ctypes.c_size_t
+    assert sig["mf_sigmoid_clamp"] == [ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p]
+    assert sig["mf_version"] == [] and proto["mf_last_error"][1] == []
+    workspace = [name for name in sig if name.endswith("_workspace")]
+    assert len(workspace) == 5
+    assert {proto[name][0] for name in workspace} == {ctypes.c_size_t}
+    assert proto["mf_last_error"][0] is ctypes.c_char_p
+    assert {proto[name][0] for name in sig if name not in workspace} == {ctypes.c_int}
+
+
+def test_unknown_parameter_type_is_refused():
+    from monoflex_b200 import _lib
+    assert _lib.parse_header("int mf_ok(const void* x, unsigned long long n, void* stream);")["mf_ok"][1] == \
+        [ctypes.c_void_p, ctypes.c_ulonglong, ctypes.c_void_p]
+    with pytest.raises(RuntimeError, match="mf_bad"):
+        _lib.parse_header("int mf_bad(const float* x, short n, void* stream);")
+    with pytest.raises(RuntimeError, match="mf_bad_ret"):
+        _lib.parse_header("float mf_bad_ret(void);")
+
+
+def test_each_entry_point_defined_once_beside_its_kernels():
+    """Every header symbol has exactly one definition under csrc/, and csrc/ defines no mf_* function the header lacks."""
+    csrc = os.path.join(ROOT, "monoflex_b200", "csrc")
+    defined = []
+    for name in sorted(os.listdir(csrc)):
+        if name.endswith(".cu"):
+            src = re.sub(r"/\*.*?\*/|//[^\n]*", "", open(os.path.join(csrc, name)).read(), flags=re.S)
+            defined += re.findall(r"\b(?:int|size_t|char\s*\*)\s*\b(mf_[a-z0-9_]+)\s*\([^;{}]*\)\s*\{", src)
+    assert sorted(defined) == header_symbols()
 
 
 def test_version_and_error_string(lib):

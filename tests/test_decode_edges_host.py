@@ -33,7 +33,7 @@ def summary():
 
 
 def test_slab_rule_matches_the_h100_splits():
-    """launch_decode's choice of S with 132 SMs, C = 3, K = 50"""
+    """mf_decode_detections' choice of S with 132 SMs, C = 3, K = 50"""
     got = {B: de.slab_count(B, 3, 96, 320, 50) for B in (1, 5, 6, 8, 11, 14, 16)}
     assert got == {1: 8, 5: 8, 6: 6, 8: 5, 11: 4, 14: 3, 16: 2}
     assert de.slab_count(6, 3, 112, 256, 50) == 7
