@@ -123,15 +123,6 @@ int mf_pack_image_pair8(const float* x_nchw, void* y_nhwc8, int B, int C, int H,
 /* image [B,3,H,W] fp32 -> [B*H*W, 16] fp16 rows [hi3 | lo3 | hi3 | 0 x 7] (the stem then is a plain 16-channel conv with
  * per-tap weights [W_hi | W_hi | W_lo | 0]) */
 int mf_pack_image_split(const float* x_nchw, void* y_rows16, int B, int C, int H, int W, void* stream);
-int mf_maxpool2_split(const void* x, int x_lo, void* y, int y_lo, int B, int H, int W, int C, int x_ld, int y_ld, void* stream);
-int mf_upsample_add_split(const void* x, int x_lo, const float* w_taps, const void* skip, int skip_lo, void* y, int y_lo, int B,
-                          int Hi, int Wi, int C, int f, int x_ld, int skip_ld, int y_ld, void* stream);
-/* edge fusion on pairs: ea / eb are [B, K+2, 512] rows = [hi 256 | lo 256] */
-int mf_edge_gather_split(const void* feat, int feat_ld, int feat_lo, int ch_a, int ch_b, const long long* edge_idx, void* ea,
-                         void* eb, int B, int H, int W, int K, int out_w, int out_h, void* stream);
-int mf_edge_head_add_split(const void* t, int t_ld, int t_lo, const float* w, const float* bias, int n_out,
-                           const long long* edge_idx, const long long* edge_len, float* out, int out_ctot, int out_ch0, int B,
-                           int K, int H, int W, void* stream);
 /* pair rows -> fp32 NCHW (hi + lo): feature-map export */
 int mf_split_to_nchw_f32(const void* x, int x_ld, int x_lo, float* y, int B, int C, int HW, void* stream);
 
@@ -166,19 +157,22 @@ int mf_dcn_nhwc_f16(const void* x, int x_ld, int B, int H, int W, int Cin, const
 /* images [B,C<=8,H,W] fp32 NCHW (engine/trainer.py:106, engine/inference.py:29) -> NHWC fp16 with 8 channels */
 int mf_pack_image(const float* x_nchw, void* y_nhwc8, int B, int C, int H, int W, void* stream);
 int mf_nchw_f32_to_nhwc_f16(const float* x, void* y, int B, int C, int HW, int y_ld, void* stream);
+/* The max-pool, up-sample and edge-fusion entry points below read and write either row format, given by the lo offsets:
+ * every `*_lo` 0 = plain fp16 rows; every `*_lo` non-zero = strict-precision pair rows, the lo block that many elements after
+ * the hi block in the same row. Mixed formats and lo offsets that are not multiples of 8 are rejected. */
 /* nn.MaxPool2d(2) of Tree.downsample (dla_dcn.py:238) */
-int mf_maxpool2_nhwc_f16(const void* x, void* y, int B, int H, int W, int C, int x_ld, int y_ld, void* stream);
+int mf_maxpool2_nhwc_f16(const void* x, int x_ld, int x_lo, void* y, int y_ld, int y_lo, int B, int H, int W, int C, void* stream);
 /* depthwise ConvTranspose2d(k=2f, stride f, pad f/2) + skip add (IDAUp.forward dla_dcn.py:419-425).
- * w_taps: fp32 [k*k, C] */
-int mf_upsample_add_nhwc_f16(const void* x, const float* w_taps, const void* skip, void* y, int B, int Hi, int Wi, int C,
-                             int f, int x_ld, int skip_ld, int y_ld, void* stream);
+ * w_taps: fp32 [k*k, C]; skip may be NULL (skip_lo is then ignored) */
+int mf_upsample_add_nhwc_f16(const void* x, int x_ld, int x_lo, const float* w_taps, const void* skip, int skip_ld, int skip_lo,
+                             void* y, int y_ld, int y_lo, int B, int Hi, int Wi, int C, int f, void* stream);
 /* edge fusion (detector_predictor.py:137-158): grid_sample of two 256-ch slices at the border pixels into two
- * replicate-padded Conv1d inputs [B, K+2, 256]; final Conv1d(256->n_out,k=1) + indexed add into an NCHW fp32 map. */
-int mf_edge_gather(const void* feat, int feat_ld, int ch_a, int ch_b, const long long* edge_idx, void* ea, void* eb, int B,
-                   int H, int W, int K, int out_w, int out_h, void* stream);
-int mf_edge_head_add(const void* t, const float* w, const float* bias, int n_out, const long long* edge_idx,
-                     const long long* edge_len, float* out, int out_ctot, int out_ch0, int B, int K, int H, int W,
-                     void* stream);
+ * replicate-padded Conv1d inputs [B, K+2, 256] (pair rows: [B, K+2, 512] = [hi 256 | lo 256], when feat_lo != 0);
+ * final Conv1d(256->n_out,k=1) of the rows of t [B*K, t_ld] + indexed add into an NCHW fp32 map. */
+int mf_edge_gather(const void* feat, int feat_ld, int feat_lo, int ch_a, int ch_b, const long long* edge_idx, void* ea, void* eb,
+                   int B, int H, int W, int K, int out_w, int out_h, void* stream);
+int mf_edge_head_add(const void* t, int t_ld, int t_lo, const float* w, const float* bias, int n_out, const long long* edge_idx,
+                     const long long* edge_len, float* out, int out_ctot, int out_ch0, int B, int K, int H, int W, void* stream);
 /* sigmoid_hm (model/layers/utils.py:39-43), in place */
 int mf_sigmoid_clamp(float* x, long long n, void* stream);
 /* FocalLoss.forward (model/layers/focal_loss.py:35-55): out2[0] = loss sum, out2[1] = num_pos */

@@ -13,20 +13,6 @@
 
 namespace mf {
 
-MF_DEVINL void bn_unpack8(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float2 t = __half22float2(h[e]);
-    f[2 * e] = t.x; f[2 * e + 1] = t.y;
-  }
-}
-MF_DEVINL uint4 bn_pack8(const float (&f)[8]) {
-  __half2 o[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) o[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
-  return *reinterpret_cast<uint4*>(o);
-}
 MF_DEVINL float bn_act_grad(float y, int act) {           // derivative of the activation, from the sign of its OUTPUT
   if (act == 1) return y > 0.f ? 1.f : 0.f;               // ReLU
   if (act == 2) return y > 0.f ? 1.f : 0.01f;             // leaky_relu(0.01) (InPlaceABN)
@@ -56,7 +42,7 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
 #pragma unroll
     for (int e = 0; e < 8; ++e) { mu[e] = mean[cv * 8 + e]; rs[e] = rstd[cv * 8 + e]; }
   } else if (pivot) {
-    bn_unpack8(__ldg(reinterpret_cast<const uint4*>(x + cv * 8)), mu);
+    Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(x + cv * 8)), mu);
   } else {
 #pragma unroll
     for (int e = 0; e < 8; ++e) mu[e] = 0.f;
@@ -81,7 +67,7 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
 #pragma unroll
       for (int u = 0; u < U; ++u) {                        // fixed accumulation order: row, row + RL, ...
         float xv[8];
-        bn_unpack8(xq[u], xv);
+        Fp16Rows::to_f32(xq[u], xv);
         if (!BWD) {
           const bool ok = row + static_cast<long long>(u) * RL < r1;    // rows past the slab add nothing
 #pragma unroll
@@ -92,8 +78,8 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
           }
         } else {
           float gv[8], yv[8];
-          bn_unpack8(gq[u], gv);
-          bn_unpack8(yq[u], yv);
+          Fp16Rows::to_f32(gq[u], gv);
+          Fp16Rows::to_f32(yq[u], yv);
 #pragma unroll
           for (int e = 0; e < 8; ++e) {
             const float g = gv[e] * bn_act_grad(yv[e], act);
@@ -167,8 +153,8 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const __half* __restrict_
   *reinterpret_cast<float4*>(&sc[4]) = __ldg(reinterpret_cast<const float4*>(scale + cv * 8 + 4));
   *reinterpret_cast<float4*>(&sh[0]) = __ldg(reinterpret_cast<const float4*>(shift + cv * 8));
   *reinterpret_cast<float4*>(&sh[4]) = __ldg(reinterpret_cast<const float4*>(shift + cv * 8 + 4));
-  bn_unpack8(xq, v);
-  bn_unpack8(rq, rv);
+  Fp16Rows::to_f32(xq, v);
+  Fp16Rows::to_f32(rq, rv);
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     float t = v[e] * sc[e] + sh[e];
@@ -177,7 +163,7 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const __half* __restrict_
     else if (act == 2) t = fmaxf(t, 0.01f * t);
     v[e] = t;
   }
-  *reinterpret_cast<uint4*>(y + row * y_ld + cv * 8) = bn_pack8(v);
+  *reinterpret_cast<uint4*>(y + row * y_ld + cv * 8) = Fp16Rows::pack(v);
 }
 
 __global__ void bn_bwd_finalize_kernel(const float* __restrict__ part, int ncta, int C, float* __restrict__ dgamma,
@@ -217,9 +203,9 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restr
     *reinterpret_cast<float4*>(&sg[4 * h]) = __ldg(reinterpret_cast<const float4*>(sum_g + cv * 8 + 4 * h));
     *reinterpret_cast<float4*>(&sgx[4 * h]) = __ldg(reinterpret_cast<const float4*>(sum_gx + cv * 8 + 4 * h));
   }
-  bn_unpack8(xq, xv);
-  bn_unpack8(gq, gv);
-  bn_unpack8(yq, yv);
+  Fp16Rows::to_f32(xq, xv);
+  Fp16Rows::to_f32(gq, gv);
+  Fp16Rows::to_f32(yq, yv);
   const float inv_m = static_cast<float>(1.0 / count);          // global element count (== M unless SyncBatchNorm)
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
@@ -228,8 +214,8 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restr
     o[e] = sc[e] * (g - sg[e] * inv_m - xhat * sgx[e] * inv_m);
     gr[e] = g;
   }
-  *reinterpret_cast<uint4*>(dx + row * dx_ld + cv * 8) = bn_pack8(o);
-  if (dres != nullptr) *reinterpret_cast<uint4*>(dres + row * dres_ld + cv * 8) = bn_pack8(gr);
+  *reinterpret_cast<uint4*>(dx + row * dx_ld + cv * 8) = Fp16Rows::pack(o);
+  if (dres != nullptr) *reinterpret_cast<uint4*>(dres + row * dres_ld + cv * 8) = Fp16Rows::pack(gr);
 }
 
 // ------------------------------------------------------------------------------------------------ SyncBatchNorm halves

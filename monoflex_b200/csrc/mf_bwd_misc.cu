@@ -17,21 +17,6 @@
 
 namespace mf {
 
-MF_DEVINL void bm_unpack8(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float2 t = __half22float2(h[e]);
-    f[2 * e] = t.x; f[2 * e + 1] = t.y;
-  }
-}
-MF_DEVINL uint4 bm_pack8(const float (&f)[8]) {
-  __half2 o[4];
-#pragma unroll
-  for (int e = 0; e < 4; ++e) o[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
-  return *reinterpret_cast<uint4*>(o);
-}
-
 // ---------------------------------------------------------------- MaxPool2d(2) backward
 __global__ void __launch_bounds__(256) maxpool2_bwd_kernel(const __half* __restrict__ x, const __half* __restrict__ dy,
                                                            __half* __restrict__ dx, int B, int H, int W, int C, int x_ld,
@@ -49,8 +34,8 @@ __global__ void __launch_bounds__(256) maxpool2_bwd_kernel(const __half* __restr
   const long long rows[4] = {r00, r00 + 1, r00 + W, r00 + W + 1};           // window scan order
   float v[4][8], g[8], o[4][8];
 #pragma unroll
-  for (int q = 0; q < 4; ++q) bm_unpack8(__ldg(reinterpret_cast<const uint4*>(x + rows[q] * x_ld + cv * 8)), v[q]);
-  bm_unpack8(__ldg(reinterpret_cast<const uint4*>(dy + pix * dy_ld + cv * 8)), g);
+  for (int q = 0; q < 4; ++q) Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(x + rows[q] * x_ld + cv * 8)), v[q]);
+  Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(dy + pix * dy_ld + cv * 8)), g);
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     int arg = 0;
@@ -62,7 +47,7 @@ __global__ void __launch_bounds__(256) maxpool2_bwd_kernel(const __half* __restr
     for (int q = 0; q < 4; ++q) o[q][e] = q == arg ? g[e] : 0.f;
   }
 #pragma unroll
-  for (int q = 0; q < 4; ++q) *reinterpret_cast<uint4*>(dx + rows[q] * dx_ld + cv * 8) = bm_pack8(o[q]);
+  for (int q = 0; q < 4; ++q) *reinterpret_cast<uint4*>(dx + rows[q] * dx_ld + cv * 8) = Fp16Rows::pack(o[q]);
 }
 
 // ---------------------------------------------------------------- depth-wise ConvTranspose2d backward: data
@@ -89,14 +74,14 @@ __global__ void __launch_bounds__(256) upsample_bwd_dx_kernel(const __half* __re
       const int ox = ix * f - pad + kx;
       if (ox < 0 || ox >= Wo) continue;
       float g[8];
-      bm_unpack8(__ldg(reinterpret_cast<const uint4*>(dy + ((b * Ho + oy) * Wo + ox) * dy_ld + cv * 8)), g);
+      Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(dy + ((b * Ho + oy) * Wo + ox) * dy_ld + cv * 8)), g);
       const float4 w0 = __ldg(reinterpret_cast<const float4*>(w + static_cast<long long>(ky * k + kx) * C + cv * 8));
       const float4 w1 = __ldg(reinterpret_cast<const float4*>(w + static_cast<long long>(ky * k + kx) * C + cv * 8 + 4));
       acc[0] += g[0] * w0.x; acc[1] += g[1] * w0.y; acc[2] += g[2] * w0.z; acc[3] += g[3] * w0.w;
       acc[4] += g[4] * w1.x; acc[5] += g[5] * w1.y; acc[6] += g[6] * w1.z; acc[7] += g[7] * w1.w;
     }
   }
-  *reinterpret_cast<uint4*>(dx + pix * dx_ld + cv * 8) = bm_pack8(acc);
+  *reinterpret_cast<uint4*>(dx + pix * dx_ld + cv * 8) = Fp16Rows::pack(acc);
 }
 // weights: part[slab][tap][c] = sum over the slab's input pixels of x[pixel, c] * dy[shifted pixel, c].
 // A warp owns one 8-channel group and 8 taps: its 32 lanes walk the slab's pixels (x loaded ONCE per pixel for the 8 taps, the
@@ -141,11 +126,11 @@ __global__ void __launch_bounds__(256) upsample_bwd_dw_kernel(const __half* __re
       gr[t] = ok ? __ldg(reinterpret_cast<const uint4*>(dy + ((b * Ho + oy) * Wo + ox) * dy_ld + cv * 8)) : make_uint4(0u, 0u, 0u, 0u);
     }
     float xv[8];
-    bm_unpack8(xr, xv);
+    Fp16Rows::to_f32(xr, xv);
 #pragma unroll
     for (int t = 0; t < UPW_TAPS; ++t) {
       float g[8];
-      bm_unpack8(gr[t], g);
+      Fp16Rows::to_f32(gr[t], g);
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[t][e] += xv[e] * g[e];
     }
@@ -209,7 +194,7 @@ __global__ void __launch_bounds__(256) column_sum_partial_kernel(const __half* _
   if (r < RL) {
     for (long long row = r0 + r; row < r1; row += RL) {
       float v[8];
-      bm_unpack8(__ldg(reinterpret_cast<const uint4*>(x + row * x_ld + cv * 8)), v);
+      Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(x + row * x_ld + cv * 8)), v);
 #pragma unroll
       for (int e = 0; e < 8; ++e) a[e] += v[e];
     }
@@ -247,22 +232,14 @@ __global__ void edge_gather_bwd_kernel(const __half* __restrict__ d_ea, const __
   const int b = static_cast<int>(t / (K + 2));
   int e = pos - 1;
   e = e < 0 ? 0 : (e > K - 1 ? K - 1 : e);
-  const float ex = static_cast<float>(edge_idx[(static_cast<long long>(b) * K + e) * 2 + 0]);
-  const float ey = static_cast<float>(edge_idx[(static_cast<long long>(b) * K + e) * 2 + 1]);
-  const float gx = ex / static_cast<float>(out_w - 1) * 2.f - 1.f;
-  const float gy = ey / static_cast<float>(out_h - 1) * 2.f - 1.f;
-  const float ix = ((gx + 1.f) / 2.f) * static_cast<float>(W - 1);
-  const float iy = ((gy + 1.f) / 2.f) * static_cast<float>(H - 1);
-  const float x0f = floorf(ix), y0f = floorf(iy);
-  const int x0 = static_cast<int>(x0f), y0 = static_cast<int>(y0f);
-  const float wx1 = ix - x0f, wy1 = iy - y0f, wx0 = 1.f - wx1, wy0 = 1.f - wy1;
+  const EdgeSample s = edge_sample(edge_idx, b, K, e, H, W, out_w, out_h);
   float g[8];
-  bm_unpack8(__ldg(reinterpret_cast<const uint4*>((which ? d_eb : d_ea) + (static_cast<long long>(b) * (K + 2) + pos) * 256 + cv * 8)), g);
+  Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>((which ? d_eb : d_ea) + (static_cast<long long>(b) * (K + 2) + pos) * 256 + cv * 8)), g);
   __half* fb = d_feat + static_cast<long long>(b) * H * W * feat_ld + (which ? ch_b : ch_a) + cv * 8;
-  const float wts[4] = {wy0 * wx0, wy0 * wx1, wy1 * wx0, wy1 * wx1};
+  const float wts[4] = {s.wy0 * s.wx0, s.wy0 * s.wx1, s.wy1 * s.wx0, s.wy1 * s.wx1};
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    const int yy = y0 + (q >> 1), xx = x0 + (q & 1);
+    const int yy = s.y0 + (q >> 1), xx = s.x0 + (q & 1);
     if (yy < 0 || yy >= H || xx < 0 || xx >= W || wts[q] == 0.f) continue;
     __half2* dst = reinterpret_cast<__half2*>(fb + static_cast<long long>(yy * W + xx) * feat_ld);
 #pragma unroll
@@ -303,7 +280,7 @@ __global__ void __launch_bounds__(256) edge_head_add_bwd_kernel(const __half* __
     for (int q = 0; q < 8; ++q) acc[q] = 0.f;
     if (e < edge_len[b]) {
       float tv[8];
-      bm_unpack8(__ldg(reinterpret_cast<const uint4*>(t + static_cast<long long>(pos) * 256 + lane * 8)), tv);
+      Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(t + static_cast<long long>(pos) * 256 + lane * 8)), tv);
       const long long ex = edge_idx[(static_cast<long long>(b) * K + e) * 2], ey = edge_idx[(static_cast<long long>(b) * K + e) * 2 + 1];
 #pragma unroll
       for (int o = 0; o < NO; ++o) {
@@ -318,7 +295,7 @@ __global__ void __launch_bounds__(256) edge_head_add_bwd_kernel(const __half* __
         }
       }
     }
-    *reinterpret_cast<uint4*>(d_t + static_cast<long long>(pos) * 256 + lane * 8) = bm_pack8(acc);
+    *reinterpret_cast<uint4*>(d_t + static_cast<long long>(pos) * 256 + lane * 8) = Fp16Rows::pack(acc);
   }
 #pragma unroll
   for (int o = 0; o < NO; ++o) {
@@ -351,11 +328,11 @@ __global__ void __launch_bounds__(256) add_rows_kernel(__half* __restrict__ dst,
   const int cv = static_cast<int>(i % CV);
   const long long row = i / CV;
   float a[8], b[8];
-  bm_unpack8(*reinterpret_cast<const uint4*>(dst + row * dst_ld + cv * 8), a);
-  bm_unpack8(__ldg(reinterpret_cast<const uint4*>(src + row * src_ld + cv * 8)), b);
+  Fp16Rows::to_f32(*reinterpret_cast<const uint4*>(dst + row * dst_ld + cv * 8), a);
+  Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(src + row * src_ld + cv * 8)), b);
 #pragma unroll
   for (int e = 0; e < 8; ++e) a[e] += b[e];
-  *reinterpret_cast<uint4*>(dst + row * dst_ld + cv * 8) = bm_pack8(a);
+  *reinterpret_cast<uint4*>(dst + row * dst_ld + cv * 8) = Fp16Rows::pack(a);
 }
 
 // ---------------------------------------------------------------- 2x2 parity interleave

@@ -97,6 +97,115 @@ MF_DEVINL void sts32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%
 MF_DEVINL float2 f2_mul(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 MF_DEVINL float2 f2_fma(float2 a, float2 b, float2 c) { return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y)); }
 
+// ------------------------------------------------------------------------------------------------ 8 channels of an activation row
+// The two storage formats of NHWC activation rows, 8 channels (16 bytes per block) at a time. load() only issues the loads
+// and to_f32() converts, so a kernel can issue all its loads before any arithmetic; pack() rounds, store() writes.
+// Fp16Rows: one fp16 block. PairRows (strict precision): v = float(hi) + float(lo) with hi = fp16(v), lo = fp16(v - hi),
+// the lo block `lo` elements after hi in the same row (`lo` is ignored for fp16 rows).
+struct Fp16Rows {
+  static constexpr int kBlocks = 1;
+  using Raw = uint4;
+  MF_DEVINL static Raw load(const __half* p, int) { return __ldg(reinterpret_cast<const uint4*>(p)); }
+  MF_DEVINL static Raw zero() { return make_uint4(0u, 0u, 0u, 0u); }
+  MF_DEVINL static void to_f32(const Raw& v, float (&f)[8]) {
+    const __half2* h = reinterpret_cast<const __half2*>(&v);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 t = __half22float2(h[e]);
+      f[2 * e] = t.x;
+      f[2 * e + 1] = t.y;
+    }
+  }
+  MF_DEVINL static Raw pack(const float (&f)[8]) {
+    __half2 o[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) o[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
+    return *reinterpret_cast<uint4*>(o);
+  }
+  MF_DEVINL static void store(__half* p, int, const Raw& v) { *reinterpret_cast<uint4*>(p) = v; }
+  // MaxPool2d on the fp16 values themselves (exact)
+  MF_DEVINL static Raw max4(const Raw& a, const Raw& b, const Raw& c, const Raw& d) {
+    uint4 o;
+    const __half2 *ha = reinterpret_cast<const __half2*>(&a), *hb = reinterpret_cast<const __half2*>(&b);
+    const __half2 *hc = reinterpret_cast<const __half2*>(&c), *hd = reinterpret_cast<const __half2*>(&d);
+    __half2* ho = reinterpret_cast<__half2*>(&o);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) ho[e] = __hmax2(__hmax2(ha[e], hb[e]), __hmax2(hc[e], hd[e]));
+    return o;
+  }
+};
+
+struct PairRows {
+  static constexpr int kBlocks = 2;
+  struct Raw { uint4 hi, lo; };
+  MF_DEVINL static Raw load(const __half* p, int lo) {
+    return {__ldg(reinterpret_cast<const uint4*>(p)), __ldg(reinterpret_cast<const uint4*>(p + lo))};
+  }
+  MF_DEVINL static Raw zero() { return {make_uint4(0u, 0u, 0u, 0u), make_uint4(0u, 0u, 0u, 0u)}; }
+  MF_DEVINL static void to_f32(const Raw& v, float (&f)[8]) {
+    const __half2* hh = reinterpret_cast<const __half2*>(&v.hi);
+    const __half2* ll = reinterpret_cast<const __half2*>(&v.lo);
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const float2 a = __half22float2(hh[e]), b = __half22float2(ll[e]);
+      f[2 * e] = a.x + b.x;
+      f[2 * e + 1] = a.y + b.y;
+    }
+  }
+  MF_DEVINL static Raw pack(const float (&f)[8]) {
+    __half2 h[4], l[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      h[e] = __floats2half2_rn(f[2 * e], f[2 * e + 1]);
+      const float2 hf = __half22float2(h[e]);
+      l[e] = __floats2half2_rn(f[2 * e] - hf.x, f[2 * e + 1] - hf.y);
+    }
+    return {*reinterpret_cast<uint4*>(h), *reinterpret_cast<uint4*>(l)};
+  }
+  MF_DEVINL static void store(__half* p, int lo, const Raw& v) {
+    *reinterpret_cast<uint4*>(p) = v.hi;
+    *reinterpret_cast<uint4*>(p + lo) = v.lo;
+  }
+  // MaxPool2d on the fp32 values; hi + lo of one input is exactly representable again, so the pair max is lossless
+  MF_DEVINL static Raw max4(const Raw& a, const Raw& b, const Raw& c, const Raw& d) {
+    float fa[8], fb[8], fc[8], fd[8], o[8];
+    to_f32(a, fa);
+    to_f32(b, fb);
+    to_f32(c, fc);
+    to_f32(d, fd);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) o[e] = fmaxf(fmaxf(fa[e], fb[e]), fmaxf(fc[e], fd[e]));
+    return pack(o);
+  }
+};
+
+// ------------------------------------------------------------------------------------------------ edge-fusion sampling point
+// F.grid_sample(bilinear, align_corners=True) coordinate of border position e of image b (edge_idx [B, K, 2] = (x, y) on the
+// out_w x out_h output map) on an H x W map: the top-left corner (x0, y0) and the bilinear weights, in the reference's fp32
+// operation order. The edge gather, its backward and mf_edge_mask all take it from here, so the mask marks exactly the
+// pixels the gather reads.
+struct EdgeSample {
+  int x0, y0;
+  float wx0, wx1, wy0, wy1;
+};
+MF_DEVINL EdgeSample edge_sample(const long long* edge_idx, int b, int K, int e, int H, int W, int out_w, int out_h) {
+  const float ex = static_cast<float>(edge_idx[(static_cast<long long>(b) * K + e) * 2 + 0]);
+  const float ey = static_cast<float>(edge_idx[(static_cast<long long>(b) * K + e) * 2 + 1]);
+  const float gx = ex / static_cast<float>(out_w - 1) * 2.f - 1.f;
+  const float gy = ey / static_cast<float>(out_h - 1) * 2.f - 1.f;
+  const float ix = ((gx + 1.f) / 2.f) * static_cast<float>(W - 1);
+  const float iy = ((gy + 1.f) / 2.f) * static_cast<float>(H - 1);
+  const float x0f = floorf(ix), y0f = floorf(iy);
+  EdgeSample s;
+  s.x0 = static_cast<int>(x0f);
+  s.y0 = static_cast<int>(y0f);
+  s.wx1 = ix - x0f;
+  s.wy1 = iy - y0f;
+  s.wx0 = 1.f - s.wx1;
+  s.wy0 = 1.f - s.wy1;
+  return s;
+}
+
 // ------------------------------------------------------------------------------------------------ cp.async
 // 16-byte global->shared copy; src_bytes == 0 zero-fills the destination (used for conv padding / K tail).
 MF_DEVINL void cp_async16(uint32_t dst_smem, const void* src, uint32_t src_bytes) {

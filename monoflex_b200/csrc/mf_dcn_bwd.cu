@@ -49,14 +49,6 @@ MF_DEVINL void red_add_v4_f16x2(__half* addr, const __half2 (&v)[4]) {
   asm volatile("red.global.add.noftz.v4.f16x2 [%0], {%1, %2, %3, %4};" ::"l"(addr), "r"(u[0]), "r"(u[1]), "r"(u[2]), "r"(u[3])
                : "memory");
 }
-MF_DEVINL void dcn_unpack8(const uint4& v, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&v);
-#pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    const float2 t = __half22float2(h[e]);
-    f[2 * e] = t.x; f[2 * e + 1] = t.y;
-  }
-}
 
 // one thread per (pixel, tap, 8-channel chunk)
 __global__ void __launch_bounds__(256) dcn_sample_cols_kernel(const __half* __restrict__ x, int x_ld, const float* __restrict__ om,
@@ -81,7 +73,7 @@ __global__ void __launch_bounds__(256) dcn_sample_cols_kernel(const __half* __re
 #pragma unroll
     for (int q = 0; q < 4; ++q) {
       float v[8];
-      dcn_unpack8(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<long long>(r.idx[q]) * x_ld)), v);
+      Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<long long>(r.idx[q]) * x_ld)), v);
       const float wq = r.w[q] * r.mask;                       // same rounding points as the fused forward producer
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[e] += wq * v[e];
@@ -116,14 +108,14 @@ __global__ void __launch_bounds__(256) dcn_col2im_kernel(const __half* __restric
     __half* dxb = dx + b * H * W * dx_ld;
     for (int cv = l; cv < CV; cv += L) {
       float g[8];
-      dcn_unpack8(__ldg(reinterpret_cast<const uint4*>(gcol + pix * (9LL * C) + tap * C + cv * 8)), g);
+      Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(gcol + pix * (9LL * C) + tap * C + cv * 8)), g);
       float val[8], vh[8], vw[8];
 #pragma unroll
       for (int e = 0; e < 8; ++e) val[e] = vh[e] = vw[e] = 0.f;
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         float v[8];
-        dcn_unpack8(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<long long>(r.idx[q]) * x_ld + cv * 8)), v);
+        Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(xb + static_cast<long long>(r.idx[q]) * x_ld + cv * 8)), v);
 #pragma unroll
         for (int e = 0; e < 8; ++e) { val[e] += r.w[q] * v[e]; vh[e] += r.dh[q] * v[e]; vw[e] += r.dw[q] * v[e]; }
         if (r.w[q] != 0.f) {

@@ -504,11 +504,8 @@ class Plan(object):
 
     def maxpool2(self, x, out=None):
         y = out if out is not None else self.act(x.B, x.H // 2, x.W // 2, x.C)
-        if x.split:
-            assert y.split
-            self.add("mf_maxpool2_split", lambda: (x.ptr(), x.lo, y.ptr(), y.lo, x.B, x.H, x.W, x.C, x.ld, y.ld))
-            return y
-        self.add("mf_maxpool2_nhwc_f16", lambda: (x.ptr(), y.ptr(), x.B, x.H, x.W, x.C, x.ld, y.ld))
+        assert y.split == x.split
+        self.add("mf_maxpool2_nhwc_f16", lambda: (x.ptr(), x.ld, x.lo, y.ptr(), y.ld, y.lo, x.B, x.H, x.W, x.C))
         if self.train:
             self.tape.append(dict(kind="maxpool2", x=x, y=y))
         return y
@@ -523,15 +520,10 @@ class Plan(object):
             uw = up_weight.detach()
             self.add_py(lambda: wt.copy_(uw.reshape(C, k * k).t()))
         y = self.act(x.B, x.H * f, x.W * f, C)
-        if x.split:
-            assert y.split and (skip is None or skip.split)
-            self.add("mf_upsample_add_split", lambda: (
-                x.ptr(), x.lo, wt.data_ptr(), skip.ptr() if skip is not None else None, skip.lo if skip is not None else 0,
-                y.ptr(), y.lo, x.B, x.H, x.W, C, f, x.ld, skip.ld if skip is not None else 0, y.ld))
-            return y
+        assert y.split == x.split and (skip is None or skip.split == x.split)
         self.add("mf_upsample_add_nhwc_f16", lambda: (
-            x.ptr(), wt.data_ptr(), skip.ptr() if skip is not None else None, y.ptr(), x.B, x.H, x.W, C, f, x.ld,
-            skip.ld if skip is not None else 0, y.ld))
+            x.ptr(), x.ld, x.lo, wt.data_ptr(), skip.ptr() if skip is not None else None, skip.ld if skip is not None else 0,
+            skip.lo if skip is not None else 0, y.ptr(), y.ld, y.lo, x.B, x.H, x.W, C, f))
         if self.train:
             self.tape.append(dict(kind="upsample_add", x=x, weight=up_weight, wt=wt, skip=skip, f=f, y=y))
         return y

@@ -74,14 +74,12 @@ class _predictor(nn.Module):
 
     # ------------------------------------------------------------------ plan
     def build_plan(self, feat, K_edge):
-        """feat: engine.Act-like description of the [B,H,W,64] fp16 feature rows."""
+        """feat: engine.Act of the [B,H,W,64] feature rows (fp16, or hi/lo pairs in strict precision)."""
         dev = feat.buf.device
-        strict = bool(getattr(feat, "split", False))
+        strict = feat.split
         P = engine.Plan(dev, train=self.training, strict=strict)
         B, H, W, hc = feat.B, feat.H, feat.W, self.head_conv
-        x = P.act(B, H, W, feat.C)
-        x.buf, x.ch_off, x.owner = feat.buf, feat.ch_off, None
-        P.acts.remove(x)                                  # externally owned storage
+        x = feat
         branches = [self.class_head] + list(self.reg_features)
         w_all = torch.cat([b[0].weight.detach() for b in branches], 0)          # [2304, 64, 3, 3]
 
@@ -152,12 +150,10 @@ class _predictor(nn.Module):
             ncls_, nreg_, hw_ = self.num_classes, self.num_reg, H * W
             P.add("mf_head2_reduce", lambda: (part.data_ptr(), head_bias.data_ptr(), cls.data_ptr(), reg.data_ptr(), B, ncls_,
                                               nreg_, hw_))
-
-            class _Hid(object):
-                pass
-            hid = _Hid()
-            hid.ptr = lambda: hid_buf.data_ptr()
-            hid.ld, hid.lo = 4 * hc, 2 * hc
+            hid = None
+            if hid_buf is not None:
+                hid = engine.Act.on(hid_buf, B, H, W, 2 * hc)
+                hid.split = True
             edge_cols = (0, hc)
         elif fused:
             # ---- one kernel: 9 x (3x3 conv + IABN) + every 1x1 head; hidden activations stay on chip (csrc/mf_head.cu)
@@ -203,12 +199,7 @@ class _predictor(nn.Module):
                 nb, ctypes.cast(arr_p, ctypes.c_void_p), ctypes.cast(arr_ct, ctypes.c_void_p),
                 ctypes.cast(arr_nc, ctypes.c_void_p), ctypes.cast(arr_hc, ctypes.c_void_p), hid_buf.data_ptr(), hid_ld,
                 mask_ptr))
-
-            class _Hid(object):
-                pass
-            hid = _Hid()
-            hid.ptr = lambda: hid_buf.data_ptr()
-            hid.ld = hid_ld
+            hid = engine.Act.on(hid_buf, B, H, W)
             edge_cols = (0, hc)
         else:
             # train mode: every branch normalises with its own InPlaceABN module (batch statistics, running-stat update)
@@ -238,12 +229,8 @@ class _predictor(nn.Module):
             ea = P.act(B, 1, K_edge + 2, hc)
             eb = P.act(B, 1, K_edge + 2, hc)
             ow, oh = self.output_width, self.output_height
-            if strict:
-                P.add("mf_edge_gather_split", lambda: (hid.ptr(), hid.ld, hid.lo, edge_cols[0], edge_cols[1],
-                                                        P.edge_idx.data_ptr(), ea.ptr(), eb.ptr(), B, H, W, K_edge, ow, oh))
-            else:
-                P.add("mf_edge_gather", lambda: (hid.ptr(), hid.ld, edge_cols[0], edge_cols[1], P.edge_idx.data_ptr(), ea.ptr(),
-                                                  eb.ptr(), B, H, W, K_edge, ow, oh))
+            P.add("mf_edge_gather", lambda: (hid.ptr(), hid.ld, hid.lo, edge_cols[0], edge_cols[1], P.edge_idx.data_ptr(),
+                                              ea.ptr(), eb.ptr(), B, H, W, K_edge, ow, oh))
             for src, seq, dst, ch0, ctot in ((ea, self.trunc_heatmap_conv, cls, 0, self.num_classes),
                                              (eb, self.trunc_offset_conv, reg, off_ch0, self.num_reg)):
                 t = P.conv(src, seq[0].weight, 1, 0, seq[1], bias=seq[0].bias, act=engine.ACT_NONE)   # [B,1,K,256]
@@ -251,14 +238,9 @@ class _predictor(nn.Module):
                 b2 = seq[3].bias.detach().float().contiguous()
                 P.keep.extend([w2, b2])
                 n_out = w2.shape[0]
-                if strict:
-                    P.add("mf_edge_head_add_split", lambda t=t, w2=w2, b2=b2, n_out=n_out, dst=dst, ch0=ch0, ctot=ctot: (
-                        t.ptr(), t.ld, t.lo, w2.data_ptr(), b2.data_ptr(), n_out, P.edge_idx.data_ptr(), P.edge_len.data_ptr(),
-                        dst.data_ptr(), ctot, ch0, B, K_edge, H, W))
-                else:
-                    P.add("mf_edge_head_add", lambda t=t, w2=w2, b2=b2, n_out=n_out, dst=dst, ch0=ch0, ctot=ctot: (
-                        t.ptr(), w2.data_ptr(), b2.data_ptr(), n_out, P.edge_idx.data_ptr(), P.edge_len.data_ptr(),
-                        dst.data_ptr(), ctot, ch0, B, K_edge, H, W))
+                P.add("mf_edge_head_add", lambda t=t, w2=w2, b2=b2, n_out=n_out, dst=dst, ch0=ch0, ctot=ctot: (
+                    t.ptr(), t.ld, t.lo, w2.data_ptr(), b2.data_ptr(), n_out, P.edge_idx.data_ptr(), P.edge_len.data_ptr(),
+                    dst.data_ptr(), ctot, ch0, B, K_edge, H, W))
         n_cls = cls.numel()
         P.add("mf_sigmoid_clamp", lambda: (cls.data_ptr(), n_cls))
         P.finalize()
@@ -275,7 +257,7 @@ class _predictor(nn.Module):
     def plan_for(self, features, K_edge):
         feat = _as_rows(features)
         key = (feat.buf.data_ptr(), feat.ch_off, feat.B, feat.H, feat.W, feat.buf.shape[1], K_edge,
-               engine.fingerprint(self, versions=not self.training), bool(getattr(feat, "split", False)))
+               engine.fingerprint(self, versions=not self.training), feat.split)
         plan = self._plans.get('plan')
         if plan is None or self._plans.get('key') != key:
             plan = self.build_plan(feat, K_edge)
@@ -307,35 +289,28 @@ class _predictor(nn.Module):
         return {'cls': plan.cls, 'reg': plan.reg}
 
 
-class _Rows(object):
-    pass
-
-
 def _as_rows(features):
-    """Accept the backbone's zero-copy channels-last fp16 view, or any [B,C,H,W] CUDA tensor (converted by a kernel)."""
+    """-> engine.Act over the predictor's input rows. Accepts the backbone's zero-copy channels-last fp16 view, or any
+    [B,C,H,W] CUDA tensor (converted by a kernel)."""
     act = features if isinstance(features, engine.Act) else getattr(features, "_mf_act", None)
     if act is not None:                          # the backbone plan's own output rows (strict precision: hi/lo pairs)
-        r = _Rows()
-        r.B, r.H, r.W, r.C, r.ch_off, r.buf, r.split = act.B, act.H, act.W, act.C, act.ch_off, act.buf, act.split
+        r = engine.Act.on(act.buf, act.B, act.H, act.W, act.C, act.ch_off)
+        r.split = act.split
         return r
     if not features.is_cuda:
         raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
     B, C, H, W = features.shape
-    r = _Rows()
-    r.B, r.H, r.W, r.C, r.ch_off, r.split = B, H, W, C, 0, False
     if features.dtype == torch.half and features.stride(1) == 1 and features.stride(3) % 8 == 0 and \
             features.stride(2) == W * features.stride(3) and features.stride(0) == H * features.stride(2):
         ld = features.stride(3)
         base = features.permute(0, 2, 3, 1)                     # [B,H,W,C] view
-        r.ch_off = base.storage_offset() % ld
-        rows = torch.as_strided(base, (B * H * W, ld), (ld, 1), storage_offset=base.storage_offset() - r.ch_off)
-        r.buf = rows
-        return r
+        ch_off = base.storage_offset() % ld
+        rows = torch.as_strided(base, (B * H * W, ld), (ld, 1), storage_offset=base.storage_offset() - ch_off)
+        return engine.Act.on(rows, B, H, W, C, ch_off)
     x = features.float().contiguous()
     buf = torch.empty(B * H * W, C, dtype=torch.half, device=x.device)
     call("mf_nchw_f32_to_nhwc_f16", x.data_ptr(), buf.data_ptr(), B, C, H * W, C, stream())
-    r.buf = buf
-    return r
+    return engine.Act.on(buf, B, H, W)
 
 
 def make_predictor(cfg, in_channels):

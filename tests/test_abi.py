@@ -90,6 +90,30 @@ def test_version_and_error_string(lib):
     assert b"not built" in lib.mf_last_error()
 
 
+# the layout entry points that take pair rows or fp16 rows by their lo offsets, called with offsets they must refuse before
+# any CUDA call (no device needed): (name, args without the stream)
+P = 16                  # a non-null pointer that is never dereferenced
+BAD_LO = [
+    ("mf_maxpool2_nhwc_f16", (P, 64, 0, P, 64, 32, 2, 4, 4, 32)),                       # fp16 x, pair y
+    ("mf_maxpool2_nhwc_f16", (P, 64, 32, P, 64, 0, 2, 4, 4, 32)),                       # pair x, fp16 y
+    ("mf_maxpool2_nhwc_f16", (P, 64, 36, P, 64, 32, 2, 4, 4, 32)),                      # x_lo not a multiple of 8
+    ("mf_upsample_add_nhwc_f16", (P, 64, 32, P, P, 64, 0, P, 64, 32, 2, 4, 4, 32, 2)),  # fp16 skip, pair x and y
+    ("mf_upsample_add_nhwc_f16", (P, 64, 0, P, None, 0, 0, P, 64, 32, 2, 4, 4, 32, 4)),  # fp16 x, pair y, no skip
+    ("mf_upsample_add_nhwc_f16", (P, 64, 32, P, P, 64, 36, P, 64, 32, 2, 4, 4, 32, 2)),  # skip_lo not a multiple of 8
+    ("mf_edge_gather", (P, 1024, 516, 0, 256, P, P, P, 2, 4, 4, 8, 16, 16)),             # feat_lo not a multiple of 8
+    ("mf_edge_head_add", (P, 512, 260, P, P, 2, P, P, P, 3, 0, 2, 8, 4, 4)),             # t_lo not a multiple of 8
+]
+
+
+@pytest.mark.parametrize("name,args", BAD_LO, ids=["%s-%d" % (n, i) for i, (n, _) in enumerate(BAD_LO)])
+def test_row_format_errors(name, args):
+    """mixed row formats and lo offsets off the 16-byte grid are refused with a message, before any CUDA call"""
+    from monoflex_b200 import _lib
+    lib = _lib.load()
+    assert getattr(lib, name)(*args, None) == -1
+    assert b"lo offsets must all be 0" in lib.mf_last_error()
+
+
 def test_conv_block_n(lib):
     assert [lib.mf_conv_block_n(c) for c in (3, 16, 27, 32, 64, 128, 256, 2304)] == [16, 16, 32, 32, 64, 128, 128, 128]
 

@@ -73,11 +73,24 @@ LAUNCHES = {
     ("conv_rows", "fast"): ("mf_conv2d_rows_f16",),
     ("dcn", "strict"): ("mf_conv2d_nhwc_f16x2", "mf_dcn_nhwc_f16x2"),
     ("dcn", "fast"): ("mf_conv2d_nhwc_f16", "mf_dcn_nhwc_f16"),
-    ("maxpool2", "strict"): ("mf_maxpool2_split",),
-    ("maxpool2", "fast"): ("mf_maxpool2_nhwc_f16",),
-    ("upsample_add", "strict"): ("mf_upsample_add_split",),
-    ("upsample_add", "fast"): ("mf_upsample_add_nhwc_f16",),
+    ("maxpool2", "strict"): lambda op: row_format_launch(op, "mf_maxpool2_nhwc_f16", True),
+    ("maxpool2", "fast"): lambda op: row_format_launch(op, "mf_maxpool2_nhwc_f16", False),
+    ("upsample_add", "strict"): lambda op: row_format_launch(op, "mf_upsample_add_nhwc_f16", True),
+    ("upsample_add", "fast"): lambda op: row_format_launch(op, "mf_upsample_add_nhwc_f16", False),
 }
+# argument positions of the lo offsets of the launches that read and write either row format (include/monoflex_b200.h);
+# the up-sample's skip_lo (6) only counts with a skip input (argument 4)
+LO_ARGS = {"mf_maxpool2_nhwc_f16": (2, 5), "mf_upsample_add_nhwc_f16": (2, 6, 9)}
+
+
+def row_format_launch(op, name, pair):
+    """(name,) when the op's launch passes pair-row lo offsets (all non-zero) in a strict plan and fp16 rows (all zero) in
+    a fast one; otherwise a description of the wrong format, which no launch list matches"""
+    args = op.plan.launches[op.first][1]
+    lo = [args[i] for i in LO_ARGS[name] if not (name == "mf_upsample_add_nhwc_f16" and i == 6 and args[4] is None)]
+    if all((v != 0) == pair for v in lo):
+        return (name,)
+    return ("%s with lo offsets %s" % (name, lo),)
 
 
 # ------------------------------------------------------------------------------------------------ recording the plan
@@ -523,8 +536,8 @@ def slice_act(v, pad, split, device="cuda"):
 @pytest.mark.parametrize("split", [True, False], ids=["split", "f16"])
 @pytest.mark.parametrize("f,C,skip", UP_CASES, ids=["f%d-C%d-%s" % (f, C, "skip" if s else "noskip") for f, C, s in UP_CASES])
 def test_upsample_add_slices(f, C, skip, split):
-    """mf_upsample_add_split / mf_upsample_add_nhwc_f16 on inputs that are channel slices of wider buffers (different
-    offsets and lo positions for x and skip, NaN in every column outside the slices), ragged 5x7 maps, against float64"""
+    """mf_upsample_add_nhwc_f16 on pair rows and fp16 rows that are channel slices of wider buffers (different offsets
+    and lo positions for x and skip, NaN in every column outside the slices), ragged 5x7 maps, against float64"""
     gen = np.random.Generator(np.random.PCG64(100 * f + C + skip))
     B, Hi, Wi = 2, 5, 7
     xv = torch.from_numpy(gen.standard_normal((B, C, Hi, Wi)).astype(np.float32))
@@ -547,8 +560,9 @@ def test_upsample_add_slices(f, C, skip, split):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("C", [64, 128, 256])
-def test_maxpool2_split_slices(C):
-    """mf_maxpool2_split from one concat slice into another: bit-exact pair values, every other column untouched"""
+def test_maxpool2_pair_slices(C):
+    """mf_maxpool2_nhwc_f16 on pair rows, from one concat slice into another: bit-exact pair values, every other column
+    untouched"""
     gen = np.random.Generator(np.random.PCG64(C))
     B, H, W = 2, 10, 14
     xv = torch.from_numpy(gen.standard_normal((B, C, H, W)).astype(np.float32))
@@ -665,11 +679,24 @@ def test_coverage_check_finds_unchecked_launches():
     """check_coverage reports a launch no recorded op claims, and an op that emitted launches of another kind"""
     class O(object):
         def __init__(self, kind, first, end):
-            self.kind, self.first, self.end = kind, first, end
-    names = ["mf_conv2d_nhwc_f16x2", "mf_conv2d_nhwc_f16x2", "mf_dcn_nhwc_f16x2", "mf_maxpool2_split"]
+            self.kind, self.first, self.end, self.plan = kind, first, end, plan
+    plan = engine.Plan("cpu")
+    names = ["mf_conv2d_nhwc_f16x2", "mf_conv2d_nhwc_f16x2", "mf_dcn_nhwc_f16x2", "mf_maxpool2_nhwc_f16"]
+    pool_args = (0, 128, 64, 0, 128, 64, 2, 10, 14, 64)        # x, x_ld, x_lo, y, y_ld, y_lo: pair rows
+    plan.launches = [(None, (), n) for n in names[:3]] + [(None, pool_args, names[3])]
     ops = [O("conv", 0, 1), O("dcn", 1, 3), O("maxpool2", 3, 4)]
     assert check_coverage(ops, names, "strict") == []
     assert len(check_coverage(ops[:2], names, "strict")) == 1                       # the max-pool launch unclaimed
     assert len(check_coverage([O("conv", 0, 1), O("maxpool2", 3, 4)], names, "strict")) == 1
     assert len(check_coverage(ops, names, "fast")) == 3                              # strict launches in a fast plan
     assert check_coverage([O("new_op", 0, 4)], names, "strict") != []
+    # the same launch name on fp16 rows in a strict plan, or with one lo offset missing, is reported
+    for lo in ((0, 0), (64, 0)):
+        plan.launches[3] = (None, pool_args[:2] + lo[:1] + pool_args[3:5] + lo[1:] + pool_args[6:], names[3])
+        assert len(check_coverage(ops, names, "strict")) == 1, lo
+    # ... and in a fast plan the fp16-row launch is accepted, the pair-row one reported
+    fast = ["mf_conv2d_nhwc_f16", "mf_conv2d_nhwc_f16", "mf_dcn_nhwc_f16", "mf_maxpool2_nhwc_f16"]
+    plan.launches[3] = (None, (0, 64, 0, 0, 64, 0, 2, 10, 14, 64), names[3])
+    assert check_coverage(ops, fast, "fast") == []
+    plan.launches[3] = (None, pool_args, names[3])
+    assert len(check_coverage(ops, fast, "fast")) == 1

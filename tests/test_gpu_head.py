@@ -49,11 +49,12 @@ CASES = [
 CASE_IDS = ["%dx%dx%d" % c[:3] for c in CASES]
 
 PATH_LAUNCHES = {
-    "head2": {"mf_edge_mask", "mf_head_conv_f16x2", "mf_head2_reduce", "mf_edge_gather_split", "mf_conv2d_nhwc_f16x2",
-              "mf_edge_head_add_split", "mf_sigmoid_clamp"},
-    "split": {"mf_conv2d_nhwc_f16x2", "mf_edge_gather_split", "mf_edge_head_add_split", "mf_sigmoid_clamp"},
+    "head2": {"mf_edge_mask", "mf_head_conv_f16x2", "mf_head2_reduce", "mf_edge_gather", "mf_conv2d_nhwc_f16x2",
+              "mf_edge_head_add", "mf_sigmoid_clamp"},
+    "split": {"mf_conv2d_nhwc_f16x2", "mf_edge_gather", "mf_edge_head_add", "mf_sigmoid_clamp"},
     "fused": {"mf_edge_mask", "mf_head_fused", "mf_edge_gather", "mf_conv2d_nhwc_f16", "mf_edge_head_add", "mf_sigmoid_clamp"},
 }
+EDGE_LO_ARG = {"mf_edge_gather": 2, "mf_edge_head_add": 2}     # feat_lo / t_lo: non-zero = pair rows
 PREFIX = "heads.predictor."
 
 
@@ -174,6 +175,9 @@ def check(precision, path, x, pred, act, idx, lens, pads, label):
     g = run_gpu(pred, act, targets_of(W, H, idx, lens, pads))
     names = {name for _, _, name in g['plan'].launches}
     assert names == PATH_LAUNCHES[path], names
+    # the edge launches read pair rows on the strict paths, fp16 rows on the fast one
+    lo = [(name, args[EDGE_LO_ARG[name]]) for _, args, name in g['plan'].launches if name in EDGE_LO_ARG]
+    assert len(lo) == 3 and all((v != 0) == (precision == "strict") for _, v in lo), lo
     if path == "split":
         assert g['mask'] is None
     else:

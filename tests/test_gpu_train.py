@@ -518,7 +518,8 @@ def test_edge_gather_backward_is_the_transpose():
     feat = torch.from_numpy((gen.standard_normal((B * H * W, 512)) * 0.5).astype(np.float32)).half().cuda()
     ea = torch.zeros(B, K + 2, 256, dtype=torch.half, device="cuda")
     eb = torch.zeros_like(ea)
-    call("mf_edge_gather", feat.data_ptr(), 512, 0, 256, edge.data_ptr(), ea.data_ptr(), eb.data_ptr(), B, H, W, K, 320, 96, stream())
+    call("mf_edge_gather", feat.data_ptr(), 512, 0, 0, 256, edge.data_ptr(), ea.data_ptr(), eb.data_ptr(), B, H, W, K, 320, 96,
+         stream())
     da = torch.from_numpy(gen.standard_normal((B, K + 2, 256)).astype(np.float32)).half().cuda()
     db = torch.from_numpy(gen.standard_normal((B, K + 2, 256)).astype(np.float32)).half().cuda()
     dfeat = torch.zeros_like(feat)

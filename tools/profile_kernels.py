@@ -47,7 +47,7 @@ if model.precision == "strict":
         ("conv512", bp, "mf_conv2d_nhwc_f16x2", lambda a: a[14] == 512 and a[6] == 512 and a[10] == 3),
         ("stem", bp, "mf_conv2d_rows_f16x2", lambda a: a[4] == 8),
         ("level0", bp, "mf_conv2d_rows_f16x2", lambda a: a[4] == 16),
-        ("upadd", bp, "mf_upsample_add_split", lambda a: a[10] == 160),
+        ("upadd", bp, "mf_upsample_add_nhwc_f16", lambda a: a[12] == 160),
     ]
 else:
     sel_spec = [
@@ -59,7 +59,7 @@ else:
         ("conv64", bp, "mf_conv2d_nhwc_f16", lambda a: a[13] == 64 and a[5] == 64 and a[9] == 3),
         ("stem", bp, "mf_conv2d_rows_f16", lambda a: a[4] == 8),
         ("level0", bp, "mf_conv2d_rows_f16", lambda a: a[4] == 16 and a[5] == 1),
-        ("upadd", bp, "mf_upsample_add_nhwc_f16", lambda a: a[6] == 160),
+        ("upadd", bp, "mf_upsample_add_nhwc_f16", lambda a: a[12] == 160),
     ]
 only = os.environ.get("ONLY")
 sel = [(n, pick(pl, k, pred)) for n, pl, k, pred in sel_spec if not only or n in only.split(",")]
