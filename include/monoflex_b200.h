@@ -431,6 +431,16 @@ int mf_decode_detections(const float* heat, const float* reg, const float* calib
                          int depth_mode, const float* gt, int G, float* ws_score, int* ws_idx, float* scores,
                          long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
                          float* depth_err, float* proj, int* min_unc, void* stream);
+/* mf_decode_detections for several estimators from one NMS / top-k / POI gather: depth_modes is a HOST array of
+ * 1 <= n_modes <= 9 distinct depth_mode values, decoded in that order (gt is needed when one of them is the oracle).
+ * The per-mode outputs take a leading mode dimension: result [n_modes,B,K,14], depth_err and min_unc [n_modes,B,K];
+ * block m equals what mf_decode_detections writes for depth_modes[m]. The other outputs are written once, as there. */
+int mf_decode_detections_depths(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
+                                const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh,
+                                int apply_sigmoid, const int* depth_modes, int n_modes, const float* gt, int G,
+                                float* ws_score, int* ws_idx, float* scores, long long* inds, float* clses, float* ys,
+                                float* xs, float* pois, float* result, int* count, float* depth_err, float* proj,
+                                int* min_unc, void* stream);
 
 /* ---- KITTI official metric (data/datasets/evaluation/kitti_object_eval_python/eval.py:644-726, rotate_iou.py) ---------
  * Objects: float64 rows of MF_KITTI_OBJ values, CSR-packed per image (gt_off / dt_off: DEVICE int32 [n_img + 1]):

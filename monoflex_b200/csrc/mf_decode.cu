@@ -14,7 +14,7 @@
 
 namespace mf {
 
-// OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode`
+// OUTPUT_DEPTH estimators of the decode (detector_infer.py:148-209); the values are the C ABI's `depth_mode` / `depth_modes`
 enum {
   MF_DEPTH_SOFT = 0, MF_DEPTH_HARD = 1, MF_DEPTH_MEAN = 2, MF_DEPTH_ORACLE = 3, MF_DEPTH_DIRECT = 4,
   MF_DEPTH_KEYPOINTS_AVG = 5, MF_DEPTH_KEYPOINTS_CENTER = 6, MF_DEPTH_KEYPOINTS_02 = 7, MF_DEPTH_KEYPOINTS_13 = 8,
@@ -270,16 +270,17 @@ struct DecodeParams {
   float* ys;              // [B, K]
   float* xs;              // [B, K]
   float* pois;            // [B, K, R]
-  float* result;          // [B, K, 14]
+  float* result;          // [M, B, K, 14]
   int* count;             // [B]
-  // OUTPUT_DEPTH estimator (MF_DEPTH_* above) and, for the oracle, the ground truth of every image:
-  // gt [B, G, 7] = (valid, class, x1, y1, x2, y2, z)
-  int depth_mode;
+  // the M = n_modes OUTPUT_DEPTH estimators (MF_DEPTH_* above) to decode, 4 bits each, the m-th at bits [4m, 4m + 4),
+  // and, for the oracle, the ground truth of every image: gt [B, G, 7] = (valid, class, x1, y1, x2, y2, z)
+  unsigned long long modes;
+  int n_modes;
   const float* gt;
   int G;
-  float* depth_err;       // [B, K] estimated depth error of the chosen depth
+  float* depth_err;       // [M, B, K] estimated depth error of the chosen depth
   float* proj;            // [B, K, 2] projected 3D centre on the output map (xs + off_x, ys + off_y)
-  int* min_unc;           // [B, K] argmax(1 / sigma) of the four estimators (ensemble modes), else -1
+  int* min_unc;           // [M, B, K] argmax(1 / sigma) of the four estimators (ensemble modes), else -1
 };
 
 // The oracle of detector_infer.py:239-278 for one detection: start from the mean of the four estimators, match the
@@ -437,53 +438,12 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
     dep[i] = fminf(fmaxf(dep[i], 0.1f), 100.f);
     sig[i] = expf(q[26 + i - 1]);
   }
-  // OUTPUT_DEPTH selection detector_infer.py:148-209. The four ensemble modes report the estimator of largest weight
-  // 1 / sigma (first maximum, :185); `hard` takes its depth.
-  float depth = 0.f, err = 0.f;
-  int min_unc = -1;
-  float dbest = dep[0], smin = sig[0];
-  if (p.depth_mode <= MF_DEPTH_ORACLE) {
-    float wbest = 1.f / sig[0];
-    min_unc = 0;
-#pragma unroll
-    for (int i = 1; i < 4; ++i) {
-      const float w = 1.f / sig[i];
-      if (w > wbest) { wbest = w; dbest = dep[i]; min_unc = i; }
-      smin = fminf(smin, sig[i]);
-    }
-  }
-  if (p.depth_mode == MF_DEPTH_SOFT) {
-    // soft ensemble :193-198
-    float wsum = 0.f, wts[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { wts[i] = 1.f / sig[i]; wsum += wts[i]; }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) { const float wn = wts[i] / wsum; depth += dep[i] * wn; err += wn * sig[i]; }
-  } else if (p.depth_mode == MF_DEPTH_HARD) {                   // :187-191
-    depth = dbest; err = smin;
-  } else if (p.depth_mode == MF_DEPTH_MEAN || p.depth_mode == MF_DEPTH_ORACLE) {   // :200-209
-    depth = (dep[0] + dep[1] + dep[2] + dep[3]) / 4.f; err = (sig[0] + sig[1] + sig[2] + sig[3]) / 4.f;
-    if (p.depth_mode == MF_DEPTH_ORACLE)
-      oracle_depth(p.gt + static_cast<long long>(b) * p.G * 7, p.G, cls, x1, y1, x2, y2, dep, sig, depth, err);
-  } else if (p.depth_mode == MF_DEPTH_DIRECT) {                 // :150-153
-    depth = dep[0]; err = sig[0];
-  } else if (p.depth_mode == MF_DEPTH_KEYPOINTS_AVG) {          // :156-158: mean over the three key-point depths
-    depth = (dep[1] + dep[2] + dep[3]) / 3.f; err = (sig[1] + sig[2] + sig[3]) / 3.f;
-  } else {                                                      // :160-170: keypoints_center / _02 / _13
-    const int i = p.depth_mode - MF_DEPTH_KEYPOINTS_CENTER + 1;
-    depth = i == 1 ? dep[1] : i == 2 ? dep[2] : dep[3];
-    err = i == 1 ? sig[1] : i == 2 ? sig[2] : sig[3];
-  }
-  p.depth_err[o] = err;
-  p.min_unc[o] = min_unc;
-  // projected 3D centre on the map (:125), then location :142-155 + kitti_utils.py:350-369
+  // projected 3D centre on the map (:125) and the multi-bin orientation :245-295: argmax over softmax(bin logits)[..., 1]
+  // (first max wins); neither depends on the depth
   const float px = xf + q[4], py = yf + q[5];
   p.proj[o * 2] = px;
   p.proj[o * 2 + 1] = py;
   const float u = px * dr - padx, v = py * dr - pady;
-  const float lx = ((u - c_u) * depth) / f_u + b_x;
-  float ly = ((v - c_v) * depth) / f_v + b_y;
-  // multi-bin orientation :245-295: argmax over softmax(bin logits)[..., 1] (first max wins)
   int bi = 0; float best = -1.f;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
@@ -495,18 +455,63 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   }
   const float PI_F = 3.14159265358979323846f;
   const float centers[4] = {0.f, PI_F / 2.f, PI_F, -PI_F / 2.f};
-  float alpha = atan2f(q[40 + 2 * bi], q[40 + 2 * bi + 1]) + centers[bi];
-  const float ray = atan2f(lx, depth);
-  float roty = alpha + ray;
-  if (roty > PI_F) roty -= 2.f * PI_F;
-  if (roty < -PI_F) roty += 2.f * PI_F;
+  const float alpha_raw = atan2f(q[40 + 2 * bi], q[40 + 2 * bi + 1]) + centers[bi];
+  float alpha = alpha_raw;
   if (alpha > PI_F) alpha -= 2.f * PI_F;
   if (alpha < -PI_F) alpha += 2.f * PI_F;
-  ly += dh / 2.f;
-  const float conf = score * (1.f - fminf(fmaxf(err, 0.01f), 1.f));
-  float* r = p.result + o * 14;
-  r[0] = static_cast<float>(cls); r[1] = alpha; r[2] = x1; r[3] = y1; r[4] = x2; r[5] = y2;
-  r[6] = dh; r[7] = dw; r[8] = dl; r[9] = lx; r[10] = ly; r[11] = depth; r[12] = roty; r[13] = conf;
+  // The four ensemble modes report the estimator of largest weight 1 / sigma (first maximum, :185); `hard` takes its depth.
+  float dbest = dep[0], smin = sig[0], wbest = 1.f / sig[0];
+  int unc_best = 0;
+#pragma unroll
+  for (int i = 1; i < 4; ++i) {
+    const float w = 1.f / sig[i];
+    if (w > wbest) { wbest = w; dbest = dep[i]; unc_best = i; }
+    smin = fminf(smin, sig[i]);
+  }
+  // Everything above is shared by the estimators. From the OUTPUT_DEPTH selection (detector_infer.py:148-209) on, each of
+  // the M modes writes its own [B, K] block of result / depth_err / min_unc.
+  const long long BK = static_cast<long long>(p.B) * p.K;
+  for (int m = 0; m < p.n_modes; ++m) {
+    const int mode = static_cast<int>((p.modes >> (4 * m)) & 15ull);
+    const long long om = m * BK + o;
+    float depth = 0.f, err = 0.f;
+    if (mode == MF_DEPTH_SOFT) {
+      // soft ensemble :193-198
+      float wsum = 0.f, wts[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { wts[i] = 1.f / sig[i]; wsum += wts[i]; }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) { const float wn = wts[i] / wsum; depth += dep[i] * wn; err += wn * sig[i]; }
+    } else if (mode == MF_DEPTH_HARD) {                         // :187-191
+      depth = dbest; err = smin;
+    } else if (mode == MF_DEPTH_MEAN || mode == MF_DEPTH_ORACLE) {   // :200-209
+      depth = (dep[0] + dep[1] + dep[2] + dep[3]) / 4.f; err = (sig[0] + sig[1] + sig[2] + sig[3]) / 4.f;
+      if (mode == MF_DEPTH_ORACLE)
+        oracle_depth(p.gt + static_cast<long long>(b) * p.G * 7, p.G, cls, x1, y1, x2, y2, dep, sig, depth, err);
+    } else if (mode == MF_DEPTH_DIRECT) {                       // :150-153
+      depth = dep[0]; err = sig[0];
+    } else if (mode == MF_DEPTH_KEYPOINTS_AVG) {                // :156-158: mean over the three key-point depths
+      depth = (dep[1] + dep[2] + dep[3]) / 3.f; err = (sig[1] + sig[2] + sig[3]) / 3.f;
+    } else {                                                    // :160-170: keypoints_center / _02 / _13
+      const int i = mode - MF_DEPTH_KEYPOINTS_CENTER + 1;
+      depth = i == 1 ? dep[1] : i == 2 ? dep[2] : dep[3];
+      err = i == 1 ? sig[1] : i == 2 ? sig[2] : sig[3];
+    }
+    p.depth_err[om] = err;
+    p.min_unc[om] = mode <= MF_DEPTH_ORACLE ? unc_best : -1;
+    // location :142-155 + kitti_utils.py:350-369
+    const float lx = ((u - c_u) * depth) / f_u + b_x;
+    float ly = ((v - c_v) * depth) / f_v + b_y;
+    const float ray = atan2f(lx, depth);
+    float roty = alpha_raw + ray;
+    if (roty > PI_F) roty -= 2.f * PI_F;
+    if (roty < -PI_F) roty += 2.f * PI_F;
+    ly += dh / 2.f;
+    const float conf = score * (1.f - fminf(fmaxf(err, 0.01f), 1.f));
+    float* r = p.result + om * 14;
+    r[0] = static_cast<float>(cls); r[1] = alpha; r[2] = x1; r[3] = y1; r[4] = x2; r[5] = y2;
+    r[6] = dh; r[7] = dw; r[8] = dl; r[9] = lx; r[10] = ly; r[11] = depth; r[12] = roty; r[13] = conf;
+  }
 }
 
 }  // namespace mf
@@ -521,18 +526,39 @@ int mf_nms_hm(const float* hm, float* out, int planes, int H, int W, void* strea
   return check_cuda(cudaGetLastError(), "nms_hm");
 }
 
-int mf_decode_detections(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
-                         const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
-                         int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores,
-                         long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
-                         float* depth_err, float* proj, int* min_unc, void* stream) {
-  if (depth_mode < 0 || depth_mode >= MF_DEPTH_MODES) {
-    set_error("decode: depth_mode %d is not one of the %d OUTPUT_DEPTH estimators", depth_mode, MF_DEPTH_MODES);
+}  // extern "C"
+
+namespace {
+
+// Both decode entry points: stage 1 once, then one stage-2 launch that decodes the n_modes estimators of the host array
+// depth_modes (validated here) into n_modes blocks of result / depth_err / min_unc.
+int decode_launch(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
+                  const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
+                  const int* depth_modes, int n_modes, const float* gt, int G, float* s1_score, int* s1_idx, float* scores,
+                  long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
+                  float* depth_err, float* proj, int* min_unc, void* stream) {
+  if (depth_modes == nullptr || n_modes < 1 || n_modes > MF_DEPTH_MODES) {
+    set_error("decode: %d depth modes; between 1 and %d OUTPUT_DEPTH estimators can be decoded at once", n_modes, MF_DEPTH_MODES);
     return -1;
   }
-  if (depth_mode == MF_DEPTH_ORACLE && (gt == nullptr || G < 0)) {
-    set_error("decode: the oracle depth needs the ground-truth table gt [B, G, 7] (gt=%p, G=%d)", static_cast<const void*>(gt), G);
-    return -1;
+  unsigned long long modes = 0ull;
+  unsigned int seen = 0u;
+  for (int m = 0; m < n_modes; ++m) {
+    const int depth_mode = depth_modes[m];
+    if (depth_mode < 0 || depth_mode >= MF_DEPTH_MODES) {
+      set_error("decode: depth_mode %d is not one of the %d OUTPUT_DEPTH estimators", depth_mode, MF_DEPTH_MODES);
+      return -1;
+    }
+    if (seen & (1u << depth_mode)) {
+      set_error("decode: depth_mode %d is listed twice", depth_mode);
+      return -1;
+    }
+    if (depth_mode == MF_DEPTH_ORACLE && (gt == nullptr || G < 0)) {
+      set_error("decode: the oracle depth needs the ground-truth table gt [B, G, 7] (gt=%p, G=%d)", static_cast<const void*>(gt), G);
+      return -1;
+    }
+    seen |= 1u << depth_mode;
+    modes |= static_cast<unsigned long long>(depth_mode) << (4 * m);
   }
   // torch.topk raises for K > H*W; here the empty slots would decode as rows with a NaN score
   if (K < 1 || K > 64 || K > H * W) {
@@ -582,9 +608,33 @@ int mf_decode_detections(const float* heat, const float* reg, const float* calib
   p.dim_mean = dim_mean; p.B = B; p.C = C; p.K = K; p.R = R; p.H = H; p.W = W; p.S = S; p.thresh = thresh; p.down_ratio = 4;
   p.scores = scores; p.inds = inds; p.clses = clses; p.ys = ys; p.xs = xs; p.pois = pois; p.result = result;
   p.count = count;
-  p.depth_mode = depth_mode; p.gt = gt; p.G = G; p.depth_err = depth_err; p.proj = proj; p.min_unc = min_unc;
+  p.modes = modes; p.n_modes = n_modes; p.gt = gt; p.G = G; p.depth_err = depth_err; p.proj = proj; p.min_unc = min_unc;
   (void)launch_k(topk_decode_stage2_kernel, dim3(B), dim3(S2_THREADS), 0, MF_STREAM(stream), p);
   return check_cuda(cudaGetLastError(), "topk_decode_stage2");
+}
+
+}  // namespace
+
+extern "C" {
+
+int mf_decode_detections(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
+                         const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh, int apply_sigmoid,
+                         int depth_mode, const float* gt, int G, float* s1_score, int* s1_idx, float* scores,
+                         long long* inds, float* clses, float* ys, float* xs, float* pois, float* result, int* count,
+                         float* depth_err, float* proj, int* min_unc, void* stream) {
+  return decode_launch(heat, reg, calib, pad, size, dim_mean, B, C, H, W, R, K, thresh, apply_sigmoid, &depth_mode, 1, gt, G,
+                       s1_score, s1_idx, scores, inds, clses, ys, xs, pois, result, count, depth_err, proj, min_unc, stream);
+}
+
+int mf_decode_detections_depths(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,
+                                const float* dim_mean, int B, int C, int H, int W, int R, int K, float thresh,
+                                int apply_sigmoid, const int* depth_modes, int n_modes, const float* gt, int G,
+                                float* s1_score, int* s1_idx, float* scores, long long* inds, float* clses, float* ys,
+                                float* xs, float* pois, float* result, int* count, float* depth_err, float* proj,
+                                int* min_unc, void* stream) {
+  return decode_launch(heat, reg, calib, pad, size, dim_mean, B, C, H, W, R, K, thresh, apply_sigmoid, depth_modes, n_modes,
+                       gt, G, s1_score, s1_idx, scores, inds, clses, ys, xs, pois, result, count, depth_err, proj, min_unc,
+                       stream);
 }
 
 }  // extern "C"

@@ -235,6 +235,18 @@ def get_official_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict
     return result, ret_dict
 
 
+def write_kitti_detections(rows, path):
+    """generate_kitti_3d_detection (kitti_object_eval_python/evaluate.py:34-53), byte for byte: one line per row of the
+    decode's result [n, 14] (class, alpha, x1, y1, x2, y2, h, w, l, x, y, z, ry, score) - the class name, 0, 0, then the
+    row after np.round(4) in float32, each value printed as the Python float it widens to - and a lone newline for an
+    image without detections. The reference's check_last_line_break leaves the file as written: its `os.SEEK_END` raises
+    NameError (evaluate.py does not import os), which its bare `except` swallows."""
+    rows = np.asarray(rows, dtype=np.float32).reshape(-1, 14).round(4)
+    lines = ["%s 0 0 %s\n" % (ID_TYPE_CONVERSION[int(r[0])], " ".join(repr(v) for v in r[1:])) for r in rows.tolist()]
+    with open(path, 'w', newline='') as f:
+        f.write("".join(lines) if lines else "\n")
+
+
 def evaluate_python(label_path, result_path, label_split_file, current_class, metric):
     """data/datasets/evaluation/__init__.py:33: the detection files (sorted ids) are paired by position with the ground
     truth of the split file's ids, in the split file's order."""

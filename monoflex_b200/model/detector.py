@@ -11,7 +11,10 @@ solver.FusedAdamW (whose `.grad`s are views of one arena).
 Eval forwards are replayed from a CUDA graph (SURVEY §8f N3): shapes are static (384x1280 zero-padded images), so the
 ~135 kernel launches of a forward are captured once per (input shape, parameter version) and replayed with one
 cudaGraphLaunch; per call only the image batch and the per-image target fields are copied into static buffers.
-`MF_CUDA_GRAPH=0` (or `model.use_cuda_graph = False`) runs the same launches eagerly."""
+`MF_CUDA_GRAPH=0` (or `model.use_cuda_graph = False`) runs the same launches eagerly.
+
+`forward_depths(images, targets, methods)` decodes several OUTPUT_DEPTH estimators from one backbone + predictor pass
+(captured in a graph of its own, next to the forward's)."""
 import os
 
 import torch
@@ -47,6 +50,7 @@ class KeypointDetector(nn.Module):
         self.test = cfg.DATASETS.TEST_SPLIT == 'test'
         self.use_cuda_graph = os.environ.get("MF_CUDA_GRAPH", "1") != "0"
         self._graph = None
+        self._graph_depths = None
         self.set_precision(engine.default_precision())
         # fp16 gradient flow of the backward tape: dL/dcls, dL/dreg are multiplied by `loss_scale` before they enter the
         # tape and every parameter gradient is divided by it again before it is accumulated into p.grad (fp32)
@@ -64,7 +68,7 @@ class KeypointDetector(nn.Module):
         if mode not in engine.PRECISIONS:
             raise ValueError("precision must be one of %s" % (engine.PRECISIONS,))
         self.precision = self.backbone.precision = mode
-        self._graph = None
+        self._graph = self._graph_depths = None
         return self
 
     def forward(self, images, targets=None):
@@ -163,23 +167,44 @@ class KeypointDetector(nn.Module):
         g = self._enqueue_graph(x, targets)
         return PendingDetections(self.heads.post_processor, g['ws'], g['plan_h'].cls)
 
+    def forward_depths(self, images, targets, methods):
+        """Eval mode: {method: what forward(images, targets) returns with heads.post_processor.output_depth = method} for
+        every OUTPUT_DEPTH name of `methods`, from one backbone + predictor pass and one decode launch. Only the depth, the
+        location, alpha / ry and the score differ between the methods; the detections are the same."""
+        if self.training:
+            raise RuntimeError("forward_depths is an inference API: call model.eval() first")
+        post = self.heads.post_processor
+        methods = post.check_config(methods)
+        x = to_image_list(images).tensors
+        if not self.use_cuda_graph or not x.is_cuda:
+            pred = self.heads.predictor(self.backbone(x), targets)
+            return post.forward_depths(pred, targets, methods, test=self.test)
+        g = self._enqueue_graph(x, targets, methods)
+        return post.finish_depths(g['ws'], g['plan_h'].cls, g['plan_h'].reg, methods)
+
     # ------------------------------------------------------------------ CUDA-graph path
     def _forward_graph(self, x, targets):
         g = self._enqueue_graph(x, targets)
         return self.heads.post_processor.finish(g['ws'], g['plan_h'].cls, g['plan_h'].reg)
 
-    def _enqueue_graph(self, x, targets):
+    def _enqueue_graph(self, x, targets, methods=None):
+        """replay the forward's graph or, given a tuple of `methods`, the graph of forward_depths (each kept in its own
+        slot, so alternating the two does not capture again)"""
         pred, post = self.heads.predictor, self.heads.post_processor
-        post.check_config()
+        post.check_config(methods)
         x = x.float().contiguous()
         k_edge = targets[0].get_field("edge_indices").shape[0]
         # per-call target fields of the decode: calib / pad / size and, for the oracle depth, the ground-truth table
-        meta = post.prepare_targets(targets, self.test, x.device)
+        meta = post.prepare_targets(targets, self.test, x.device, methods)
         key = (tuple(x.shape), x.device, k_edge, engine.fingerprint(self), post.det_threshold, post.max_detection, self.precision,
-               post.output_depth, tuple(tuple(m.shape) for m in meta))
-        g = self._graph
+               post.output_depth if methods is None else methods, tuple(tuple(m.shape) for m in meta))
+        g = self._graph if methods is None else self._graph_depths
         if g is None or g['key'] != key:
-            g = self._capture(x, targets, key, meta)
+            g = self._capture(x, targets, key, meta, methods)
+            if methods is None:
+                self._graph = g
+            else:
+                self._graph_depths = g
         g['x'].copy_(x, non_blocking=True)
         pred.load_targets(g['plan_h'], targets)
         for dst, src in zip(g['meta'], meta):
@@ -188,7 +213,7 @@ class KeypointDetector(nn.Module):
         g['graph'].replay()
         return g
 
-    def _capture(self, x, targets, key, meta):
+    def _capture(self, x, targets, key, meta, methods=None):
         pred, post = self.heads.predictor, self.heads.post_processor
         xs = x.clone()
         plan_b = self.backbone._plan_for(xs)
@@ -199,14 +224,13 @@ class KeypointDetector(nn.Module):
         def body():
             self.backbone.run_plan(plan_b, xs)
             plan_h.run()
-            return post.launch(plan_h.cls, plan_h.reg, meta)
+            return post.launch(plan_h.cls, plan_h.reg, meta, methods)
         body()                                   # eager warm-up: func attributes, tensor-map driver entry points, workspaces
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             ws = body()
-        self._graph = {'key': key, 'graph': graph, 'x': xs, 'plan_b': plan_b, 'plan_h': plan_h, 'meta': meta, 'ws': ws}
-        return self._graph
+        return {'key': key, 'graph': graph, 'x': xs, 'plan_b': plan_b, 'plan_h': plan_h, 'meta': meta, 'ws': ws}
 
 
 class PendingDetections(object):

@@ -5,6 +5,9 @@ reference for batch size 1. Unlike the reference (valid for B == 1 only: detecto
 CUDA decode takes per-image calibration / padding / size, so for B > 1 `result` is the concatenation of the valid rows
 of every image and `eval_utils['batch_idxs']` / `['counts']` say which image each row belongs to (SURVEY H8).
 
+forward_depths(predictions, targets, methods) -> {method: what forward returns with output_depth = method}: one NMS /
+top-k / POI gather and one decode kernel for all the methods (engine/inference.py's inference_all_depths in one pass).
+
 Every OUTPUT_DEPTH estimator of the reference is decoded by the kernel: 'soft' (runs/monoflex.yaml), 'hard', 'mean',
 'direct', 'keypoints_avg', 'keypoints_center', 'keypoints_02', 'keypoints_13' and 'oracle'. `output_depth` is read at
 every forward, so engine/inference.py's inference_all_depths can switch it between passes. The oracle matches every
@@ -48,12 +51,14 @@ class PostProcessor(nn.Module):
                 or not self.uncertainty_as_conf or self.down_ratio != 4:
             raise NotImplementedError("decode kernel is built for the runs/monoflex.yaml decode settings")
         self._ws = None
+        self._ws_depths = None
         self._meta_cache = None
 
-    def prepare_targets(self, targets, test, device):
+    def prepare_targets(self, targets, test, device, methods=None):
         """calib / pad_size / size of every image as three small device tensors (detector_infer.py:53-58). The host-side
         scalars (calibration, image size) are cached BY VALUE; pad_size is stacked on the device like the reference
-        does, so a CUDA `pad_size` field costs no host sync."""
+        does, so a CUDA `pad_size` field costs no host sync. The oracle table is appended when `methods` (default: the
+        output_depth alone) include 'oracle'."""
         calib, size = [], []
         for t in targets:
             c = t.get_field("calib")
@@ -65,7 +70,7 @@ class PostProcessor(nn.Module):
                                 torch.tensor(size, dtype=torch.float32).to(device))
         pad = torch.stack([torch.as_tensor(t.get_field("pad_size")) for t in targets]).to(device=device, dtype=torch.float32,
                                                                                          non_blocking=True).view(-1, 2)
-        if self.output_depth != 'oracle':
+        if 'oracle' not in ((self.output_depth,) if methods is None else methods):
             return self._meta_cache[1], pad, self._meta_cache[2]
         return self._meta_cache[1], pad, self._meta_cache[2], self.oracle_table(targets, device)
 
@@ -85,19 +90,32 @@ class PostProcessor(nn.Module):
             rows.append(torch.cat([f[0].view(n, 1), f[1].view(n, 1), f[2].view(n, 4), f[3].view(n, 3)[:, 2:]], 1))
         return torch.stack(rows).contiguous()
 
-    def launch(self, heat, reg, meta):
-        """the two decode kernels (asynchronous; no host sync)"""
+    def launch(self, heat, reg, meta, methods=None):
+        """the two decode kernels (asynchronous; no host sync) for the output_depth or, given a tuple of `methods`, for all
+        of them into a workspace of one block per method"""
         calib, pad, size = meta[:3]
         B, K = heat.shape[0], self.max_detection
-        if self._ws is None or (self._ws.B, self._ws.C) != (B, heat.shape[1]) or self._ws.scores.device != heat.device:
-            self._ws = DecodeWorkspace(B, heat.shape[1], K, reg.shape[1], heat.device)
-        return decode_detections(heat, reg, calib, pad, size, self.dim_mean, K, self.det_threshold, False, self._ws,
-                                 depth_mode=self.output_depth, gt=meta[3] if len(meta) > 3 else None)
+        n_modes = None if methods is None else len(methods)
+        ws = self._ws if methods is None else self._ws_depths
+        if ws is None or (ws.B, ws.C, ws.n_modes) != (B, heat.shape[1], n_modes) or ws.scores.device != heat.device:
+            ws = DecodeWorkspace(B, heat.shape[1], K, reg.shape[1], heat.device, n_modes)
+            if methods is None:
+                self._ws = ws
+            else:
+                self._ws_depths = ws
+        return decode_detections(heat, reg, calib, pad, size, self.dim_mean, K, self.det_threshold, False, ws,
+                                 depth_mode=self.output_depth if methods is None else methods,
+                                 gt=meta[3] if len(meta) > 3 else None)
 
     def finish(self, ws, heat, reg):
         """host side: read the valid counts (the reference syncs at `valid_mask.sum() == 0`, :106) and slice."""
+        return self.finish_depths(ws, heat, reg, (self.output_depth,))[self.output_depth]
+
+    def finish_depths(self, ws, heat, reg, methods):
+        """finish() of every method of `methods`, the estimators of the workspace's result blocks in order (a
+        single-mode workspace holds one block without the mode dimension). The counts are read once; the tensors that do
+        not depend on the estimator are shared between the methods' dicts."""
         B = heat.shape[0]
-        visualize_preds = {'heat_map': heat}
         counts = ws.count.tolist()
 
         def rows(t):
@@ -109,26 +127,39 @@ class PostProcessor(nn.Module):
             return torch.cat([t[b, :n] for b, n in enumerate(counts)], 0)
         batch_idxs = torch.cat([torch.full((n,), b, dtype=torch.long, device=heat.device) for b, n in enumerate(counts)], 0)
         # detections are tiny: hand out copies, not views of the (re-used) decode workspace
-        result, vis_scores, pois = rows(ws.result).clone(), rows(ws.scores).clone(), rows(ws.pois).clone()
-        depth_err = rows(ws.depth_err).clone()
-        visualize_preds['keypoints'] = pois[:, self.key2channel('corner_offset')].reshape(-1, 10, 2)
-        visualize_preds['proj_center'] = rows(ws.proj).clone()                                          # :125
-        visualize_preds['depth_uncertainty'] = reg[:, self.key2channel('depth_uncertainty')].squeeze(1)  # :136
-        if self.output_depth in ENSEMBLE_DEPTH_MODES:
-            visualize_preds['min_uncertainty'] = rows(ws.min_unc).long()                                # :185
-        conf = result[:, 13] / vis_scores.clamp_min(1e-12) if result.shape[0] else result.new_zeros(0)
-        eval_utils = {'dis_ious': None, 'depth_errors': None, 'uncertainty_conf': conf,
-                      'estimated_depth_error': depth_err, 'vis_scores': vis_scores, 'batch_idxs': batch_idxs,
-                      'counts': counts, 'topk': (ws.scores, ws.inds, ws.clses, ws.ys, ws.xs), 'padded_result': ws.result}
-        return result, eval_utils, visualize_preds
+        vis_scores, pois = rows(ws.scores).clone(), rows(ws.pois).clone()
+        keypoints = pois[:, self.key2channel('corner_offset')].reshape(-1, 10, 2)
+        proj_center = rows(ws.proj).clone()                                                             # :125
+        depth_uncertainty = reg[:, self.key2channel('depth_uncertainty')].squeeze(1)                    # :136
+        out = {}
+        for m, method in enumerate(methods):
+            block = (lambda t: t) if ws.n_modes is None else (lambda t: t[m])
+            result, depth_err = rows(block(ws.result)).clone(), rows(block(ws.depth_err)).clone()
+            visualize_preds = {'heat_map': heat, 'keypoints': keypoints, 'proj_center': proj_center,
+                               'depth_uncertainty': depth_uncertainty}
+            if method in ENSEMBLE_DEPTH_MODES:
+                visualize_preds['min_uncertainty'] = rows(block(ws.min_unc)).long()                     # :185
+            conf = result[:, 13] / vis_scores.clamp_min(1e-12) if result.shape[0] else result.new_zeros(0)
+            eval_utils = {'dis_ious': None, 'depth_errors': None, 'uncertainty_conf': conf,
+                          'estimated_depth_error': depth_err, 'vis_scores': vis_scores, 'batch_idxs': batch_idxs,
+                          'counts': counts, 'topk': (ws.scores, ws.inds, ws.clses, ws.ys, ws.xs),
+                          'padded_result': block(ws.result)}
+            out[method] = (result, eval_utils, visualize_preds)
+        return out
 
-    def check_config(self):
-        if self.output_depth not in DEPTH_MODES:
-            if isinstance(self.output_depth, str) and self.output_depth.find('keypoints') >= 0:     # :172-173
-                raise ValueError("unknown key-point depth OUTPUT_DEPTH=%r" % (self.output_depth,))
-            raise ValueError("OUTPUT_DEPTH=%r is not one of %s" % (self.output_depth, ", ".join(DEPTH_MODES)))
+    def check_config(self, methods=None):
+        """the output_depth, or every method of `methods` (a non-empty sequence of distinct names) -> the tuple of them"""
+        names = (self.output_depth,) if methods is None else methods
+        if isinstance(names, str) or not isinstance(names, (tuple, list)) or not names or len(set(names)) != len(names):
+            raise ValueError("methods must be a non-empty list of distinct OUTPUT_DEPTH names, got %r" % (methods,))
+        for name in names:
+            if name not in DEPTH_MODES:
+                if isinstance(name, str) and name.find('keypoints') >= 0:                            # :172-173
+                    raise ValueError("unknown key-point depth OUTPUT_DEPTH=%r" % (name,))
+                raise ValueError("OUTPUT_DEPTH=%r is not one of %s" % (name, ", ".join(DEPTH_MODES)))
         if self.eval_dis_iou or self.eval_depth:
             raise NotImplementedError("--eval_iou / --eval_depth diagnostics are out of scope")
+        return tuple(names)
 
     def forward(self, predictions, targets, features=None, test=False, refine_module=None):
         self.check_config()
@@ -138,3 +169,14 @@ class PostProcessor(nn.Module):
         heat, reg = heat.float().contiguous(), reg.float().contiguous()
         ws = self.launch(heat, reg, self.prepare_targets(targets, test, heat.device))
         return self.finish(ws, heat, reg)
+
+    def forward_depths(self, predictions, targets, methods, test=False):
+        """{method: forward(predictions, targets) with output_depth = method} for every method of `methods`, from one
+        decode launch; the oracle table is built once, and only when 'oracle' is among the methods."""
+        methods = self.check_config(methods)
+        heat, reg = predictions['cls'], predictions['reg']
+        if not heat.is_cuda:
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
+        heat, reg = heat.float().contiguous(), reg.float().contiguous()
+        ws = self.launch(heat, reg, self.prepare_targets(targets, test, heat.device, methods), methods)
+        return self.finish_depths(ws, heat, reg, methods)

@@ -1,6 +1,8 @@
 """Heat-map helpers with the reference's names (model/layers/utils.py:22-145), backed by the fused CUDA decode kernel.
 `select_topk` uses floor division for ys / class ids (torch-1.4 semantics the reference relies on, SURVEY H5) and the
 tie rule (score desc, index asc)."""
+import ctypes
+
 import torch
 
 from ..._lib import call, stream
@@ -24,11 +26,14 @@ def sigmoid_hm(hm_features):
 
 
 class DecodeWorkspace(object):
-    """Caller-owned output / scratch buffers of mf_decode_detections for a fixed (B, C, K, R)."""
+    """Caller-owned output / scratch buffers of mf_decode_detections for a fixed (B, C, K, R). With `n_modes` (the
+    number of estimators of one mf_decode_detections_depths call) the per-mode outputs result, depth_err and min_unc
+    take a leading mode dimension: [n_modes, B, K, ...]."""
 
-    def __init__(self, B, C, K, R, device):
+    def __init__(self, B, C, K, R, device, n_modes=None):
         f = dict(dtype=torch.float32, device=device)
-        self.B, self.C, self.K, self.R = B, C, K, R
+        self.B, self.C, self.K, self.R, self.n_modes = B, C, K, R, n_modes
+        lead = () if n_modes is None else (n_modes,)
         slabs = 8     # MF_DECODE_SLABS: stage 1 splits every (image, class) plane into 8 pixel ranges
         self.ws_score = torch.empty(B * C * K * slabs, **f)
         self.ws_idx = torch.empty(B * C * K * slabs, dtype=torch.int32, device=device)
@@ -36,11 +41,11 @@ class DecodeWorkspace(object):
         self.ys, self.xs = torch.empty(B, K, **f), torch.empty(B, K, **f)
         self.inds = torch.empty(B, K, dtype=torch.long, device=device)
         self.pois = torch.empty(B, K, R, **f)
-        self.result = torch.empty(B, K, 14, **f)
+        self.result = torch.empty(*lead, B, K, 14, **f)
         self.count = torch.empty(B, dtype=torch.int32, device=device)
-        self.depth_err = torch.empty(B, K, **f)
+        self.depth_err = torch.empty(*lead, B, K, **f)
         self.proj = torch.empty(B, K, 2, **f)
-        self.min_unc = torch.empty(B, K, dtype=torch.int32, device=device)
+        self.min_unc = torch.empty(*lead, B, K, dtype=torch.int32, device=device)
 
 
 # OUTPUT_DEPTH estimators of the decode kernel (detector_infer.py:148-209), in the order of the C ABI's `depth_mode`
@@ -53,23 +58,35 @@ def decode_detections(heat, reg, calib, pad, size, dim_mean, K, thresh, apply_si
                       gt=None):
     """nms_hm + select_topk + select_point_of_interest + 3D decode in two kernels. All arguments are CUDA tensors.
     `depth_mode` is one of DEPTH_MODES; 'oracle' needs `gt` [B, G, 7] fp32 = (valid, class, x1, y1, x2, y2, z) per
-    ground-truth slot of every image."""
+    ground-truth slot of every image. A tuple of distinct DEPTH_MODES decodes all of them from one NMS / top-k / POI
+    gather: the workspace's result, depth_err and min_unc then hold one [B, K, ...] block per mode, in the tuple's order,
+    each equal to the single-mode decode of that mode."""
     B, C, H, W = heat.shape
     R = reg.shape[1]
-    if depth_mode not in DEPTH_MODES:
-        raise ValueError("depth_mode %r is not one of %s" % (depth_mode, DEPTH_MODES))
-    if depth_mode == 'oracle':
+    several = isinstance(depth_mode, (tuple, list))
+    modes = tuple(depth_mode) if several else (depth_mode,)
+    for m in modes:
+        if m not in DEPTH_MODES:
+            raise ValueError("depth_mode %r is not one of %s" % (m, DEPTH_MODES))
+    if not modes or len(set(modes)) != len(modes):
+        raise ValueError("depth_mode %r: give one or more distinct modes" % (depth_mode,))
+    if 'oracle' in modes:
         if gt is None or gt.dim() != 3 or tuple(gt.shape[::2]) != (B, 7) or gt.dtype != torch.float32 \
                 or not gt.is_contiguous():
             raise ValueError("the oracle depth needs gt as a contiguous float32 [B, G, 7] tensor")
-    if ws is None or (ws.B, ws.C, ws.K, ws.R) != (B, C, K, R):
-        ws = DecodeWorkspace(B, C, K, R, heat.device)
+    n_modes = len(modes) if several else None
+    if ws is None or (ws.B, ws.C, ws.K, ws.R, getattr(ws, 'n_modes', None)) != (B, C, K, R, n_modes):
+        ws = DecodeWorkspace(B, C, K, R, heat.device, n_modes)
     gt_ptr, G = (gt.data_ptr(), gt.shape[1]) if gt is not None else (None, 0)
-    call("mf_decode_detections", heat.data_ptr(), reg.data_ptr(), calib.data_ptr(), pad.data_ptr(), size.data_ptr(),
-         dim_mean.data_ptr(), B, C, H, W, R, K, float(thresh), 1 if apply_sigmoid else 0, DEPTH_MODES.index(depth_mode),
-         gt_ptr, G, ws.ws_score.data_ptr(), ws.ws_idx.data_ptr(), ws.scores.data_ptr(), ws.inds.data_ptr(),
-         ws.clses.data_ptr(), ws.ys.data_ptr(), ws.xs.data_ptr(), ws.pois.data_ptr(), ws.result.data_ptr(),
-         ws.count.data_ptr(), ws.depth_err.data_ptr(), ws.proj.data_ptr(), ws.min_unc.data_ptr(), stream())
+    if n_modes is None:
+        name, mode_args = "mf_decode_detections", (DEPTH_MODES.index(depth_mode),)
+    else:
+        name, mode_args = "mf_decode_detections_depths", ((ctypes.c_int * n_modes)(*map(DEPTH_MODES.index, modes)), n_modes)
+    call(name, heat.data_ptr(), reg.data_ptr(), calib.data_ptr(), pad.data_ptr(), size.data_ptr(), dim_mean.data_ptr(),
+         B, C, H, W, R, K, float(thresh), 1 if apply_sigmoid else 0, *mode_args, gt_ptr, G, ws.ws_score.data_ptr(),
+         ws.ws_idx.data_ptr(), ws.scores.data_ptr(), ws.inds.data_ptr(), ws.clses.data_ptr(), ws.ys.data_ptr(),
+         ws.xs.data_ptr(), ws.pois.data_ptr(), ws.result.data_ptr(), ws.count.data_ptr(), ws.depth_err.data_ptr(),
+         ws.proj.data_ptr(), ws.min_unc.data_ptr(), stream())
     return ws
 
 
