@@ -458,7 +458,12 @@ int mf_decode_detections_depths(const float* heat, const float* reg, const float
  *   AP [2 (R40, R11)][4 (bbox, bev, 3d, aos)][ncls][3][2], then compute_aos (first detection's alpha != -10), then the
  *   detection count of the largest image over MF_KITTI_MAX_DT (0: none; otherwise the tables are not valid).
  * mf_kitti_pack_results: the decode's rows [n, 14] fp32 (class, alpha, x1, y1, x2, y2, h, w, l, x, y, z, ry, score) as
- *   generate_kitti_3d_detection writes and get_label_anno parses them: np.round(x, 4) in float32, widened. */
+ *   generate_kitti_3d_detection writes and get_label_anno parses them: np.round(x, 4) in float32, widened.
+ * mf_kitti_eval_sets_*: the same stages for any number of overlap sets, e.g. get_coco_eval_result's ten
+ *   (eval.py:626-643, 729-788). min_overlaps: HOST float64 [n_sets][3 metric][ncls], compared as given (`overlap >
+ *   min_overlap`); the configuration count is 9 * n_sets * ncls, every overlap-set axis above has length n_sets, and
+ *   mf_kitti_eval_sets_workspace_size writes the workspace bytes to *bytes (HOST). The official entry points above are
+ *   these with get_official_eval_result's table gathered for the class list and n_sets = 2. */
 #define MF_KITTI_OBJ 16
 #define MF_KITTI_DONTCARE 6
 #define MF_KITTI_MAX_DT 128
@@ -471,6 +476,13 @@ int mf_kitti_eval_statistics(const double* gt, const int* gt_off, const double* 
                              long long n_pair, const int* classes, int ncls, void* workspace, size_t ws_bytes,
                              void* stream);
 int mf_kitti_eval_ap(const void* workspace, int n_gt, int n_dt, int ncls, double* out, void* stream);
+int mf_kitti_eval_sets_workspace_size(int n_gt, int n_dt, int ncls, int n_sets, size_t* bytes);
+int mf_kitti_eval_sets_statistics(const double* gt, const int* gt_off, const double* dt, const int* dt_off,
+                                  const long long* pair_off, int n_img, int n_gt, int n_dt, int max_dt,
+                                  const double* overlaps, long long n_pair, const int* classes, int ncls,
+                                  const double* min_overlaps, int n_sets, void* workspace, size_t ws_bytes,
+                                  void* stream);
+int mf_kitti_eval_sets_ap(const void* workspace, int n_gt, int n_dt, int ncls, int n_sets, double* out, void* stream);
 
 /* ---- boundary B: the reference's native operator ABI (_ext, src/vision.cpp:4-9, src/dcn_v2.h:9-59) ------------ */
 /* at::Tensor dcn_v2_forward(input, weight, bias, offset, mask, kh,kw,sh,sw,ph,pw,dh,dw,deformable_group): fp32 NCHW,

@@ -1,17 +1,19 @@
 // KITTI official 3D-detection metric (data/datasets/evaluation/kitti_object_eval_python/eval.py, rotate_iou.py):
 // 2D / BEV / 3D precision-recall tables, AOS and AP|R40 / AP|R11 for every (metric, class, difficulty, overlap set) at once.
+// The overlap sets are data: get_official_eval_result's two, or get_coco_eval_result's ten (eval.py:626-643, 729-788).
 //
 // Objects are CSR-packed per image as float64 rows of MF_KITTI_OBJ values (see include/monoflex_b200.h). Stages:
 //   overlaps    one CTA per image: the detection x ground-truth blocks of metric 0 (2D), 1 (BEV) and 2 (3D);
 //   statistics  flags (clean_data), the compute_fp=False pass, a segmented sort of the true-positive scores, get_thresholds
 //               (sequential per configuration), the compute_fp=True pass per (configuration, threshold) over all images;
-//   ap          recall / precision / AOS, their suffix maxima and both AP sums.
+//   ap          recall / precision / AOS, their suffix maxima and both AP sums, one thread per configuration.
 // The launch count depends on neither the number of images nor of configurations. Greedy matching is sequential inside one
 // (image, threshold) as in the reference, and parallel across them; the AOS similarity is summed over images in image
 // order like the reference's pr[t, 3], the integer counts in any order. No floating-point atomics.
 #include "mf_common.cuh"
 #include "../../include/monoflex_b200.h"
 #include <cub/device/device_segmented_radix_sort.cuh>
+#include <climits>
 #include <math.h>
 
 namespace mf {
@@ -23,6 +25,7 @@ constexpr int MAX_DT = MF_KITTI_MAX_DT;    // detections per image: the assigned
 constexpr int MAX_CLS = 8;
 constexpr int STAT_THREADS = 128;
 constexpr int THR_THREADS = 256;
+constexpr int AP_THREADS = 64;
 constexpr double NO_DETECTION = -10000000.0;
 
 // object columns
@@ -30,8 +33,10 @@ enum { C_CLS = 0, C_TRUNC, C_OCC, C_ALPHA, C_X1, C_Y1, C_X2, C_Y2, C_L, C_H, C_W
 
 struct Classes { int c[MAX_CLS]; };
 
-// get_official_eval_result's min_overlaps[k][metric][class] (overlap_0_7, overlap_0_5)
-__constant__ double c_min_overlap[2][3][6] = {
+// get_official_eval_result's min_overlaps[k][metric][class code] (overlap_0_7, overlap_0_5); the official entry points
+// gather it into the [n_sets][metric][ncls] table every configuration reads
+constexpr int OFFICIAL_SETS = 2;
+const double k_official_min_overlap[OFFICIAL_SETS][3][6] = {
     {{0.7, 0.5, 0.5, 0.7, 0.5, 0.7}, {0.7, 0.5, 0.5, 0.7, 0.5, 0.7}, {0.7, 0.5, 0.5, 0.7, 0.5, 0.7}},
     {{0.7, 0.5, 0.5, 0.7, 0.5, 0.5}, {0.5, 0.25, 0.25, 0.5, 0.25, 0.5}, {0.5, 0.25, 0.25, 0.5, 0.25, 0.5}}};
 __constant__ double c_min_height[3] = {40, 25, 25};
@@ -200,8 +205,9 @@ __global__ void overlaps_kernel(const double* __restrict__ gt, const int* __rest
 // ------------------------------------------------------------------------------------------------------------ statistics
 struct StatArgs {
   const double* gt; const int* gt_off; const double* dt; const int* dt_off; const long long* pair_off; const double* ov;
-  int n_img, n_gt, n_dt, ncls; long long n_pair;
+  int n_img, n_gt, n_dt, ncls, n_sets; long long n_pair;
   Classes cls;
+  const double* min_overlap;          // [n_sets][3 metric][ncls], the caller's doubles
   signed char* fg; signed char* fd;   // clean_data flags [ncls * 3][n_gt] / [ncls * 3][n_dt]
   int* seg;                           // [C + 1] segment offsets of the score sort
   double* tps; double* tps_sorted;    // [C][n_gt] true-positive scores of the first pass, -inf padded
@@ -210,18 +216,19 @@ struct StatArgs {
   int* aos;                           // [2]: compute_aos of get_official_eval_result, largest over-limit image (0: none)
 };
 
-// configuration c = ((metric * ncls + m) * 3 + difficulty) * 2 + k
+// configuration c = ((metric * ncls + m) * 3 + difficulty) * n_sets + k, C = 9 * n_sets * ncls of them
+MF_DEVINL int n_configs(int ncls, int n_sets) { return 9 * n_sets * ncls; }
 struct Cfg { int metric, m, l, k; double min_overlap; };
 MF_DEVINL Cfg config(const StatArgs& a, int c) {
   Cfg f;
-  f.k = c % 2; f.l = (c / 2) % 3; f.m = (c / 6) % a.ncls; f.metric = c / (6 * a.ncls);
-  f.min_overlap = c_min_overlap[f.k][f.metric][a.cls.c[f.m]];
+  f.k = c % a.n_sets; f.l = (c / a.n_sets) % 3; f.m = (c / (3 * a.n_sets)) % a.ncls; f.metric = c / (3 * a.n_sets * a.ncls);
+  f.min_overlap = a.min_overlap[(f.k * 3 + f.metric) * a.ncls + f.m];
   return f;
 }
 
 __global__ void flags_kernel(StatArgs a) {
   const int x = blockIdx.x * blockDim.x + threadIdx.x;
-  const int C = 18 * a.ncls;
+  const int C = n_configs(a.ncls, a.n_sets);
   if (x <= C) a.seg[x] = x * a.n_gt;
   if (x == 0) { a.aos[0] = a.n_dt > 0 && a.dt[C_ALPHA] != -10.0; a.aos[1] = 0; }
   if (x < a.n_gt) {
@@ -254,7 +261,7 @@ MF_DEVINL void set_bit(unsigned* s, int j) { s[j >> 5] |= 1u << (j & 31); }
 // compute_statistics_jit(compute_fp=False, thresh=0) per (configuration, image): the scores of the true positives, in order
 __global__ void first_pass_kernel(StatArgs a) {
   const long long x = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (x >= static_cast<long long>(18 * a.ncls) * a.n_img) return;
+  if (x >= static_cast<long long>(n_configs(a.ncls, a.n_sets)) * a.n_img) return;
   const int c = static_cast<int>(x / a.n_img), img = static_cast<int>(x % a.n_img);
   const Cfg f = config(a, c);
   const int g0 = a.gt_off[img], ng = a.gt_off[img + 1] - g0, d0 = a.dt_off[img], nd = a.dt_off[img + 1] - d0;
@@ -403,11 +410,13 @@ __global__ void __launch_bounds__(STAT_THREADS) second_pass_kernel(StatArgs a) {
 // eval_class's tail and get_mAP_R40 / get_mAP; NaN from 0/0 propagates through the suffix maximum like np.max
 MF_DEVINL double nanmax(double a, double b) { return (isnan(a) || isnan(b)) ? NAN : (b > a ? b : a); }
 
-__global__ void ap_kernel(const double* __restrict__ pr, const int* __restrict__ nthr, const int* __restrict__ aos_flag,
-                          int ncls, double* __restrict__ out) {
-  const int C = 18 * ncls, c = threadIdx.x;
+__global__ void __launch_bounds__(AP_THREADS) ap_kernel(const double* __restrict__ pr, const int* __restrict__ nthr,
+                                                        const int* __restrict__ aos_flag, int ncls, int n_sets,
+                                                        double* __restrict__ out) {
+  const int C = n_configs(ncls, n_sets), c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const int metric = c / (6 * ncls), rest = c % (6 * ncls);   // rest = (m * 3 + l) * 2 + k
+  const int per = 3 * n_sets * ncls;
+  const int metric = c / per, rest = c % per;                  // rest = (m * 3 + l) * n_sets + k
   const bool aos = metric == 0 && aos_flag[0];
   double rec[NPTS], prec[NPTS], ori[NPTS];
   for (int i = 0; i < NPTS; ++i) {
@@ -430,9 +439,8 @@ __global__ void ap_kernel(const double* __restrict__ pr, const int* __restrict__
     out[tab + c * NPTS + i] = prec[i];
     out[2 * tab + c * NPTS + i] = ori[i];
   }
-  // ap[R40, R11][bbox, bev, 3d, aos][ncls][3][2]
+  // ap[R40, R11][bbox, bev, 3d, aos][ncls][3][n_sets]
   double* ap = out + 3 * tab;
-  const int per = 6 * ncls;
   double s40 = 0.0, s11 = 0.0, o40 = 0.0, o11 = 0.0;
   for (int i = 1; i < NPTS; ++i) { s40 = s40 + prec[i]; o40 = o40 + ori[i]; }
   for (int i = 0; i < NPTS; i += 4) { s11 = s11 + prec[i]; o11 = o11 + ori[i]; }
@@ -459,11 +467,11 @@ __global__ void pack_results_kernel(const float* __restrict__ rows, int n, doubl
 
 // workspace carve-up shared by the size query and the stages
 struct Layout {
-  size_t fg, fd, seg, tps, tps_sorted, thr, nthr, pr, aos, cub, cub_bytes, total;
+  size_t fg, fd, seg, tps, tps_sorted, thr, nthr, pr, aos, min_overlap, cub, cub_bytes, total;
 };
 size_t align256(size_t x) { return (x + 255) & ~static_cast<size_t>(255); }
-Layout layout(int n_gt, int n_dt, int ncls) {
-  const size_t C = 18 * static_cast<size_t>(ncls);
+Layout layout(int n_gt, int n_dt, int ncls, int n_sets) {
+  const size_t C = 9 * static_cast<size_t>(n_sets) * ncls;
   Layout L;
   size_t o = 0;
   L.fg = o; o = align256(o + ncls * 3 * static_cast<size_t>(n_gt));
@@ -475,6 +483,7 @@ Layout layout(int n_gt, int n_dt, int ncls) {
   L.nthr = o; o = align256(o + C * sizeof(int));
   L.pr = o; o = align256(o + C * NPTS * 4 * sizeof(double));
   L.aos = o; o = align256(o + 2 * sizeof(int));
+  L.min_overlap = o; o = align256(o + n_sets * 3 * static_cast<size_t>(ncls) * sizeof(double));
   L.cub_bytes = 0;
   cub::DeviceSegmentedRadixSort::SortKeysDescending(nullptr, L.cub_bytes, static_cast<const double*>(nullptr),
                                                     static_cast<double*>(nullptr), static_cast<int>(C * n_gt),
@@ -485,6 +494,102 @@ Layout layout(int n_gt, int n_dt, int ncls) {
   return L;
 }
 
+// the stages index the sorted scores [C][n_gt], the segment offsets and the second pass's C * 41 blocks with int
+bool sets_fit(int n_gt, int ncls, int n_sets) {
+  if (n_sets < 1 || ncls < 1 || ncls > MAX_CLS || n_gt < 0) return false;
+  const long long C = 9LL * n_sets * ncls;
+  return C * NPTS <= INT_MAX && C * (n_gt + 1LL) <= INT_MAX;
+}
+
+// get_official_eval_result's table for the class list: [2][3][ncls]; a class code outside 0..5 gets 0 and is refused by
+// run_statistics
+void official_table(const int* classes, int ncls, double* table) {
+  if (ncls < 1 || ncls > MAX_CLS) return;                 // refused by run_statistics
+  for (int k = 0; k < OFFICIAL_SETS; ++k)
+    for (int metric = 0; metric < 3; ++metric)
+      for (int m = 0; m < ncls; ++m) {
+        const int code = classes[m];
+        table[(k * 3 + metric) * ncls + m] = code >= 0 && code <= 5 ? k_official_min_overlap[k][metric][code] : 0.0;
+      }
+}
+
+int run_statistics(const char* who, const double* gt, const int* gt_off, const double* dt, const int* dt_off,
+                   const long long* pair_off, int n_img, int n_gt, int n_dt, int max_dt, const double* overlaps,
+                   long long n_pair, const int* classes, int ncls, const double* min_overlaps, int n_sets,
+                   void* workspace, size_t ws_bytes, void* stream) {
+  if (n_img < 1 || n_gt < 0 || n_dt < 0) { set_error("%s: %d images", who, n_img); return -1; }
+  if (ncls < 1 || ncls > MAX_CLS) { set_error("%s: %d classes (1..%d)", who, ncls, MAX_CLS); return -1; }
+  if (max_dt > MAX_DT) {
+    set_error("%s: an image has %d detections, more than the %d per image this kernel matches", who, max_dt, MAX_DT);
+    return -1;
+  }
+  if (min_overlaps == nullptr || !sets_fit(n_gt, ncls, n_sets)) {
+    set_error("%s: %d overlap sets of %d classes over %d ground-truth objects (at least one set, and 9 * sets * classes "
+              "* (objects + 1) below 2^31)", who, n_sets, ncls, n_gt);
+    return -1;
+  }
+  const Layout L = layout(n_gt, n_dt, ncls, n_sets);
+  if (workspace == nullptr || ws_bytes < L.total) {
+    set_error("%s: workspace of %zu bytes, %zu needed", who, ws_bytes, L.total);
+    return -1;
+  }
+  cudaStream_t st = MF_STREAM(stream);
+  char* ws = static_cast<char*>(workspace);
+  StatArgs a;
+  a.gt = gt; a.gt_off = gt_off; a.dt = dt; a.dt_off = dt_off; a.pair_off = pair_off; a.ov = overlaps;
+  a.n_img = n_img; a.n_gt = n_gt; a.n_dt = n_dt; a.ncls = ncls; a.n_sets = n_sets; a.n_pair = n_pair;
+  for (int m = 0; m < MAX_CLS; ++m) {
+    a.cls.c[m] = m < ncls ? classes[m] : -1;
+    if (m < ncls && (classes[m] < 0 || classes[m] > 5)) {
+      set_error("%s: class %d is not one of 0..5", who, classes[m]);
+      return -1;
+    }
+  }
+  a.fg = reinterpret_cast<signed char*>(ws + L.fg); a.fd = reinterpret_cast<signed char*>(ws + L.fd);
+  a.seg = reinterpret_cast<int*>(ws + L.seg);
+  a.tps = reinterpret_cast<double*>(ws + L.tps); a.tps_sorted = reinterpret_cast<double*>(ws + L.tps_sorted);
+  a.thr = reinterpret_cast<double*>(ws + L.thr); a.nthr = reinterpret_cast<int*>(ws + L.nthr);
+  a.pr = reinterpret_cast<double*>(ws + L.pr); a.aos = reinterpret_cast<int*>(ws + L.aos);
+  a.min_overlap = reinterpret_cast<const double*>(ws + L.min_overlap);
+  // the host table as given, bit for bit: staged before the call returns, so it may live on the caller's stack
+  if (check_cuda(cudaMemcpyAsync(ws + L.min_overlap, min_overlaps, n_sets * 3 * static_cast<size_t>(ncls) * sizeof(double),
+                                 cudaMemcpyHostToDevice, st),
+                 "kitti_eval_min_overlaps"))
+    return -1;
+  const int C = 9 * n_sets * ncls;
+  const long long nflag = static_cast<long long>(n_gt) + n_dt + C + 1;
+  flags_kernel<<<static_cast<unsigned>((nflag + 255) / 256), 256, 0, st>>>(a);
+  if (check_cuda(cudaGetLastError(), "kitti_eval_flags")) return -1;
+  const long long npass = static_cast<long long>(C) * n_img;
+  first_pass_kernel<<<static_cast<unsigned>((npass + 127) / 128), 128, 0, st>>>(a);
+  if (check_cuda(cudaGetLastError(), "kitti_eval_first_pass")) return -1;
+  if (n_gt > 0) {
+    size_t bytes = L.cub_bytes;
+    if (check_cuda(cub::DeviceSegmentedRadixSort::SortKeysDescending(ws + L.cub, bytes, a.tps, a.tps_sorted, C * n_gt, C,
+                                                                      a.seg, a.seg + 1, 0, 64, st),
+                   "kitti_eval_sort"))
+      return -1;
+  }
+  thresholds_kernel<<<C, THR_THREADS, 0, st>>>(a);
+  if (check_cuda(cudaGetLastError(), "kitti_eval_thresholds")) return -1;
+  second_pass_kernel<<<C * NPTS, STAT_THREADS, 0, st>>>(a);
+  return check_cuda(cudaGetLastError(), "kitti_eval_second_pass");
+}
+
+int run_ap(const char* who, const void* workspace, int n_gt, int n_dt, int ncls, int n_sets, double* out, void* stream) {
+  if (workspace == nullptr || !sets_fit(n_gt, ncls, n_sets)) {
+    set_error("%s: %d classes, %d overlap sets", who, ncls, n_sets);
+    return -1;
+  }
+  const Layout L = layout(n_gt, n_dt, ncls, n_sets);
+  const char* ws = static_cast<const char*>(workspace);
+  const int C = 9 * n_sets * ncls;
+  ap_kernel<<<(C + AP_THREADS - 1) / AP_THREADS, AP_THREADS, 0, MF_STREAM(stream)>>>(
+      reinterpret_cast<const double*>(ws + L.pr), reinterpret_cast<const int*>(ws + L.nthr),
+      reinterpret_cast<const int*>(ws + L.aos), ncls, n_sets, out);
+  return check_cuda(cudaGetLastError(), "kitti_eval_ap");
+}
+
 }  // namespace
 }  // namespace mf
 
@@ -493,8 +598,19 @@ using namespace mf;
 extern "C" {
 
 size_t mf_kitti_eval_workspace(int n_gt, int n_dt, int ncls) {
-  if (n_gt < 0 || n_dt < 0 || ncls < 1 || ncls > MAX_CLS) return 0;
-  return layout(n_gt, n_dt, ncls).total;
+  if (n_gt < 0 || n_dt < 0 || !sets_fit(n_gt, ncls, OFFICIAL_SETS)) return 0;
+  return layout(n_gt, n_dt, ncls, OFFICIAL_SETS).total;
+}
+
+int mf_kitti_eval_sets_workspace_size(int n_gt, int n_dt, int ncls, int n_sets, size_t* bytes) {
+  if (bytes == nullptr || n_dt < 0 || !sets_fit(n_gt, ncls, n_sets)) {
+    set_error("mf_kitti_eval_sets_workspace_size: %d classes (1..%d), %d overlap sets, %d ground-truth objects, %d "
+              "detections (at least one set, and 9 * sets * classes * (objects + 1) below 2^31)",
+              ncls, MAX_CLS, n_sets, n_gt, n_dt);
+    return -1;
+  }
+  *bytes = layout(n_gt, n_dt, ncls, n_sets).total;
+  return 0;
 }
 
 int mf_kitti_pack_results(const float* rows, int n, double* out, void* stream) {
@@ -515,63 +631,27 @@ int mf_kitti_eval_statistics(const double* gt, const int* gt_off, const double* 
                              const long long* pair_off, int n_img, int n_gt, int n_dt, int max_dt, const double* overlaps,
                              long long n_pair, const int* classes, int ncls, void* workspace, size_t ws_bytes,
                              void* stream) {
-  if (n_img < 1 || n_gt < 0 || n_dt < 0) { set_error("mf_kitti_eval_statistics: %d images", n_img); return -1; }
-  if (ncls < 1 || ncls > MAX_CLS) { set_error("mf_kitti_eval_statistics: %d classes (1..%d)", ncls, MAX_CLS); return -1; }
-  if (max_dt > MAX_DT) {
-    set_error("mf_kitti_eval_statistics: an image has %d detections, more than the %d per image this kernel matches",
-              max_dt, MAX_DT);
-    return -1;
-  }
-  const Layout L = layout(n_gt, n_dt, ncls);
-  if (workspace == nullptr || ws_bytes < L.total) {
-    set_error("mf_kitti_eval_statistics: workspace of %zu bytes, %zu needed", ws_bytes, L.total);
-    return -1;
-  }
-  cudaStream_t st = MF_STREAM(stream);
-  char* ws = static_cast<char*>(workspace);
-  StatArgs a;
-  a.gt = gt; a.gt_off = gt_off; a.dt = dt; a.dt_off = dt_off; a.pair_off = pair_off; a.ov = overlaps;
-  a.n_img = n_img; a.n_gt = n_gt; a.n_dt = n_dt; a.ncls = ncls; a.n_pair = n_pair;
-  for (int m = 0; m < MAX_CLS; ++m) {
-    a.cls.c[m] = m < ncls ? classes[m] : -1;
-    if (m < ncls && (classes[m] < 0 || classes[m] > 5)) {
-      set_error("mf_kitti_eval_statistics: class %d is not one of 0..5", classes[m]);
-      return -1;
-    }
-  }
-  a.fg = reinterpret_cast<signed char*>(ws + L.fg); a.fd = reinterpret_cast<signed char*>(ws + L.fd);
-  a.seg = reinterpret_cast<int*>(ws + L.seg);
-  a.tps = reinterpret_cast<double*>(ws + L.tps); a.tps_sorted = reinterpret_cast<double*>(ws + L.tps_sorted);
-  a.thr = reinterpret_cast<double*>(ws + L.thr); a.nthr = reinterpret_cast<int*>(ws + L.nthr);
-  a.pr = reinterpret_cast<double*>(ws + L.pr); a.aos = reinterpret_cast<int*>(ws + L.aos);
-  const int C = 18 * ncls;
-  const long long nflag = static_cast<long long>(n_gt) + n_dt + C + 1;
-  flags_kernel<<<static_cast<unsigned>((nflag + 255) / 256), 256, 0, st>>>(a);
-  if (check_cuda(cudaGetLastError(), "kitti_eval_flags")) return -1;
-  const long long npass = static_cast<long long>(C) * n_img;
-  first_pass_kernel<<<static_cast<unsigned>((npass + 127) / 128), 128, 0, st>>>(a);
-  if (check_cuda(cudaGetLastError(), "kitti_eval_first_pass")) return -1;
-  if (n_gt > 0) {
-    size_t bytes = L.cub_bytes;
-    if (check_cuda(cub::DeviceSegmentedRadixSort::SortKeysDescending(ws + L.cub, bytes, a.tps, a.tps_sorted, C * n_gt, C,
-                                                                      a.seg, a.seg + 1, 0, 64, st),
-                   "kitti_eval_sort"))
-      return -1;
-  }
-  thresholds_kernel<<<C, THR_THREADS, 0, st>>>(a);
-  if (check_cuda(cudaGetLastError(), "kitti_eval_thresholds")) return -1;
-  second_pass_kernel<<<C * NPTS, STAT_THREADS, 0, st>>>(a);
-  return check_cuda(cudaGetLastError(), "kitti_eval_second_pass");
+  double table[OFFICIAL_SETS * 3 * MAX_CLS];
+  official_table(classes, ncls, table);
+  return run_statistics("mf_kitti_eval_statistics", gt, gt_off, dt, dt_off, pair_off, n_img, n_gt, n_dt, max_dt, overlaps,
+                        n_pair, classes, ncls, table, OFFICIAL_SETS, workspace, ws_bytes, stream);
+}
+
+int mf_kitti_eval_sets_statistics(const double* gt, const int* gt_off, const double* dt, const int* dt_off,
+                                  const long long* pair_off, int n_img, int n_gt, int n_dt, int max_dt,
+                                  const double* overlaps, long long n_pair, const int* classes, int ncls,
+                                  const double* min_overlaps, int n_sets, void* workspace, size_t ws_bytes,
+                                  void* stream) {
+  return run_statistics("mf_kitti_eval_sets_statistics", gt, gt_off, dt, dt_off, pair_off, n_img, n_gt, n_dt, max_dt,
+                        overlaps, n_pair, classes, ncls, min_overlaps, n_sets, workspace, ws_bytes, stream);
 }
 
 int mf_kitti_eval_ap(const void* workspace, int n_gt, int n_dt, int ncls, double* out, void* stream) {
-  if (ncls < 1 || ncls > MAX_CLS || workspace == nullptr) { set_error("mf_kitti_eval_ap: %d classes", ncls); return -1; }
-  const Layout L = layout(n_gt, n_dt, ncls);
-  const char* ws = static_cast<const char*>(workspace);
-  ap_kernel<<<1, 18 * ncls, 0, MF_STREAM(stream)>>>(reinterpret_cast<const double*>(ws + L.pr),
-                                                     reinterpret_cast<const int*>(ws + L.nthr),
-                                                     reinterpret_cast<const int*>(ws + L.aos), ncls, out);
-  return check_cuda(cudaGetLastError(), "kitti_eval_ap");
+  return run_ap("mf_kitti_eval_ap", workspace, n_gt, n_dt, ncls, OFFICIAL_SETS, out, stream);
+}
+
+int mf_kitti_eval_sets_ap(const void* workspace, int n_gt, int n_dt, int ncls, int n_sets, double* out, void* stream) {
+  return run_ap("mf_kitti_eval_sets_ap", workspace, n_gt, n_dt, ncls, n_sets, out, stream);
 }
 
 }  // extern "C"

@@ -1,15 +1,24 @@
-"""KITTI official 3D-detection metric on the GPU: 2D / BEV / 3D / AOS AP at R40 and R11.
+"""KITTI official 3D-detection metric on the GPU: 2D / BEV / 3D / AOS AP at R40 and R11, and the COCO-style AP over a
+sweep of overlap thresholds.
 
 A drop-in for the reference's `evaluate_python` (data/datasets/evaluation/__init__.py:33), which every `inference()`
-ends in, and for `get_official_eval_result` (kitti_object_eval_python/eval.py:644-726): the same `result` text and the
-same `ret_dict`. Overlaps, flags, matching, thresholds and AP run in monoflex_b200/csrc/mf_kitti_eval.cu; the host parses
-label files, packs the objects and formats the text. There is no CPU fallback: without the library or a GPU, calls raise.
+ends in, for `get_official_eval_result` (kitti_object_eval_python/eval.py:644-726) and `get_coco_eval_result`
+(eval.py:729-788): the same `result` text and the same `ret_dict`; and for kitti_object_eval_python's `evaluate()`
+entry (evaluate.py:14-32), also as a command line:
+
+    python -m monoflex_b200.evaluation --label_path L --result_path R --label_split_file S [--current_class 0,1,2]
+        [--coco] [--score_thresh T] [--metric R40|R11]
+
+Overlaps, flags, matching, thresholds and AP run in monoflex_b200/csrc/mf_kitti_eval.cu; the host parses label files,
+packs the objects and formats the text. There is no CPU fallback: without the library or a GPU, calls raise.
 """
+import argparse
 import ctypes
 import io
 import os
 import pathlib
 import re
+import sys
 
 import numpy as np
 import torch
@@ -28,6 +37,10 @@ N_SAMPLE_PTS = 41
 MIN_OVERLAPS = np.stack([np.array([[0.7, 0.5, 0.5, 0.7, 0.5, 0.7]] * 3),
                          np.array([[0.7, 0.5, 0.5, 0.7, 0.5, 0.5], [0.5, 0.25, 0.25, 0.5, 0.25, 0.5],
                                    [0.5, 0.25, 0.25, 0.5, 0.25, 0.5]])], axis=0)
+# get_coco_eval_result's classes and their (start, stop, count) of overlap thresholds; Truck has none
+COCO_CLASS_TO_NAME = {0: 'Car', 1: 'Pedestrian', 2: 'Cyclist', 3: 'Van', 4: 'Person_sitting'}
+COCO_CLASS_TO_RANGE = {0: [0.5, 0.95, 10], 1: [0.25, 0.7, 10], 2: [0.25, 0.7, 10], 3: [0.5, 0.95, 10],
+                       4: [0.25, 0.7, 10]}
 
 
 def class_code(name):
@@ -120,11 +133,17 @@ def _as_annos(a):
     return a if isinstance(a, KittiAnnos) else KittiAnnos.from_annos(a)
 
 
-def eval_tables(gt, dt, classes, events=None):
+def eval_tables(gt, dt, classes, events=None, min_overlaps=None):
     """every configuration at once on the GPU. Returns (tables, overlaps): tables has recall / precision / aos
-    [3 metric][ncls][3 difficulty][2 overlap set][41] (eval_class's arrays per metric), ap [2 (R40, R11)][4 (bbox, bev,
-    3d, aos)][ncls][3][2] and compute_aos; overlaps is the device tensor [3, n_pair] of the per-image blocks. `events`, if
-    given, receives CUDA events recorded before and after each stage."""
+    [3 metric][ncls][3 difficulty][n_sets overlap set][41] (eval_class's arrays per metric), ap [2 (R40, R11)][4 (bbox,
+    bev, 3d, aos)][ncls][3][n_sets] and compute_aos; overlaps is the device tensor [3, n_pair] of the per-image blocks.
+    min_overlaps: eval_class's float64 table [n_sets][3 metric][ncls], its values compared as given; None is
+    get_official_eval_result's two sets. `events`, if given, receives CUDA events recorded before and after each stage."""
+    if min_overlaps is not None:
+        min_overlaps = np.ascontiguousarray(min_overlaps, dtype=np.float64)
+        if min_overlaps.ndim != 3 or min_overlaps.shape[1:] != (3, len(classes)) or min_overlaps.shape[0] < 1:
+            raise ValueError("eval_tables: min_overlaps must be [n_sets >= 1, 3, %d], got %s"
+                             % (len(classes), min_overlaps.shape))
     gt, dt = _as_annos(gt), _as_annos(dt)
     for name, a in (("ground truth", gt), ("detections", dt)):
         if not a.objects.is_cuda:
@@ -146,12 +165,19 @@ def eval_tables(gt, dt, classes, events=None):
     pair_off = torch.from_numpy(pair_off).to(dev)
     n_gt, n_dt = gt.objects.shape[0], dt.objects.shape[0]
     overlaps = torch.empty(3, max(n_pair, 1), dtype=torch.float64, device=dev)
-    ws_bytes = _lib.load().mf_kitti_eval_workspace(n_gt, n_dt, ncls)
+    n_sets = 2 if min_overlaps is None else min_overlaps.shape[0]
+    if min_overlaps is None:
+        ws_bytes = _lib.load().mf_kitti_eval_workspace(n_gt, n_dt, ncls)
+    else:
+        size = ctypes.c_size_t(0)
+        if _lib.load().mf_kitti_eval_sets_workspace_size(n_gt, n_dt, ncls, n_sets, ctypes.byref(size)) != 0:
+            raise ValueError(_lib.load().mf_last_error().decode())
+        ws_bytes = size.value
     if ws_bytes == 0:
         raise ValueError("%d classes: between 1 and 8 are supported" % ncls)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
-    C = 18 * ncls
-    out = torch.empty(3 * C * N_SAMPLE_PTS + 8 * 6 * ncls + 2, dtype=torch.float64, device=dev)
+    C = 9 * n_sets * ncls
+    out = torch.empty(3 * C * N_SAMPLE_PTS + 8 * C // 3 + 2, dtype=torch.float64, device=dev)
     st = _lib.stream()
     cls_arr = (ctypes.c_int * ncls)(*classes)
     common = (_lib.ptr(gt.objects), _lib.ptr(gt.offsets), _lib.ptr(dt.objects), _lib.ptr(dt.offsets), _lib.ptr(pair_off))
@@ -164,20 +190,29 @@ def eval_tables(gt, dt, classes, events=None):
     mark()
     _lib.call("mf_kitti_eval_overlaps", *common, len(gt), n_pair, _lib.ptr(overlaps), st)
     mark()
-    _lib.call("mf_kitti_eval_statistics", *common, len(gt), n_gt, n_dt, int(dt.counts.max()), _lib.ptr(overlaps), n_pair,
-              cls_arr, ncls, _lib.ptr(ws), ws_bytes, st)
+    max_dt = int(dt.counts.max())
+    if min_overlaps is None:
+        _lib.call("mf_kitti_eval_statistics", *common, len(gt), n_gt, n_dt, max_dt, _lib.ptr(overlaps), n_pair,
+                  cls_arr, ncls, _lib.ptr(ws), ws_bytes, st)
+    else:
+        _lib.call("mf_kitti_eval_sets_statistics", *common, len(gt), n_gt, n_dt, max_dt, _lib.ptr(overlaps), n_pair,
+                  cls_arr, ncls, min_overlaps.ctypes.data, n_sets, _lib.ptr(ws), ws_bytes, st)
     mark()
-    _lib.call("mf_kitti_eval_ap", _lib.ptr(ws), n_gt, n_dt, ncls, _lib.ptr(out), st)
+    if min_overlaps is None:
+        _lib.call("mf_kitti_eval_ap", _lib.ptr(ws), n_gt, n_dt, ncls, _lib.ptr(out), st)
+    else:
+        _lib.call("mf_kitti_eval_sets_ap", _lib.ptr(ws), n_gt, n_dt, ncls, n_sets, _lib.ptr(out), st)
     mark()
     h = out.cpu().numpy()
     if h[-1] > 0:
         raise RuntimeError("eval_tables: an image has %d detections, more than the %d per image the matching kernels take"
                            % (int(h[-1]), MAX_DT))
-    shape = (3, ncls, 3, 2, N_SAMPLE_PTS)
+    shape = (3, ncls, 3, n_sets, N_SAMPLE_PTS)
     n = int(np.prod(shape))
+    n_ap = 8 * ncls * 3 * n_sets
     tables = {'recall': h[:n].reshape(shape), 'precision': h[n:2 * n].reshape(shape),
-              'orientation': h[2 * n:3 * n].reshape(shape), 'ap': h[3 * n:3 * n + 48 * ncls].reshape(2, 4, ncls, 3, 2),
-              'compute_aos': bool(h[-2])}
+              'orientation': h[2 * n:3 * n].reshape(shape),
+              'ap': h[3 * n:3 * n + n_ap].reshape(2, 4, ncls, 3, n_sets), 'compute_aos': bool(h[-2])}
     return tables, overlaps[:, :n_pair]
 
 
@@ -235,6 +270,63 @@ def get_official_eval_result(gt_annos, dt_annos, current_classes, PR_detail_dict
     return result, ret_dict
 
 
+def coco_min_overlaps(current_classes):
+    """do_coco_style_eval's [10 set][3 metric][ncls] table: each class's (start, stop, count) through np.linspace with an
+    integer count, the same thresholds for 2D, BEV and 3D. A class without a range (Truck) raises KeyError."""
+    overlap_ranges = np.zeros([3, 3, len(current_classes)])
+    for i, curcls in enumerate(current_classes):
+        overlap_ranges[:, :, i] = np.array(COCO_CLASS_TO_RANGE[curcls])[:, np.newaxis]
+    min_overlaps = np.zeros([10, *overlap_ranges.shape[1:]])
+    for i in range(overlap_ranges.shape[1]):
+        for j in range(overlap_ranges.shape[2]):
+            start, stop, num = overlap_ranges[:, i, j]
+            min_overlaps[:, i, j] = np.linspace(start, stop, int(num))
+    return min_overlaps
+
+
+def get_coco_eval_result(gt_annos, dt_annos, current_classes):
+    """eval.py:729-788 on the GPU: the same text. 2D / BEV / 3D / AOS AP at R40 per overlap set, averaged over the ten
+    sets of coco_min_overlaps by numpy's mean. gt_annos / dt_annos: KittiAnnos or the reference's lists of get_label_anno
+    dicts; classes by id or name, Truck excluded (KeyError, as in the reference)."""
+    name_to_class = {v: n for n, v in COCO_CLASS_TO_NAME.items()}
+    if not isinstance(current_classes, (list, tuple)):
+        current_classes = [current_classes]
+    current_classes = [name_to_class[c] if isinstance(c, str) else c for c in current_classes]
+    min_overlaps = coco_min_overlaps(current_classes)
+    tables, _ = eval_tables(gt_annos, dt_annos, current_classes, min_overlaps=min_overlaps)
+    return coco_result_text(current_classes, tables['ap'][0], tables['compute_aos'])
+
+
+def coco_result_text(current_classes, ap, compute_aos):
+    """get_coco_eval_result's text from the AP at R40 (do_eval's default metric) per overlap set, ap [4 (bbox, bev, 3d,
+    aos)][ncls][3][10], of the class ids current_classes"""
+    mAPbbox, mAPbev, mAP3d = (np.ascontiguousarray(ap[i]).mean(-1) for i in range(3))
+    mAPaos = np.ascontiguousarray(ap[3]).mean(-1) if compute_aos else None
+    result = ''
+    for j, curcls in enumerate(current_classes):
+        o_range = np.array(COCO_CLASS_TO_RANGE[curcls])[[0, 2, 1]]
+        o_range[1] = (o_range[2] - o_range[0]) / (o_range[1] - 1)
+        result += print_str((f"{COCO_CLASS_TO_NAME[curcls]} " "coco AP@{:.2f}:{:.2f}:{:.2f}:".format(*o_range)))
+        result += print_str(f"bbox AP:{mAPbbox[j, 0]:.2f}, {mAPbbox[j, 1]:.2f}, {mAPbbox[j, 2]:.2f}")
+        result += print_str(f"bev  AP:{mAPbev[j, 0]:.2f}, {mAPbev[j, 1]:.2f}, {mAPbev[j, 2]:.2f}")
+        result += print_str(f"3d   AP:{mAP3d[j, 0]:.2f}, {mAP3d[j, 1]:.2f}, {mAP3d[j, 2]:.2f}")
+        if compute_aos:
+            result += print_str(f"aos  AP:{mAPaos[j, 0]:.2f}, {mAPaos[j, 1]:.2f}, {mAPaos[j, 2]:.2f}")
+    return result
+
+
+def filter_low_score(annos, thresh):
+    """kitti_common.filter_annos_low_score on the device: the detections whose score is >= thresh, in order, each image
+    recounted"""
+    annos = _as_annos(annos)
+    obj = annos.objects
+    keep = obj[:, 15] >= thresh
+    image = torch.repeat_interleave(torch.arange(len(annos), device=obj.device),
+                                    torch.from_numpy(annos.counts).to(obj.device))
+    counts = torch.bincount(image[keep], minlength=len(annos))
+    return KittiAnnos(obj[keep], counts.cpu().numpy())
+
+
 def write_kitti_detections(rows, path):
     """generate_kitti_3d_detection (kitti_object_eval_python/evaluate.py:34-53), byte for byte: one line per row of the
     decode's result [n, 14] (class, alpha, x1, y1, x2, y2, h, w, l, x, y, z, ry, score) - the class name, 0, 0, then the
@@ -255,3 +347,44 @@ def evaluate_python(label_path, result_path, label_split_file, current_class, me
         ids = [int(line) for line in f.readlines()]
     gt = KittiAnnos.from_label_dir(label_path, ids)
     return get_official_eval_result(gt, dt, current_class, metric=metric)
+
+
+def evaluate(label_path, result_path, label_split_file, current_class=0, coco=False, score_thresh=-1, metric='R40'):
+    """kitti_object_eval_python/evaluate.py:14-32: the result folder's detection files (sorted ids) against the ground
+    truth of the split file's ids, paired by position. score_thresh > 0 first drops the detections scored below it.
+    Returns get_coco_eval_result's text when coco, else get_official_eval_result's (result, ret_dict) at `metric`."""
+    dt = KittiAnnos.from_label_dir(result_path)
+    if score_thresh > 0:
+        dt = filter_low_score(dt, score_thresh)
+    with open(label_split_file, 'r') as f:
+        ids = [int(line) for line in f.readlines()]
+    gt = KittiAnnos.from_label_dir(label_path, ids)
+    if coco:
+        return get_coco_eval_result(gt, dt, current_class)
+    return get_official_eval_result(gt, dt, current_class, metric=metric)
+
+
+def parse_classes(text):
+    """'0,1,2' or 'Car,Pedestrian': class ids and names as evaluate() takes them"""
+    return [int(c) if re.fullmatch(r'-?\d+', c) else c for c in (t.strip() for t in text.split(','))]
+
+
+def main(argv=None):
+    p = argparse.ArgumentParser(prog="python -m monoflex_b200.evaluation",
+                                description="Score a folder of KITTI result files against the labels of a split: the "
+                                            "official AP table, or the COCO-style AP over overlap thresholds.")
+    p.add_argument("--label_path", required=True, help="folder of ground-truth label files (000123.txt)")
+    p.add_argument("--result_path", required=True, help="folder of detection files, one per image of the split")
+    p.add_argument("--label_split_file", required=True, help="image ids of the split, one per line")
+    p.add_argument("--current_class", default="0", help="comma-separated class ids or names (default: 0)")
+    p.add_argument("--coco", action="store_true", help="AP averaged over ten overlap thresholds per class")
+    p.add_argument("--score_thresh", type=float, default=-1, help="drop detections scored below it when > 0")
+    p.add_argument("--metric", choices=("R40", "R11"), default="R40", help="recall positions of the official AP")
+    args = p.parse_args(argv)
+    out = evaluate(args.label_path, args.result_path, args.label_split_file, parse_classes(args.current_class),
+                   coco=args.coco, score_thresh=args.score_thresh, metric=args.metric)
+    sys.stdout.write(out if args.coco else out[0])
+
+
+if __name__ == "__main__":
+    main()
