@@ -441,6 +441,18 @@ int mf_decode_detections_depths(const float* heat, const float* reg, const float
                                 float* ws_score, int* ws_idx, float* scores, long long* inds, float* clses, float* ys,
                                 float* xs, float* pois, float* result, int* count, float* depth_err, float* proj,
                                 int* min_unc, void* stream);
+/* PostProcessor.evaluate_3D_depths (model/head/detector_infer.py:280-359; the --eval_depth diagnostic): the depth errors
+ * of every estimator at the ground-truth centres, replacing its POI gather of a permuted map (layers/utils.py:120-145),
+ * decode_dimension / decode_depth / decode_depth_from_keypoints_batch (anno_encoder.py:124-243) and the torch reductions.
+ * reg [B,R=50,H,W] fp32 NCHW, calib [B,6] as above (each image uses its own f_u), dim_mean [C,3], gt [B,M,5] fp32 =
+ * (reg_mask, cls_id, target_centers x, y, locations z) per object slot. A slot with reg_mask == 0 is skipped and never
+ * read through. Outputs: out [13, B*M] fp32, the valid slots compacted in the order of reg_mask.view(-1), one column
+ * each, rows = direct, direct_sigma, keypoint_center, keypoint_02, keypoint_13, keypoint_center_sigma, keypoint_02_sigma,
+ * keypoint_13_sigma, sigma_min, sigma_weighted, mean, min, target (columns past the valid count are not written);
+ * counts [B] int32 = valid slots per image. A valid slot whose centre lies outside the HxW map, or whose class lies
+ * outside 0..C-1, is not read: its column is NaN in every row. */
+int mf_eval_depth_errors(const float* reg, const float* calib, const float* dim_mean, const float* gt, int B, int M, int C,
+                         int H, int W, int R, float* out, int* counts, void* stream);
 
 /* ---- KITTI official metric (data/datasets/evaluation/kitti_object_eval_python/eval.py:644-726, rotate_iou.py) ---------
  * Objects: float64 rows of MF_KITTI_OBJ values, CSR-packed per image (gt_off / dt_off: DEVICE int32 [n_img + 1]):

@@ -321,6 +321,37 @@ __device__ __forceinline__ void oracle_depth(const float* __restrict__ gt, int G
   err = bs;
 }
 
+// decode_dimension anno_encoder.py:221-243 ('exp', class mean, no std) of a POI q[50] -> (l, h, w)
+__device__ __forceinline__ void decode_dims(const float* q, const float* __restrict__ dim_mean, int cls, float& dl, float& dh,
+                                            float& dw) {
+  dl = expf(q[29]) * dim_mean[cls * 3 + 0];
+  dh = expf(q[30]) * dim_mean[cls * 3 + 1];
+  dw = expf(q[31]) * dim_mean[cls * 3 + 2];
+}
+
+// The four depth estimators of a POI q[50] and their uncertainties, in the ensemble's order (direct, key-point centre,
+// corners 02, corners 13): decode_depth :124-140 (inv_sigmoid, DEPTH_RANGE [0.1, 100]) and
+// decode_depth_from_keypoints_batch :187-219 with the object height dh and the image's f_u; sig = exp of
+// depth_uncertainty / corner_uncertainty (detector_infer.py:135, :146).
+__device__ __forceinline__ void decode_four_depths(const float* q, float f_u, float dh, float dr, float dep[4], float sig[4]) {
+  dep[0] = fminf(fmaxf(1.f / (1.f / (1.f + expf(-q[48]))) - 1.f, 0.1f), 100.f);
+  sig[0] = expf(q[49]);
+  const float* kp = q + 6;   // 10 x (x, y)
+  const float ch_ = kp[8 * 2 + 1] - kp[9 * 2 + 1];
+  dep[1] = f_u * dh / (fmaxf(ch_, 0.f) * dr + 1e-3f);
+  const float a02 = f_u * dh / (fmaxf(kp[0 * 2 + 1] - kp[4 * 2 + 1], 0.f) * dr + 1e-3f);
+  const float b02 = f_u * dh / (fmaxf(kp[2 * 2 + 1] - kp[6 * 2 + 1], 0.f) * dr + 1e-3f);
+  dep[2] = (a02 + b02) / 2.f;
+  const float a13 = f_u * dh / (fmaxf(kp[1 * 2 + 1] - kp[5 * 2 + 1], 0.f) * dr + 1e-3f);
+  const float b13 = f_u * dh / (fmaxf(kp[3 * 2 + 1] - kp[7 * 2 + 1], 0.f) * dr + 1e-3f);
+  dep[3] = (a13 + b13) / 2.f;
+#pragma unroll
+  for (int i = 1; i < 4; ++i) {
+    dep[i] = fminf(fmaxf(dep[i], 0.1f), 100.f);
+    sig[i] = expf(q[26 + i - 1]);
+  }
+}
+
 // channel map runs/monoflex.yaml:27-28: 2d_dim 0:4 | 3d_offset 4:6 | corner_offset 6:26 | corner_uncertainty 26:29 |
 // 3d_dim 29:32 | ori_cls 32:40 | ori_offset 40:48 | depth 48 | depth_uncertainty 49
 static constexpr int S2_THREADS = 1024;
@@ -416,28 +447,10 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
   float x2 = (xf + fmaxf(q[2], 0.f)) * dr - padx, y2 = (yf + fmaxf(q[3], 0.f)) * dr - pady;
   x1 = fminf(fmaxf(x1, 0.f), wmax); x2 = fminf(fmaxf(x2, 0.f), wmax);
   y1 = fminf(fmaxf(y1, 0.f), hmax); y2 = fminf(fmaxf(y2, 0.f), hmax);
-  // decode_dimension :221-243 -> (l, h, w)
-  const float dl = expf(q[29]) * p.dim_mean[cls * 3 + 0];
-  const float dh = expf(q[30]) * p.dim_mean[cls * 3 + 1];
-  const float dw = expf(q[31]) * p.dim_mean[cls * 3 + 2];
-  // depths :124-140, :187-219
-  float dep[4], sig[4];
-  dep[0] = fminf(fmaxf(1.f / (1.f / (1.f + expf(-q[48]))) - 1.f, 0.1f), 100.f);
-  sig[0] = expf(q[49]);
-  const float* kp = q + 6;   // 10 x (x, y)
-  const float ch_ = kp[8 * 2 + 1] - kp[9 * 2 + 1];
-  dep[1] = f_u * dh / (fmaxf(ch_, 0.f) * dr + 1e-3f);
-  const float a02 = f_u * dh / (fmaxf(kp[0 * 2 + 1] - kp[4 * 2 + 1], 0.f) * dr + 1e-3f);
-  const float b02 = f_u * dh / (fmaxf(kp[2 * 2 + 1] - kp[6 * 2 + 1], 0.f) * dr + 1e-3f);
-  dep[2] = (a02 + b02) / 2.f;
-  const float a13 = f_u * dh / (fmaxf(kp[1 * 2 + 1] - kp[5 * 2 + 1], 0.f) * dr + 1e-3f);
-  const float b13 = f_u * dh / (fmaxf(kp[3 * 2 + 1] - kp[7 * 2 + 1], 0.f) * dr + 1e-3f);
-  dep[3] = (a13 + b13) / 2.f;
-#pragma unroll
-  for (int i = 1; i < 4; ++i) {
-    dep[i] = fminf(fmaxf(dep[i], 0.1f), 100.f);
-    sig[i] = expf(q[26 + i - 1]);
-  }
+  float dl, dh, dw;                                  // decode_dimension :221-243 -> (l, h, w)
+  decode_dims(q, p.dim_mean, cls, dl, dh, dw);
+  float dep[4], sig[4];                              // depths :124-140, :187-219
+  decode_four_depths(q, f_u, dh, dr, dep, sig);
   // projected 3D centre on the map (:125) and the multi-bin orientation :245-295: argmax over softmax(bin logits)[..., 1]
   // (first max wins); neither depends on the depth
   const float px = xf + q[4], py = yf + q[5];
@@ -511,6 +524,93 @@ __global__ void __launch_bounds__(S2_THREADS) topk_decode_stage2_kernel(const De
     float* r = p.result + om * 14;
     r[0] = static_cast<float>(cls); r[1] = alpha; r[2] = x1; r[3] = y1; r[4] = x2; r[5] = y2;
     r[6] = dh; r[7] = dw; r[8] = dl; r[9] = lx; r[10] = ly; r[11] = depth; r[12] = roty; r[13] = conf;
+  }
+}
+
+// PostProcessor.evaluate_3D_depths (detector_infer.py:280-359): the errors of every depth estimator at the ground-truth
+// centres. gt [B, M, 5] = (reg_mask, cls_id, x, y, z) per object slot. One CTA walks the B*M slots in chunks of
+// ED_THREADS, one thread per slot; a block-wide scan of the valid flags puts the valid slots' rows in the order of
+// reg_mask.view(-1), so column j of out [EVAL_DEPTH_KEYS, B*M] is the j-th valid object. An invalid slot is never read
+// through. The POI index is float(y) * W + float(x) truncated like .long() (layers/utils.py:132), read straight from the
+// NCHW map. A valid slot whose centre or class lies outside the map / dim_mean (the reference fails in gather or in the
+// dim_mean lookup there) is not read either: its column is NaN in every key.
+static constexpr int EVAL_DEPTH_KEYS = 13;
+static constexpr int ED_THREADS = 256;
+
+__global__ void __launch_bounds__(ED_THREADS)
+eval_depth_errors_kernel(const float* __restrict__ reg, const float* __restrict__ calib, const float* __restrict__ dim_mean,
+                         const float* __restrict__ gt, int B, int M, int C, int H, int W, int R, float* __restrict__ out,
+                         int* __restrict__ counts) {
+  __shared__ int warp_valid[ED_THREADS / 32];
+  __shared__ int s_base;
+  const int n = B * M, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const long long HW = static_cast<long long>(H) * W;
+  if (threadIdx.x == 0) s_base = 0;
+  __syncthreads();
+  for (int c0 = 0; c0 < n; c0 += ED_THREADS) {
+    const int i = c0 + static_cast<int>(threadIdx.x);
+    const float* t = gt + static_cast<long long>(i) * 5;
+    const bool valid = i < n && t[0] != 0.f;
+    const unsigned int ballot = __ballot_sync(0xffffffffu, valid);
+    if (lane == 0) warp_valid[warp] = __popc(ballot);
+    __syncthreads();
+    int row = s_base + __popc(ballot & ((1u << lane) - 1u));
+    for (int w = 0; w < warp; ++w) row += warp_valid[w];
+    if (valid) {
+      const int b = i / M;
+      const float x = t[2], y = t[3], z = t[4], cls_f = t[1];
+      const float idx_f = __fadd_rn(__fmul_rn(y, static_cast<float>(W)), x);     // index[:, :, 1] * w + index[:, :, 0]
+      const bool inside = x >= 0.f && x < static_cast<float>(W) && y >= 0.f && y < static_cast<float>(H) &&
+                          idx_f < static_cast<float>(HW) && cls_f > -1.f && cls_f < static_cast<float>(C);
+      float e[EVAL_DEPTH_KEYS];
+      if (inside) {
+        const long long idx = static_cast<long long>(idx_f);
+        const int cls = static_cast<int>(cls_f);
+        float q[50];
+#pragma unroll
+        for (int ch = 0; ch < 50; ++ch) q[ch] = __ldg(reg + (static_cast<long long>(b) * R + ch) * HW + idx);
+        float dl, dh, dw;
+        decode_dims(q, dim_mean, cls, dl, dh, dw);
+        float dep[4], sig[4];
+        decode_four_depths(q, calib[b * 6 + 0], dh, 4.f, dep, sig);
+        // min-uncertainty: the depth at argmin of the uncertainties (first index on ties, :318)
+        int am = 0;
+#pragma unroll
+        for (int k = 1; k < 4; ++k)
+          if (sig[k] < sig[am]) am = k;
+        const float d_min_unc = am == 0 ? dep[0] : am == 1 ? dep[1] : am == 2 ? dep[2] : dep[3];
+        // inverse-uncertainty weighted (:320-323)
+        float wts[4], wsum = 0.f, d_weighted = 0.f;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { wts[k] = 1.f / sig[k]; wsum += wts[k]; }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) d_weighted += dep[k] * (wts[k] / wsum);
+        const float d_mean = (dep[0] + dep[1] + dep[2] + dep[3]) / 4.f;
+        float err[4], err_min;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) err[k] = fabsf(dep[k] - z);
+        err_min = fminf(fminf(err[0], err[1]), fminf(err[2], err[3]));
+        e[0] = err[0]; e[1] = sig[0];
+        e[2] = err[1]; e[3] = err[2]; e[4] = err[3];
+        e[5] = sig[1]; e[6] = sig[2]; e[7] = sig[3];
+        e[8] = fabsf(d_min_unc - z); e[9] = fabsf(d_weighted - z); e[10] = fabsf(d_mean - z); e[11] = err_min;
+        e[12] = z;
+      } else {
+#pragma unroll
+        for (int k = 0; k < EVAL_DEPTH_KEYS; ++k) e[k] = CUDART_NAN_F;
+      }
+#pragma unroll
+      for (int k = 0; k < EVAL_DEPTH_KEYS; ++k) out[static_cast<long long>(k) * n + row] = e[k];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int w = 0; w < ED_THREADS / 32; ++w) s_base += warp_valid[w];
+    __syncthreads();
+  }
+  for (int b = threadIdx.x; b < B; b += ED_THREADS) {
+    int cnt = 0;
+    for (int m = 0; m < M; ++m) cnt += gt[(static_cast<long long>(b) * M + m) * 5] != 0.f ? 1 : 0;
+    counts[b] = cnt;
   }
 }
 
@@ -624,6 +724,24 @@ int mf_decode_detections(const float* heat, const float* reg, const float* calib
                          float* depth_err, float* proj, int* min_unc, void* stream) {
   return decode_launch(heat, reg, calib, pad, size, dim_mean, B, C, H, W, R, K, thresh, apply_sigmoid, &depth_mode, 1, gt, G,
                        s1_score, s1_idx, scores, inds, clses, ys, xs, pois, result, count, depth_err, proj, min_unc, stream);
+}
+
+int mf_eval_depth_errors(const float* reg, const float* calib, const float* dim_mean, const float* gt, int B, int M, int C,
+                         int H, int W, int R, float* out, int* counts, void* stream) {
+  if (reg == nullptr || calib == nullptr || dim_mean == nullptr || gt == nullptr || out == nullptr || counts == nullptr) {
+    set_error("eval_depth_errors: null pointer (reg=%p calib=%p dim_mean=%p gt=%p out=%p counts=%p)",
+              static_cast<const void*>(reg), static_cast<const void*>(calib), static_cast<const void*>(dim_mean),
+              static_cast<const void*>(gt), static_cast<void*>(out), static_cast<void*>(counts));
+    return -1;
+  }
+  if (B < 1 || M < 1 || C < 1 || H < 1 || W < 1 || R != 50 || static_cast<long long>(B) * M * EVAL_DEPTH_KEYS > 0x7fffffffLL) {
+    set_error("eval_depth_errors: unsupported shape B=%d M=%d C=%d H=%d W=%d R=%d (R must be 50, the others positive)",
+              B, M, C, H, W, R);
+    return -1;
+  }
+  (void)launch_k(eval_depth_errors_kernel, dim3(1), dim3(ED_THREADS), 0, MF_STREAM(stream), reg, calib, dim_mean, gt, B, M,
+                 C, H, W, R, out, counts);
+  return check_cuda(cudaGetLastError(), "eval_depth_errors");
 }
 
 int mf_decode_detections_depths(const float* heat, const float* reg, const float* calib, const float* pad, const float* size,

@@ -24,6 +24,7 @@ from .. import engine
 from ..structures import to_image_list
 from .backbone import build_backbone
 from .head.detector_head import bulid_head
+from .layers.utils import depth_error_dict
 
 
 class _TapeBridge(torch.autograd.Function):
@@ -158,7 +159,8 @@ class KeypointDetector(nn.Module):
         """Enqueue one eval forward (graph replay) and return a handle; `handle.result()` waits for it and returns what
         `forward` returns. Lets a caller overlap the host-side read of step i with the GPU work of step i+1 (the decode
         workspace is re-used by the next forward, so call `result()` - or at least `stage()` - before the forward after
-        next)."""
+        next). With TEST.EVAL_DEPTH, `result()` also sets `handle.eval_utils['depth_errors']` /
+        `['depth_error_counts']` as forward fills them."""
         if self.training:
             raise RuntimeError("forward_async is an inference API")
         x = to_image_list(images).tensors
@@ -194,10 +196,11 @@ class KeypointDetector(nn.Module):
         post.check_config(methods)
         x = x.float().contiguous()
         k_edge = targets[0].get_field("edge_indices").shape[0]
-        # per-call target fields of the decode: calib / pad / size and, for the oracle depth, the ground-truth table
+        # per-call target fields of the decode: calib / pad / size and, for the oracle depth and for TEST.EVAL_DEPTH, the
+        # ground-truth tables
         meta = post.prepare_targets(targets, self.test, x.device, methods)
         key = (tuple(x.shape), x.device, k_edge, engine.fingerprint(self), post.det_threshold, post.max_detection, self.precision,
-               post.output_depth if methods is None else methods, tuple(tuple(m.shape) for m in meta))
+               post.output_depth if methods is None else methods, post.eval_depth, tuple(tuple(m.shape) for m in meta))
         g = self._graph if methods is None else self._graph_depths
         if g is None or g['key'] != key:
             g = self._capture(x, targets, key, meta, methods)
@@ -235,32 +238,43 @@ class KeypointDetector(nn.Module):
 
 class PendingDetections(object):
     """Handle of an enqueued forward: `stage()` starts the device->host copy of the padded detections + counts into
-    pinned buffers (asynchronous, stream ordered), `result()` waits for it and slices on the host."""
+    pinned buffers (asynchronous, stream ordered), `result()` waits for it and slices on the host. With TEST.EVAL_DEPTH
+    the same copy carries the depth errors' counts, and `stage()` copies their table on the device into a buffer of its
+    own; `result()` then sets `eval_utils` = {'depth_errors': the dict forward returns, 'depth_error_counts': [B]}
+    (before it, and without EVAL_DEPTH, eval_utils['depth_errors'] is None)."""
 
     def __init__(self, post, ws, heat):
         self.post, self.ws, self.heat = post, ws, heat
         self._staged = None
+        self.eval_utils = {'depth_errors': None}
 
     def stage(self):
         if self._staged is None:
             ws = self.ws
             host = getattr(ws, "_pinned", None)
             if host is None:
-                host = ws._pinned = [(torch.empty(ws.result.shape).pin_memory(), torch.empty(ws.count.shape, dtype=torch.int32).pin_memory(),
-                                      torch.cuda.Event()) for _ in range(2)]
+                cnt = ws.count if ws.depth_errors is None else ws.counts
+                host = ws._pinned = [(torch.empty(ws.result.shape).pin_memory(), torch.empty(cnt.shape, dtype=torch.int32).pin_memory(),
+                                      torch.cuda.Event(), None if ws.depth_errors is None else torch.empty_like(ws.depth_errors))
+                                     for _ in range(2)]
                 ws._pin_i = 0
-            res_h, cnt_h, ev = host[ws._pin_i]
+            res_h, cnt_h, ev, errs = host[ws._pin_i]
             ws._pin_i ^= 1
             res_h.copy_(ws.result, non_blocking=True)
-            cnt_h.copy_(ws.count, non_blocking=True)
+            cnt_h.copy_(ws.count if errs is None else ws.counts, non_blocking=True)
+            if errs is not None:
+                errs.copy_(ws.depth_errors)
             ev.record()
-            self._staged = (res_h, cnt_h, ev)
+            self._staged = (res_h, cnt_h, ev, errs)
         return self
 
     def result(self):
         """-> (result[N,14] on the HOST, counts list): the rows `forward` would return, read through pinned memory."""
-        res_h, cnt_h, ev = self.stage()._staged
+        res_h, cnt_h, ev, errs = self.stage()._staged
         ev.synchronize()
         counts = cnt_h.tolist()
+        if errs is not None:
+            counts, depth_counts = counts
+            self.eval_utils = {'depth_errors': depth_error_dict(errs, depth_counts), 'depth_error_counts': depth_counts}
         rows = [res_h[b, :n] for b, n in enumerate(counts)]
         return (torch.cat(rows, 0) if len(rows) > 1 else rows[0].clone()), counts

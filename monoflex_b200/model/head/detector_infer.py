@@ -13,14 +13,20 @@ Every OUTPUT_DEPTH estimator of the reference is decoded by the kernel: 'soft' (
 every forward, so engine/inference.py's inference_all_depths can switch it between passes. The oracle matches every
 detection against its own image's ground truth (reg_mask, cls_ids, gt_bboxes, locations); the reference matches the
 whole batch against targets[0], which is the same thing for B = 1. An image without valid ground truth keeps the mean
-of the four estimators, where the reference raises (argmin of an empty tensor). The --eval_iou / --eval_depth
-diagnostics are out of scope (DESIGN.md §9)."""
+of the four estimators, where the reference raises (argmin of an empty tensor).
+
+TEST.EVAL_DEPTH (--eval_depth) runs evaluate_3D_depths in one more kernel after the decode (inside the captured graph
+of KeypointDetector): eval_utils['depth_errors'] is the reference's dict of 13 per-object tensors, with the rows of
+every image in (image, slot) order, and eval_utils['depth_error_counts'] the valid objects of each image. The reference
+is batch-1 only there too. The --eval_iou diagnostic (TEST.EVAL_DIS_IOUS) is out of scope (DESIGN.md §9)."""
 import torch
 from torch import nn
 
-from ..layers.utils import DEPTH_MODES, ENSEMBLE_DEPTH_MODES, Converter_key2channel, DecodeWorkspace, decode_detections
+from ..layers.utils import (DEPTH_MODES, ENSEMBLE_DEPTH_MODES, Converter_key2channel, DecodeWorkspace, decode_detections,
+                            depth_error_dict, eval_depth_errors)
 
 ORACLE_FIELDS = ('reg_mask', 'cls_ids', 'gt_bboxes', 'locations')
+EVAL_DEPTH_FIELDS = ('target_centers', 'reg_mask', 'cls_ids', 'locations')
 
 
 def make_post_processor(cfg):
@@ -58,7 +64,7 @@ class PostProcessor(nn.Module):
         """calib / pad_size / size of every image as three small device tensors (detector_infer.py:53-58). The host-side
         scalars (calibration, image size) are cached BY VALUE; pad_size is stacked on the device like the reference
         does, so a CUDA `pad_size` field costs no host sync. The oracle table is appended when `methods` (default: the
-        output_depth alone) include 'oracle'."""
+        output_depth alone) include 'oracle', then the depth_table when TEST.EVAL_DEPTH is set."""
         calib, size = [], []
         for t in targets:
             c = t.get_field("calib")
@@ -70,9 +76,12 @@ class PostProcessor(nn.Module):
                                 torch.tensor(size, dtype=torch.float32).to(device))
         pad = torch.stack([torch.as_tensor(t.get_field("pad_size")) for t in targets]).to(device=device, dtype=torch.float32,
                                                                                          non_blocking=True).view(-1, 2)
-        if 'oracle' not in ((self.output_depth,) if methods is None else methods):
-            return self._meta_cache[1], pad, self._meta_cache[2]
-        return self._meta_cache[1], pad, self._meta_cache[2], self.oracle_table(targets, device)
+        meta = (self._meta_cache[1], pad, self._meta_cache[2])
+        if 'oracle' in ((self.output_depth,) if methods is None else methods):
+            meta += (self.oracle_table(targets, device),)
+        if self.eval_depth:
+            meta += (self.depth_table(targets, device),)
+        return meta
 
     @staticmethod
     def oracle_table(targets, device):
@@ -90,22 +99,41 @@ class PostProcessor(nn.Module):
             rows.append(torch.cat([f[0].view(n, 1), f[1].view(n, 1), f[2].view(n, 4), f[3].view(n, 3)[:, 2:]], 1))
         return torch.stack(rows).contiguous()
 
+    @staticmethod
+    def depth_table(targets, device):
+        """Ground truth of every image for evaluate_3D_depths (detector_infer.py:280-359) as one [B, M, 5] device tensor:
+        (reg_mask, cls_id, target centre x, y, location z) per object slot, from the label fields the training loader
+        attaches."""
+        missing = [f for f in EVAL_DEPTH_FIELDS if not all(t.has_field(f) for t in targets)]
+        if missing:
+            raise RuntimeError("TEST.EVAL_DEPTH measures the depths at the ground-truth centres, but the targets lack %s "
+                               "(a TEST_SPLIT='test' loader attaches no labels)" % ", ".join(missing))
+        return _depth_table(*(torch.stack([torch.as_tensor(t.get_field(k)) for t in targets]) for k in EVAL_DEPTH_FIELDS),
+                            device=device)
+
     def launch(self, heat, reg, meta, methods=None):
         """the two decode kernels (asynchronous; no host sync) for the output_depth or, given a tuple of `methods`, for all
-        of them into a workspace of one block per method"""
+        of them into a workspace of one block per method; with TEST.EVAL_DEPTH the depth-error kernel after them"""
         calib, pad, size = meta[:3]
         B, K = heat.shape[0], self.max_detection
         n_modes = None if methods is None else len(methods)
+        modes = (self.output_depth,) if methods is None else methods
+        table = meta[-1] if self.eval_depth else None
+        eval_slots = 0 if table is None else table.shape[1]
         ws = self._ws if methods is None else self._ws_depths
-        if ws is None or (ws.B, ws.C, ws.n_modes) != (B, heat.shape[1], n_modes) or ws.scores.device != heat.device:
-            ws = DecodeWorkspace(B, heat.shape[1], K, reg.shape[1], heat.device, n_modes)
+        if ws is None or (ws.B, ws.C, ws.n_modes, ws.eval_slots) != (B, heat.shape[1], n_modes, eval_slots) \
+                or ws.scores.device != heat.device:
+            ws = DecodeWorkspace(B, heat.shape[1], K, reg.shape[1], heat.device, n_modes, eval_slots)
             if methods is None:
                 self._ws = ws
             else:
                 self._ws_depths = ws
-        return decode_detections(heat, reg, calib, pad, size, self.dim_mean, K, self.det_threshold, False, ws,
-                                 depth_mode=self.output_depth if methods is None else methods,
-                                 gt=meta[3] if len(meta) > 3 else None)
+        ws = decode_detections(heat, reg, calib, pad, size, self.dim_mean, K, self.det_threshold, False, ws,
+                               depth_mode=self.output_depth if methods is None else methods,
+                               gt=meta[3] if 'oracle' in modes else None)
+        if table is not None:
+            eval_depth_errors(reg, calib, self.dim_mean, table, ws.depth_errors, ws.depth_counts)
+        return ws
 
     def finish(self, ws, heat, reg):
         """host side: read the valid counts (the reference syncs at `valid_mask.sum() == 0`, :106) and slice."""
@@ -116,7 +144,12 @@ class PostProcessor(nn.Module):
         single-mode workspace holds one block without the mode dimension). The counts are read once; the tensors that do
         not depend on the estimator are shared between the methods' dicts."""
         B = heat.shape[0]
-        counts = ws.count.tolist()
+        depth_errors = None
+        if ws.depth_errors is None:
+            counts = ws.count.tolist()
+        else:                                  # the decode's and the depth errors' counts in one copy
+            counts, depth_counts = ws.counts.tolist()
+            depth_errors = depth_error_dict(ws.depth_errors, depth_counts)
 
         def rows(t):
             """the valid rows of every image of a [B, K, ...] workspace tensor, concatenated"""
@@ -140,10 +173,12 @@ class PostProcessor(nn.Module):
             if method in ENSEMBLE_DEPTH_MODES:
                 visualize_preds['min_uncertainty'] = rows(block(ws.min_unc)).long()                     # :185
             conf = result[:, 13] / vis_scores.clamp_min(1e-12) if result.shape[0] else result.new_zeros(0)
-            eval_utils = {'dis_ious': None, 'depth_errors': None, 'uncertainty_conf': conf,
+            eval_utils = {'dis_ious': None, 'depth_errors': depth_errors, 'uncertainty_conf': conf,
                           'estimated_depth_error': depth_err, 'vis_scores': vis_scores, 'batch_idxs': batch_idxs,
                           'counts': counts, 'topk': (ws.scores, ws.inds, ws.clses, ws.ys, ws.xs),
                           'padded_result': block(ws.result)}
+            if depth_errors is not None:
+                eval_utils['depth_error_counts'] = depth_counts
             out[method] = (result, eval_utils, visualize_preds)
         return out
 
@@ -157,9 +192,26 @@ class PostProcessor(nn.Module):
                 if isinstance(name, str) and name.find('keypoints') >= 0:                            # :172-173
                     raise ValueError("unknown key-point depth OUTPUT_DEPTH=%r" % (name,))
                 raise ValueError("OUTPUT_DEPTH=%r is not one of %s" % (name, ", ".join(DEPTH_MODES)))
-        if self.eval_dis_iou or self.eval_depth:
-            raise NotImplementedError("--eval_iou / --eval_depth diagnostics are out of scope")
+        if self.eval_dis_iou:
+            raise NotImplementedError("the --eval_iou diagnostic (TEST.EVAL_DIS_IOUS) is out of scope")
         return tuple(names)
+
+    def evaluate_3D_depths(self, targets, pred_regression):
+        """detector_infer.py:280-359: {key: 1-D float32 CUDA tensor} of the depth errors of every estimator at the
+        ground-truth centres, one entry per valid object in the order of targets['reg_mask'].view(-1). `targets` is the
+        dict of the reference's prepare_targets(test=False): calib (a list), target_centers [B, M, 2], reg_mask [B, M],
+        cls_ids [B, M], locations [B, M, 3]. Each image uses its own calibration. Synchronises once, to read the count."""
+        reg = pred_regression.float().contiguous()
+        if not reg.is_cuda:
+            raise RuntimeError("monoflex_b200 runs on sm_90a GPUs only; no CPU fallback")
+        missing = [f for f in EVAL_DEPTH_FIELDS if f not in targets]
+        if missing:
+            raise RuntimeError("evaluate_3D_depths needs the label fields %s" % ", ".join(missing))
+        calib = torch.tensor([(float(c.f_u), float(c.f_v), float(c.c_u), float(c.c_v), float(c.b_x), float(c.b_y))
+                              for c in targets['calib']], dtype=torch.float32).to(reg.device)
+        table = _depth_table(*(torch.as_tensor(targets[k]) for k in EVAL_DEPTH_FIELDS), device=reg.device)
+        out, counts = eval_depth_errors(reg, calib, self.dim_mean, table)
+        return depth_error_dict(out, counts.tolist())
 
     def forward(self, predictions, targets, features=None, test=False, refine_module=None):
         self.check_config()
@@ -180,3 +232,11 @@ class PostProcessor(nn.Module):
         heat, reg = heat.float().contiguous(), reg.float().contiguous()
         ws = self.launch(heat, reg, self.prepare_targets(targets, test, heat.device, methods), methods)
         return self.finish_depths(ws, heat, reg, methods)
+
+
+def _depth_table(target_centers, reg_mask, cls_ids, locations, device):
+    """the [B, M, 5] depth_table (reg_mask, cls_id, x, y, z) from the stacked label fields [B, M, ...]: a handful of
+    launches whatever B is"""
+    f = [v.to(device=device, dtype=torch.float32, non_blocking=True) for v in (target_centers, reg_mask, cls_ids, locations)]
+    B, M = f[1].shape[0], f[1][0].numel()
+    return torch.cat([f[1].view(B, M, 1), f[2].view(B, M, 1), f[0].view(B, M, 2), f[3].view(B, M, 3)[..., 2:]], 2)

@@ -28,11 +28,13 @@ def sigmoid_hm(hm_features):
 class DecodeWorkspace(object):
     """Caller-owned output / scratch buffers of mf_decode_detections for a fixed (B, C, K, R). With `n_modes` (the
     number of estimators of one mf_decode_detections_depths call) the per-mode outputs result, depth_err and min_unc
-    take a leading mode dimension: [n_modes, B, K, ...]."""
+    take a leading mode dimension: [n_modes, B, K, ...]. With `eval_slots` = M > 0 it also holds the outputs of
+    mf_eval_depth_errors for M object slots per image: depth_errors [13, B*M] and depth_counts [B], the second row of
+    `counts` [2, B] whose first row is `count`, so one device-to-host copy reads both."""
 
-    def __init__(self, B, C, K, R, device, n_modes=None):
+    def __init__(self, B, C, K, R, device, n_modes=None, eval_slots=0):
         f = dict(dtype=torch.float32, device=device)
-        self.B, self.C, self.K, self.R, self.n_modes = B, C, K, R, n_modes
+        self.B, self.C, self.K, self.R, self.n_modes, self.eval_slots = B, C, K, R, n_modes, eval_slots
         lead = () if n_modes is None else (n_modes,)
         slabs = 8     # MF_DECODE_SLABS: stage 1 splits every (image, class) plane into 8 pixel ranges
         self.ws_score = torch.empty(B * C * K * slabs, **f)
@@ -42,7 +44,13 @@ class DecodeWorkspace(object):
         self.inds = torch.empty(B, K, dtype=torch.long, device=device)
         self.pois = torch.empty(B, K, R, **f)
         self.result = torch.empty(*lead, B, K, 14, **f)
-        self.count = torch.empty(B, dtype=torch.int32, device=device)
+        if eval_slots:
+            self.counts = torch.empty(2, B, dtype=torch.int32, device=device)
+            self.count, self.depth_counts = self.counts[0], self.counts[1]
+            self.depth_errors = torch.empty(len(EVAL_DEPTH_KEYS), B * eval_slots, **f)
+        else:
+            self.count = torch.empty(B, dtype=torch.int32, device=device)
+            self.counts = self.depth_counts = self.depth_errors = None
         self.depth_err = torch.empty(*lead, B, K, **f)
         self.proj = torch.empty(B, K, 2, **f)
         self.min_unc = torch.empty(*lead, B, K, dtype=torch.int32, device=device)
@@ -52,6 +60,9 @@ class DecodeWorkspace(object):
 DEPTH_MODES = ('soft', 'hard', 'mean', 'oracle', 'direct', 'keypoints_avg', 'keypoints_center', 'keypoints_02',
                'keypoints_13')
 ENSEMBLE_DEPTH_MODES = DEPTH_MODES[:4]
+# keys of PostProcessor.evaluate_3D_depths' dict (detector_infer.py:341-357), in the row order of mf_eval_depth_errors
+EVAL_DEPTH_KEYS = ('direct', 'direct_sigma', 'keypoint_center', 'keypoint_02', 'keypoint_13', 'keypoint_center_sigma',
+                   'keypoint_02_sigma', 'keypoint_13_sigma', 'sigma_min', 'sigma_weighted', 'mean', 'min', 'target')
 
 
 def decode_detections(heat, reg, calib, pad, size, dim_mean, K, thresh, apply_sigmoid=False, ws=None, depth_mode='soft',
@@ -88,6 +99,30 @@ def decode_detections(heat, reg, calib, pad, size, dim_mean, K, thresh, apply_si
          ws.xs.data_ptr(), ws.pois.data_ptr(), ws.result.data_ptr(), ws.count.data_ptr(), ws.depth_err.data_ptr(),
          ws.proj.data_ptr(), ws.min_unc.data_ptr(), stream())
     return ws
+
+
+def eval_depth_errors(reg, calib, dim_mean, gt, out=None, counts=None):
+    """PostProcessor.evaluate_3D_depths at the ground-truth centres in one kernel (asynchronous). reg [B, 50, H, W],
+    calib [B, 6], dim_mean [C, 3] and gt [B, M, 5] = (reg_mask, cls_id, x, y, z) are float32 CUDA tensors. Returns
+    (out [13, B*M], counts [B] int32): the valid slots' errors compacted in the order of reg_mask.view(-1), one row per
+    key of EVAL_DEPTH_KEYS, and the valid slots of each image. Slots past sum(counts) are not written."""
+    B, R, H, W = reg.shape
+    if gt.dim() != 3 or gt.shape[0] != B or gt.shape[2] != 5 or gt.dtype != torch.float32 or not gt.is_contiguous():
+        raise ValueError("eval_depth_errors needs gt as a contiguous float32 [B, M, 5] tensor, got %s %s"
+                         % (tuple(gt.shape), gt.dtype))
+    M = gt.shape[1]
+    if out is None:
+        out = torch.empty(len(EVAL_DEPTH_KEYS), B * M, dtype=torch.float32, device=reg.device)
+        counts = torch.empty(B, dtype=torch.int32, device=reg.device)
+    call("mf_eval_depth_errors", reg.data_ptr(), calib.data_ptr(), dim_mean.data_ptr(), gt.data_ptr(), B, M,
+         dim_mean.shape[0], H, W, R, out.data_ptr(), counts.data_ptr(), stream())
+    return out, counts
+
+
+def depth_error_dict(table, counts):
+    """{key: 1-D tensor} of the first sum(counts) columns of an eval_depth_errors table: one copy, the keys are its rows"""
+    rows = table[:, :sum(counts)].clone()
+    return {k: rows[i] for i, k in enumerate(EVAL_DEPTH_KEYS)}
 
 
 def _dummy_decode_inputs(heat):
