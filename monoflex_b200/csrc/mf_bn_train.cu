@@ -21,15 +21,16 @@ MF_DEVINL float bn_act_grad(float y, int act) {           // derivative of the a
 
 // thread (cv, r): channel chunk cv (8 channels), row lane r; the CTA walks rows r0 + r, r0 + r + RL, ... of ITS slab.
 // part layout: [ncta][2][C] (sum a, sum b)
-// Forward with pivot != 0: the sums are of d = x - x[row 0], the channel's first value. E[d^2] - E[d]^2 then cancels only
-// as much as the spread of the channel allows, not its mean: summed as E[x^2] - E[x]^2 in fp32, the variance was off by
-// ~2^-24 (mean/std)^2 of itself, and a constant channel kept a variance of rounding noise instead of 0. The SyncBatchNorm
-// halves pass pivot = 0: their sums are added across ranks, whose first rows differ.
+// Forward: the sums are of d = x - x[row 0], the channel's first value. E[d^2] - E[d]^2 then cancels only as much as the
+// spread of the channel allows, not its mean: summed as E[x^2] - E[x]^2 in fp32, the variance was off by ~2^-24
+// (mean/std)^2 of itself, and a constant channel kept a variance of rounding noise instead of 0. The SyncBatchNorm halves
+// pivot on their local first row as well; bn_reduce_kernel un-pivots their sums in double before the exchange, because
+// the ranks' first rows differ.
 template <bool BWD>
 __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restrict__ x, int x_ld, const __half* __restrict__ dy,
                                                          int dy_ld, const __half* __restrict__ y, int y_ld,
                                                          const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                         long long M, int C, int act, long long rows_per_cta, int pivot,
+                                                         long long M, int C, int act, long long rows_per_cta,
                                                          float* __restrict__ part) {
   extern __shared__ float sm[];                            // [RL][2][C]
   const int CV = C / 8, RL = blockDim.x / CV;
@@ -41,11 +42,8 @@ __global__ void __launch_bounds__(256) bn_partial_kernel(const __half* __restric
   if (BWD) {
 #pragma unroll
     for (int e = 0; e < 8; ++e) { mu[e] = mean[cv * 8 + e]; rs[e] = rstd[cv * 8 + e]; }
-  } else if (pivot) {
-    Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(x + cv * 8)), mu);
   } else {
-#pragma unroll
-    for (int e = 0; e < 8; ++e) mu[e] = 0.f;
+    Fp16Rows::to_f32(__ldg(reinterpret_cast<const uint4*>(x + cv * 8)), mu);
   }
   const long long r0 = static_cast<long long>(blockIdx.x) * rows_per_cta;
   const long long r1 = r0 + rows_per_cta < M ? r0 + rows_per_cta : M;
@@ -225,11 +223,22 @@ __global__ void __launch_bounds__(256) bn_bwd_apply_kernel(const __half* __restr
 //   backward: bn_partial<BWD> -> bn_reduce (+ local dgamma / dbeta, which DDP averages like every other gradient) |
 //             all-reduce of [2][C] doubles | bn_bwd_apply with the global sums and the global element count
 // The collective itself is issued by the host between the two C-ABI calls (torch.distributed / NCCL on the same stream).
-__global__ void bn_reduce_kernel(const float* __restrict__ part, int ncta, int C, double* __restrict__ sums) {
+// x != nullptr (forward): the partials are of d = x - p, p = x[row 0]; the sums written are of x and x^2,
+// sum x = sum d + M p and sum x^2 = sum d^2 + 2 p sum d + M p^2, so E[x^2] - E[x]^2 cancels in double after the exchange
+// (M p and M p^2 are exact in double for fp16 p and M < 2^31: a constant channel keeps var = 0 exactly).
+__global__ void bn_reduce_kernel(const float* __restrict__ part, int ncta, int C, const __half* __restrict__ x, long long M,
+                                 double* __restrict__ sums) {
   const int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (c >= C) return;
-  const double s0 = bn_warp_sum(part, ncta, C, 0, c, lane), s1 = bn_warp_sum(part, ncta, C, 1, c, lane);
-  if (lane == 0) { sums[c] = s0; sums[C + c] = s1; }
+  double s0 = bn_warp_sum(part, ncta, C, 0, c, lane), s1 = bn_warp_sum(part, ncta, C, 1, c, lane);
+  if (lane != 0) return;
+  if (x != nullptr) {
+    const double p = static_cast<double>(__half2float(x[c])), m = static_cast<double>(M);
+    s1 += 2.0 * p * s0 + m * p * p;
+    s0 += m * p;
+  }
+  sums[c] = s0;
+  sums[C + c] = s1;
 }
 __global__ void bn_finalize_sums_kernel(const double* __restrict__ sums, int C, double count, const float* __restrict__ gamma,
                                         const float* __restrict__ beta, float eps, float momentum, int abs_gamma,
@@ -312,7 +321,7 @@ int mf_bn_train_forward(const void* x, int x_ld, long long M, int C, const float
   if (sm > 64 * 1024) { set_error("bn_train_forward: shared memory"); return -1; }
   (void)launch_k(bn_partial_kernel<false>, dim3(ncta), dim3(th), sm, st, x, x_ld, static_cast<const __half*>(nullptr), 0,
                  static_cast<const __half*>(nullptr), 0, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), M,
-                 C, 0, rpc, 1, workspace);
+                 C, 0, rpc, workspace);
   bn_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, M, static_cast<const __half*>(x), gamma, beta, eps, momentum, abs_gamma,
                                                       running_mean, running_var, mean, rstd, scale, shift);
   const long long n = M * (C / 8);
@@ -334,7 +343,7 @@ int mf_bn_train_backward(const void* x, int x_ld, const void* dy, int dy_ld, con
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_train_backward: C=%d too wide", C); return -1; }
   float* sums = workspace + static_cast<size_t>(ncta) * 2 * C;        // [2][C] after the partials
   (void)launch_k(bn_partial_kernel<true>, dim3(ncta), dim3(th), sm, st, x, x_ld, dy, dy_ld, y, y_ld, mean, rstd, M, C, act, rpc,
-                 0, workspace);
+                 workspace);
   bn_bwd_finalize_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, dgamma, dbeta, sums, sums + C);
   const long long n = M * (C / 8);
   (void)launch_k(bn_bwd_apply_kernel, dim3(static_cast<unsigned>((n + 255) / 256)), dim3(256), 0, st, x, x_ld, dy, dy_ld, y, y_ld,
@@ -358,8 +367,8 @@ int mf_bn_sync_forward_stats(const void* x, int x_ld, long long M, int C, float*
   }
   (void)launch_k(bn_partial_kernel<false>, dim3(ncta), dim3(th), sm, st, x, x_ld, static_cast<const __half*>(nullptr), 0,
                  static_cast<const __half*>(nullptr), 0, static_cast<const float*>(nullptr), static_cast<const float*>(nullptr), M,
-                 C, 0, rpc, 0, workspace);
-  bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, sums);
+                 C, 0, rpc, workspace);
+  bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, static_cast<const __half*>(x), M, sums);
   return check_cuda(cudaGetLastError(), "bn_sync_forward_stats");
 }
 
@@ -386,8 +395,8 @@ int mf_bn_sync_backward_stats(const void* x, int x_ld, const void* dy, int dy_ld
   const int ncta = bn_grid(M, C, rpc, th, sm);
   if (ncta < 0 || sm > 64 * 1024) { set_error("bn_sync_backward_stats: C=%d too wide", C); return -1; }
   (void)launch_k(bn_partial_kernel<true>, dim3(ncta), dim3(th), sm, st, x, x_ld, dy, dy_ld, y, y_ld, mean, rstd, M, C, act, rpc,
-                 0, workspace);
-  bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, sums);
+                 workspace);
+  bn_reduce_kernel<<<(C * 32 + 127) / 128, 128, 0, st>>>(workspace, ncta, C, static_cast<const __half*>(nullptr), M, sums);
   bn_bwd_sums_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, nullptr, nullptr, dgamma, dbeta);      // local parameter gradients
   return check_cuda(cudaGetLastError(), "bn_sync_backward_stats");
 }

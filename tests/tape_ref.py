@@ -21,23 +21,34 @@ def act_mask(y, act):
     return torch.ones_like(y, dtype=torch.float64)
 
 
-def bn_backward(raw, y, dy, gamma, eps, act, abs_weight=False):
+def bn_xhat(raw, eps):
+    """(xhat, rstd) of training-mode BatchNorm: statistics over every dimension but 1, biased variance (float64)"""
+    raw = raw.double()
+    dims = [d for d in range(raw.dim()) if d != 1]
+    mean = raw.mean(dims, keepdim=True)
+    rstd = (((raw - mean) ** 2).mean(dims, keepdim=True) + eps).rsqrt()
+    return (raw - mean) * rstd, rstd
+
+
+def bn_backward(raw, y, dy, gamma, eps, act, abs_weight=False, count=None, rows=None):
     """y = act(BN_train(raw; gamma, beta) + residual), biased batch variance over every dimension but 1 ->
-    (d_raw, d_residual, dgamma, dbeta). abs_weight: InPlaceABN's |gamma| + eps, dgamma carries sign(gamma)."""
-    raw, dy, gamma = raw.double(), dy.double(), gamma.double()
+    (d_raw, d_residual, dgamma, dbeta). abs_weight: InPlaceABN's |gamma| + eps, dgamma carries sign(gamma).
+    count: the element count dividing the sums in d_raw (a SyncBatchNorm's global count; raw's own by default); rows: a
+    0/1 mask, broadcastable to raw, of the elements the sums take (all by default)."""
+    dy, gamma = dy.double(), gamma.double()
     dims = [d for d in range(raw.dim()) if d != 1]
     shape = [1, -1] + [1] * (raw.dim() - 2)
-    mean = raw.mean(dims, keepdim=True)
-    var = ((raw - mean) ** 2).mean(dims, keepdim=True)
-    rstd = (var + eps).rsqrt()
-    xhat = (raw - mean) * rstd
+    xhat, rstd = bn_xhat(raw, eps)
     g = dy * act_mask(y, act)
+    gs = g if rows is None else g * rows.double()
+    sg, sgx = gs.sum(dims, keepdim=True), (gs * xhat).sum(dims, keepdim=True)
+    n = raw.numel() // raw.shape[1] if count is None else count
     g_eff = gamma.abs() + eps if abs_weight else gamma
-    d_raw = g_eff.view(shape) * rstd * (g - g.mean(dims, keepdim=True) - xhat * (g * xhat).mean(dims, keepdim=True))
-    dgamma = (g * xhat).sum(dims)
+    d_raw = g_eff.view(shape) * rstd * (g - sg / n - xhat * sgx / n)
+    dgamma = sgx.flatten()
     if abs_weight:
         dgamma = dgamma * torch.sign(gamma)
-    return d_raw, g, dgamma, g.sum(dims)
+    return d_raw, g, dgamma, sg.flatten()
 
 
 def conv_backward(x, weight, d_out, stride, pad):
