@@ -411,6 +411,28 @@ int mf_encode_targets_views(const double* labels, const double* P2, const int* s
                             long long* edge_indices, long long* edge_len, int* status, void* stream);
 int mf_encode_edges(const int* sizes, int B, int H, int W, long long* edge_indices, long long* edge_len, void* stream);
 
+/* ---- PNG image data (8-bit RGB, non-interlaced; the host checked the chunks, their CRCs, IHDR and the zlib header).
+ * desc: DEVICE int64 [n][6] = (src_off, src_len, w, h, filt_off, out_off): image i's zlib stream (header included) is
+ *   src[src_off .. src_off + src_len), its filtered scanlines filtered[filt_off .. + h (1 + 3 w)), its pixels
+ *   images[out_off .. + h w 3) as uint8 HWC RGB. filt_off must be a multiple of 4. Nothing outside those ranges is written.
+ * mf_png_inflate: RFC 1950/1951 of every stream into its filtered buffer (one warp per image); status DEVICE int32 [n]
+ *   receives MF_PNG_OK or the first error of each image.
+ * mf_png_unfilter: the PNG filters of every image whose status is MF_PNG_OK (one CTA per image); a filter type above 4
+ *   sets MF_PNG_BAD_FILTER. */
+#define MF_PNG_OK 0
+#define MF_PNG_TRUNCATED 1      /* the stream ends before its final block or its Adler-32 */
+#define MF_PNG_BAD_CODE 2       /* an invalid, over-subscribed or incomplete Huffman code, or an invalid symbol */
+#define MF_PNG_BAD_BLOCK 3      /* block type 3, or a stored block whose LEN and NLEN disagree */
+#define MF_PNG_FAR_DISTANCE 4   /* a back-reference reaching before the start of the output */
+#define MF_PNG_TOO_LONG 5       /* more output than h (1 + 3 w) bytes */
+#define MF_PNG_TOO_SHORT 6      /* the final block ends before h (1 + 3 w) bytes */
+#define MF_PNG_ADLER 7          /* Adler-32 mismatch */
+#define MF_PNG_BAD_FILTER 8     /* a scanline filter type above 4 */
+int mf_png_inflate(const unsigned char* src, const long long* desc, int n, unsigned char* filtered, int* status,
+                   void* stream);
+int mf_png_unfilter(const unsigned char* filtered, const long long* desc, int n, unsigned char* images, int* status,
+                    void* stream);
+
 /* nms_hm alone (model/layers/utils.py:45-58): out = heat * (maxpool3x3(heat) == heat), planes = B*C */
 int mf_nms_hm(const float* heat, float* out, int planes, int H, int W, void* stream);
 

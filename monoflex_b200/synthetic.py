@@ -396,3 +396,18 @@ def make_train_predictions(batch, fields, seed=6, out_w=320, out_h=96):
             z = f["locations"][i, 2] * float(np.exp(g.normal(0, 0.1)))
             reg[b, 48, y, x] = -math.log(z)                              # 1/sigmoid(v) - 1 = exp(-v) = z
     return torch.from_numpy(cls), torch.from_numpy(reg)
+
+
+def natural_image(w, h, seed):
+    """uint8 [h, w, 3] RGB with smooth gradients, a few soft shapes and sensor-like noise: compressed as a PNG it behaves
+    like a photograph rather than like zeros (the PNG decode's tests and tools/bench_png.py)"""
+    g = np.random.default_rng(seed)
+    y, x = np.mgrid[0:h, 0:w].astype(np.float64)
+    img = np.empty((h, w, 3))
+    for c in range(3):
+        img[..., c] = 90 + 60 * np.sin(x / (37 + 11 * c) + g.uniform(0, 6)) * np.cos(y / (23 + 5 * c)) + 0.1 * y
+    for _ in range(6):
+        cx, cy, r = g.uniform(0, w), g.uniform(0, h), g.uniform(5, 80)
+        img += (g.uniform(-60, 60, 3) * np.exp(-((x - cx) ** 2 + (y - cy) ** 2) / (2 * r * r))[..., None])
+    img += g.normal(0, 4, img.shape)
+    return np.clip(img, 0, 255).astype(np.uint8)
