@@ -14,8 +14,24 @@ The files are decoded DECODE_WINDOW images at a time (rounded up to whole batche
 one window, the next one decodes on a side stream ordered by events. The one after it has its host half (reading the
 files, their CRCs, staging them in pinned memory: about 2.3-2.4 ms per 800 KB file) done on a worker thread. Each
 window's status is checked before its first batch is yielded, so a malformed file raises ValueError before any
-detection of its window is written; a file the host rejects raises one window earlier still."""
+detection of its window is written; a file the host rejects raises one window earlier still.
+
+The training loader: `make_data_loader(cfg, is_train=True)` (data/build.py: TrainingSampler, BatchSampler(drop_last=True),
+KITTIDataset with its horizontal flip and right-camera items) from images decoded once into device memory.
+
+    loader = KittiTrainLoader(cfg, "kitti/training")               # split: cfg.DATASETS.TRAIN_SPLIT, e.g. "train"
+    for batch in loader:                                           # infinite, as the reference's
+        loss_dict, log = model(batch["images"], batch["targets"])  # or Trainer.step(batch["images"].tensors,
+                                                                   #                 batch["encoded"], sync_log=False)
+
+At construction it reads every label and calibration file and every image's IHDR, refuses what the reference would
+refuse (before any decode), decodes every view (image_2, and image_3 with DATASETS.USE_RIGHT_IMAGE) into a store of
+uint8 HWC images in device memory and encodes every view in both flip states once to find the items the reference
+cannot encode. A batch is then GpuInputPipeline.images over store views and GpuTargetEncoder.encode over rows of host
+tables: no file, no decode and no host synchronisation per batch.
+"""
 import os
+import time
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
@@ -23,7 +39,7 @@ import torch
 
 from . import targets as T
 from .data import GpuInputPipeline
-from .png import DecodedImages, PngBatch, read_png
+from .png import DecodedImages, PngBatch, read_ihdr, read_png, window_bytes
 from .structures import to_image_list
 
 # Images decoded per launch, chosen with tools/bench_png.py (README, "PNG decode and evaluation loader"). A launch takes
@@ -32,6 +48,44 @@ from .structures import to_image_list
 # runs below the same loop fed from pinned memory. At 1024 the kernels take 0.26 ms per image, but the loop at B = 8
 # ran slower than at 256.
 DECODE_WINDOW = 256
+
+
+def decode_windows(windows, device="cuda"):
+    """Decode windows (lists of PNG paths) in order and yield each window's DecodedImages, checked and ordered before the
+    current stream's later work. While the consumer works on window k, window k + 1 decodes on a side stream and window
+    k + 2 is read, checked and staged in pinned memory on a worker thread. A malformed file raises ValueError when its
+    window comes up, before that window is yielded; a file the host rejects raises one window earlier."""
+    device = torch.device(device)
+    main = torch.cuda.current_stream(device)
+    side = torch.cuda.Stream(device)
+    pool = ThreadPoolExecutor(max_workers=1)
+    staged = []
+
+    def launch(batch):
+        with torch.cuda.stream(side):
+            return DecodedImages(batch, device)
+
+    try:
+        staged = [pool.submit(_stage, w) for w in windows[:2]]
+        pending = launch(staged.pop(0).result()) if windows else None
+        for k in range(len(windows)):
+            dec = pending
+            if k + 2 < len(windows):
+                staged.append(pool.submit(_stage, windows[k + 2]))
+            pending = launch(staged.pop(0).result()) if staged else None
+            dec.check()
+            main.wait_event(dec.event)
+            dec.buffer.record_stream(main)              # read on the main stream after the side stream lets it go
+            yield dec
+    finally:
+        for f in staged:
+            f.cancel()
+        pool.shutdown(wait=True)
+
+
+def _stage(paths):
+    """the host half of a window's decode: read, check and stage its files (runs in the worker thread)"""
+    return PngBatch([read_png(p) for p in paths])
 
 
 class KittiSplit(object):
@@ -92,37 +146,242 @@ class KittiEvalLoader(object):
         batches = self.batches()
         per = self.window // self.batch_size
         windows = [sum(batches[i:i + per], []) for i in range(0, len(batches), per)]
-        main = torch.cuda.current_stream(self.device)
-        side = torch.cuda.Stream(self.device)
-        pool = ThreadPoolExecutor(max_workers=1)
-        staged = []
-        try:
-            # window k + 2 is read and staged on the worker thread and window k + 1 decodes on the side stream while the
-            # consumer runs the model on window k
-            staged = [pool.submit(self._stage, w) for w in windows[:2]]
-            pending = self._launch(staged.pop(0).result(), side) if windows else None
-            for k in range(len(windows)):
-                dec = pending
-                if k + 2 < len(windows):
-                    staged.append(pool.submit(self._stage, windows[k + 2]))
-                pending = self._launch(staged.pop(0).result(), side) if staged else None
-                dec.check()
-                main.wait_event(dec.event)
-                dec.buffer.record_stream(main)              # read on the main stream after the side stream lets it go
-                for j in range(0, len(windows[k]), self.batch_size):
-                    b_ids = windows[k][j:j + self.batch_size]
-                    images, _ = self.pipe.images(dec.images[j:j + len(b_ids)])
-                    yield dict(images=to_image_list(images),
-                               targets=self._targets(b_ids, dec.sizes[j:j + len(b_ids)]), img_ids=tuple(b_ids))
-        finally:
-            for f in staged:
-                f.cancel()
-            pool.shutdown(wait=True)
+        paths = [[os.path.join(self.dataset.image_dir, i + ".png") for i in w] for w in windows]
+        for ids, dec in zip(windows, decode_windows(paths, self.device)):
+            for j in range(0, len(ids), self.batch_size):
+                b_ids = ids[j:j + self.batch_size]
+                images, _ = self.pipe.images(dec.images[j:j + len(b_ids)])
+                yield dict(images=to_image_list(images),
+                           targets=self._targets(b_ids, dec.sizes[j:j + len(b_ids)]), img_ids=tuple(b_ids))
 
-    def _stage(self, ids):
-        """the host half of a window's decode: read, check and stage its files (runs in the loader's worker thread)"""
-        return PngBatch([read_png(os.path.join(self.dataset.image_dir, i + ".png")) for i in ids])
 
-    def _launch(self, batch, side):
-        with torch.cuda.stream(side):
-            return DecodedImages(batch, self.device)
+# Images decoded per launch while the training store is built. The build is bound by the host half of the decode (2.5-2.6
+# ms per file on the worker thread), so the window only has to keep the kernels fed: tools/bench_train_loader.py built
+# 1,024 views in 4.56-4.61 s at 256 and 4.59-5.40 s at 512 (README). The transient filtered buffer is about as large as
+# a window's images, and two windows are in flight.
+TRAIN_DECODE_WINDOW = 256
+VALIDATE_CHUNK = 256                  # views per GpuTargetEncoder.encode call of the start-up validation
+# The flip generator's seed is (sampler seed + FLIP_SEED_OFFSET) mod 2**64: a fixed rule, so that a run's flips follow
+# from its seed, and a different stream from the index generator's, which keeps the reference's seed.
+FLIP_SEED_OFFSET = 0x9E3779B97F4A7C15
+
+
+def _pinned(a):
+    return torch.from_numpy(np.ascontiguousarray(a)).pin_memory()
+
+
+def _dist_rank_world():
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized():
+        return dist.get_rank(), dist.get_world_size()
+    return 0, 1
+
+
+def sampler_seed(cfg, seed=None):
+    """The TrainingSampler seed of a run: `seed` if given; for cfg.SEED >= 0 the value comm.shared_random_seed() returns
+    after default_setup's seed_all_rng(cfg.SEED + rank), rank 0's: np.random.RandomState(cfg.SEED).randint(2 ** 31);
+    otherwise (SEED = -1, the default, also when cfg has no SEED) a draw from numpy's global RNG on rank 0, broadcast to
+    every rank when torch.distributed is initialised. numpy's global RNG is never reseeded here."""
+    if seed is not None:
+        return int(seed)
+    cfg_seed = int(getattr(cfg, "SEED", -1))
+    if cfg_seed >= 0:
+        return int(np.random.RandomState(cfg_seed).randint(2 ** 31))
+    value = [int(np.random.randint(2 ** 31))]
+    import torch.distributed as dist
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1:
+        dist.broadcast_object_list(value, src=0)
+    return value[0]
+
+
+class TrainSampler(object):
+    """TrainingSampler (data/samplers/distributed_sampler.py:12-54) followed by BatchSampler(drop_last=True), with the
+    horizontal flip drawn alongside. Iterating yields int64 [images_per_batch // world, 2] arrays of (dataset index, flip)
+    rows, forever, starting at position 0 of the stream.
+
+    Indices: torch.randperm(size, generator=g) epoch after epoch, g = torch.Generator() seeded with `seed`; this rank's
+    rows are positions rank, rank + world, ... of that stream, and batches run across epoch boundaries, as the
+    reference's do. Flips: a second torch.Generator seeded with (seed + FLIP_SEED_OFFSET) mod 2**64 draws torch.rand(size)
+    per epoch; position j of epoch e is flipped when u_e[j] < flip_prob. The index generator never sees these draws, and
+    the (index, flip) at a global position depends on the seed alone, not on the world size, the rank or the batch size.
+    The reference's flips come from random.random() in its DataLoader workers (worker_init_reset_seed), which depends on
+    NUM_WORKERS and on torch's RNG after the model is built, so they are not reproduced."""
+
+    def __init__(self, size, images_per_batch, seed, rank=0, world=1, flip_prob=0.5):
+        if size < 1:
+            raise ValueError("TrainSampler: dataset size %d" % size)
+        if world < 1 or not 0 <= rank < world:
+            raise ValueError("TrainSampler: rank %d of world %d" % (rank, world))
+        if images_per_batch % world:
+            raise ValueError("SOLVER.IMS_PER_BATCH (%d) must be divisible by the number of GPUs (%d) used"
+                             % (images_per_batch, world))
+        self.size, self.rank, self.world, self.seed = int(size), int(rank), int(world), int(seed)
+        self.batch_size = images_per_batch // world
+        if self.batch_size < 1:
+            raise ValueError("SOLVER.IMS_PER_BATCH = %d" % images_per_batch)
+        self.flip_prob = float(flip_prob)
+
+    def epochs(self):
+        """(indices int64 [size], flips bool [size]) of epoch 0, 1, ... of the global stream"""
+        g, gf = torch.Generator(), torch.Generator()
+        g.manual_seed(self.seed)
+        gf.manual_seed((self.seed + FLIP_SEED_OFFSET) % 2 ** 64)
+        while True:
+            idx = torch.randperm(self.size, generator=g).numpy()
+            flips = torch.rand(self.size, generator=gf).numpy() < self.flip_prob
+            yield idx, flips
+
+    def rows(self):
+        """this rank's (index, flip) rows, one epoch's part at a time: int64 [n, 2] arrays"""
+        for e, (idx, flips) in enumerate(self.epochs()):
+            first = (self.rank - e * self.size) % self.world          # the first position j with e*size + j = rank (mod world)
+            yield np.stack([idx[first::self.world], flips[first::self.world].astype(np.int64)], axis=1)
+
+    def __iter__(self):
+        B, pending = self.batch_size, np.zeros((0, 2), dtype=np.int64)
+        for part in self.rows():
+            pending = np.concatenate([pending, part])
+            n = len(pending) // B * B
+            for i in range(0, n, B):
+                yield pending[i:i + B]
+            pending = pending[n:]
+
+
+class KittiTrainSplit(KittiSplit):
+    """KittiSplit with the right camera's images: len() is len(KITTIDataset), twice the frames with
+    DATASETS.USE_RIGHT_IMAGE (targets.dataset_len), as tools/plain_train_net.py reads it."""
+
+    def __init__(self, cfg, root, split):
+        super(KittiTrainSplit, self).__init__(cfg, root, split)
+        self.image_right_dir = os.path.join(root, "image_3")
+        self.use_right = T.dataset_len(1, cfg) == 2
+        self._len = T.dataset_len(len(self.ids), cfg)
+
+    def __len__(self):
+        return self._len
+
+
+class KittiTrainLoader(object):
+    """The reference's training loader on the GPU (module docstring). rank / world default to torch.distributed's, or
+    (0, 1); seed to sampler_seed(cfg), kept as `.seed` so a run can be repeated. Yields, per batch of
+    SOLVER.IMS_PER_BATCH // world rows of TrainSampler:
+
+        images   ImageList of GpuInputPipeline.images(store views, flips)
+        targets  tuple of ParamsList (kitti.py:496-521 without ori_img), what do_train moves to the device
+        encoded  EncodedTargets of GpuTargetEncoder.encode, for Trainer.step(images, encoded, sync_log=False)
+        img_ids  the frames' 6-character ids, left and right items alike (kitti.py:261)
+
+    Differences from the reference, besides the flip stream (TrainSampler): whatever the reference raises on when it
+    draws an item - a missing image_3, an image larger than the input, an object it cannot encode in either flip state -
+    raises here at construction, naming the file or the frame, camera and flip. Over the reference's 100 epochs every
+    item is drawn in both flip states with near certainty, so it would raise too. The store has to fit in free device
+    memory (KITTI train, left: about 5.2 GB; trainval, both cameras: about 20.9 GB); a larger one raises with both byte
+    counts. A new iterator starts the stream at position 0, as the reference's do_train does on resume."""
+
+    def __init__(self, cfg, root, split=None, rank=None, world=None, seed=None, device="cuda"):
+        split = split if split is not None else getattr(cfg.DATASETS, "TRAIN_SPLIT", None)
+        if not split:
+            raise ValueError("KittiTrainLoader: no split (neither `split` nor cfg.DATASETS.TRAIN_SPLIT is set)")
+        if rank is None or world is None:
+            r, w = _dist_rank_world()
+            rank, world = r if rank is None else rank, w if world is None else world
+        self.device = torch.device(device)
+        self.encoder = T.GpuTargetEncoder(cfg, device)          # refuses every INPUT / DATASETS option not built
+        self.pipe = GpuInputPipeline(cfg, device)
+        self.dataset = ds = KittiTrainSplit(cfg, root, split)
+        if not ds.labelled:
+            raise ValueError("KittiTrainLoader: split %r has no labels" % split)
+        F = len(ds.ids)
+        self.seed = sampler_seed(cfg, seed)
+        self.sampler = TrainSampler(len(ds), int(cfg.SOLVER.IMS_PER_BATCH), self.seed, rank, world,
+                                    flip_prob=float(getattr(cfg.INPUT, "AUG_PARAMS", [[0.5]])[0][0]))
+        self.build_seconds = {}
+        t0 = time.perf_counter()
+        self.labels = self._read_labels(cfg)
+        self.P = np.stack([T.read_kitti_calib(os.path.join(ds.calib_dir, i + ".txt")) for i in ds.ids]
+                          + ([T.read_kitti_calib(os.path.join(ds.calib_dir, i + ".txt"), use_right_cam=True)
+                              for i in ds.ids] if ds.use_right else [])).reshape(-1, 3, 4)
+        # per dataset index (targets.dataset_view): frame, right flag, file, (w, h), camera matrix
+        views = [T.dataset_view(i, F, cfg) for i in range(len(ds))]
+        self.frames = np.array([f for f, _ in views], dtype=np.int64)
+        self.right = np.array([r for _, r in views], dtype=bool)
+        self.files = [os.path.join(ds.image_right_dir if r else ds.image_dir, ds.ids[f] + ".png")
+                      for f, r in zip(self.frames, self.right)]
+        t1 = time.perf_counter()
+        self.sizes = np.array([self._ihdr(p) for p in self.files], dtype=np.int64).reshape(-1, 2)
+        windows = [self.files[i:i + TRAIN_DECODE_WINDOW] for i in range(0, len(self.files), TRAIN_DECODE_WINDOW)]
+        per_window = [window_bytes([tuple(s) for s in self.sizes[i:i + TRAIN_DECODE_WINDOW]])
+                      for i in range(0, len(self.files), TRAIN_DECODE_WINDOW)]
+        self.store_bytes = int(sum(b for b, _ in per_window))
+        need = self.store_bytes + 2 * max(f for _, f in per_window)
+        free = torch.cuda.mem_get_info(self.device)[0]
+        if need > free:
+            raise MemoryError("KittiTrainLoader: the decoded images of split %r take %d bytes on the device (%d with the "
+                              "decode's transient buffers), more than the %d bytes free; streaming is not built"
+                              % (split, self.store_bytes, need, free))
+        t2 = time.perf_counter()
+        self.store, self.images = [], []
+        for dec in decode_windows(windows, self.device):
+            self.store.append(dec.buffer)
+            self.images += dec.images
+        t3 = time.perf_counter()
+        self._validate()
+        torch.cuda.current_stream(self.device).synchronize()
+        self.build_seconds = dict(labels_calib=t1 - t0, headers=t2 - t1, decode=t3 - t2, validate=time.perf_counter() - t3)
+
+    def _read_labels(self, cfg):
+        ds, M = self.dataset, int(cfg.DATASETS.MAX_OBJECTS)
+        rows = []
+        for i in ds.ids:
+            path = os.path.join(ds.label_dir, i + ".txt")
+            try:
+                r = T.read_kitti_label(path, tuple(ds.classes))
+            except ValueError as e:
+                raise ValueError("%s: %s" % (path, e))
+            if len(r) > M:
+                raise ValueError("%s: %d objects of the detected classes, more than MAX_OBJECTS = %d" % (path, len(r), M))
+            rows.append(r)
+        return T.pack_labels(rows, M)
+
+    def _ihdr(self, path):
+        if not os.path.exists(path):
+            raise FileNotFoundError("KittiTrainLoader: image file not found: %s" % path)
+        w, h = read_ihdr(path)
+        if w > self.encoder.W or h > self.encoder.H:
+            raise ValueError("%s: image %dx%d larger than the input %dx%d (INPUT.WIDTH_TRAIN x HEIGHT_TRAIN)"
+                             % (path, w, h, self.encoder.W, self.encoder.H))
+        return w, h
+
+    def _encode(self, idx, flips):
+        """GpuTargetEncoder.encode of the dataset indices `idx` with `flips`, from rows of the host tables staged in pinned
+        memory, so that their copies to the device do not wait for the stream"""
+        right = _pinned(self.right[idx].astype(np.int32)) if self.dataset.use_right else None
+        return self.encoder.encode(_pinned(self.labels[self.frames[idx]]), _pinned(self.P[idx]), _pinned(self.sizes[idx]),
+                                   _pinned(np.asarray(flips, dtype=np.int32)), right=right)
+
+    def _validate(self):
+        """every item in both flip states through the encoder, one status read in all; a chunk that reports objects the
+        reference cannot encode is encoded item by item to name the item"""
+        n = len(self.dataset)
+        chunks = [(np.arange(i, min(i + VALIDATE_CHUNK, n)), f) for i in range(0, n, VALIDATE_CHUNK) for f in (0, 1)]
+        status = torch.cat([self._encode(idx, np.full(len(idx), f)).status for idx, f in chunks]).cpu().numpy()
+        for (idx, f), s in zip(chunks, status):
+            if not s:
+                continue
+            for i in idx:
+                if int(self._encode(np.array([i]), np.array([f])).status.item()):
+                    raise RuntimeError("KittiTrainLoader: frame %s, %s, %s: an object the reference cannot encode (an edge "
+                                       "object with two non-zero heat-map radii, or an outside object whose 2D box centre "
+                                       "lies outside the image)" % (self.dataset.ids[self.frames[i]],
+                                                                    "image_3" if self.right[i] else "image_2",
+                                                                    "flipped" if f else "not flipped"))
+
+    def __iter__(self):
+        ids = self.dataset.ids
+        for rows in self.sampler:
+            idx, flips = rows[:, 0], rows[:, 1].astype(bool)
+            images, _ = self.pipe.images([self.images[i] for i in idx], flips=flips)
+            enc = self._encode(idx, flips)
+            P = T.flip_calib(self.P[idx], self.sizes[idx, 0], flips)
+            yield dict(images=to_image_list(images), targets=tuple(enc.param_lists(P)), encoded=enc,
+                       img_ids=tuple(ids[f] for f in self.frames[idx]))

@@ -105,6 +105,28 @@ def read_png(path):
         return parse_png(f.read(), path)
 
 
+IHDR_END = 33                    # signature, IHDR length and type, its 13 bytes and its CRC
+
+
+def read_ihdr(path):
+    """(w, h) of a PNG file from its first 33 bytes, with the signature, the IHDR CRC and the PNG kind checked as
+    parse_png checks them; the rest of the file is not read."""
+    with open(path, "rb") as f:
+        data = f.read(IHDR_END)
+    if data[:8] != SIGNATURE:
+        raise ValueError("%s: not a PNG file (bad signature)" % path)
+    if len(data) < IHDR_END:
+        raise ValueError("%s: truncated chunk header at byte 8" % path)
+    length, ctype = struct.unpack(">I4s", data[8:16])
+    if ctype != b"IHDR" or length != 13:
+        raise ValueError("%s: the first chunk is %r of %d bytes, not a 13-byte IHDR" % (path, ctype, length))
+    if zlib.crc32(data[12:29]) & 0xffffffff != struct.unpack(">I", data[29:33])[0]:
+        raise ValueError("%s: CRC error in the b'IHDR' chunk at byte 8" % path)
+    ihdr = struct.unpack(">IIBBBBB", data[16:29])
+    _check_ihdr(ihdr, path)
+    return ihdr[0], ihdr[1]
+
+
 def _aligned(sizes):
     """offsets of buffers of `sizes` bytes, each on an _ALIGN boundary with at least _ALIGN bytes before and after it;
     and the total"""
@@ -113,6 +135,12 @@ def _aligned(sizes):
         offs.append(pos)
         pos += (s + 2 * _ALIGN - 1) // _ALIGN * _ALIGN
     return offs, pos
+
+
+def window_bytes(sizes):
+    """The device bytes DecodedImages allocates for one window of images of `sizes` ((w, h) each), as PngBatch lays them
+    out: (the images buffer, the filtered buffer that lives until the kernels have run)."""
+    return (_aligned([w * h * 3 for w, h in sizes])[1], _aligned([h * (1 + 3 * w) for w, h in sizes])[1])
 
 
 class PngBatch(object):

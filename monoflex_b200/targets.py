@@ -89,6 +89,18 @@ def dataset_view(idx, num_samples, cfg, is_train=True):
     return (idx - num_samples, True) if idx >= num_samples else (idx, False)
 
 
+def flip_calib(P, widths, flips):
+    """The camera matrices encode() writes to EncodedTargets.P2, on the host: float64 P [B, 3, 4] with the horizontal flip's
+    calibration change (augmentations.py:71-74, P[0, 2] = w - P[0, 2] - 1, P[0, 3] = -P[0, 3]) where flips[b] is set,
+    w = widths[b] the width of the view's own image."""
+    P = np.array(P, dtype=np.float64).reshape(-1, 3, 4)
+    f = np.asarray(flips, dtype=bool).reshape(-1)
+    w = np.asarray(widths, dtype=np.float64).reshape(-1)
+    P[f, 0, 2] = w[f] - P[f, 0, 2] - 1
+    P[f, 0, 3] = -P[f, 0, 3]
+    return P
+
+
 def _use_right(cfg, is_train):
     return bool(_get(cfg.DATASETS, "USE_RIGHT_IMAGE", False)) and bool(is_train)
 
@@ -283,14 +295,19 @@ class EncodedTargets(object):
             out.append(t)
         return out
 
-    def param_lists(self):
+    def param_lists(self, P2=None):
         """Reference-shaped ParamsLists (kitti.py:496-521 without ori_img): device tensor views of the encoded tables and a
-        host Calibration of the (flipped) P2 or P3 (one device-to-host copy). prepare_targets(param_lists()) == prepared."""
+        host Calibration of the (flipped) P2 or P3 (one device-to-host copy). prepare_targets(param_lists()) == prepared.
+        P2: host float64 [B, 3, 4] equal to self.P2 (flip_calib of the encoded matrices) for the Calibrations, so that
+        nothing here waits for the device."""
         enc = self
         hm, obj, img = self.prepared
         B, M = len(self), self.encoder.max_objs
         o = obj.view(B, M, obj.shape[1])
-        P2 = self.P2.cpu().numpy()
+        if P2 is None:
+            P2 = self.P2.cpu().numpy()
+        elif np.shape(P2) != (B, 3, 4):
+            raise ValueError("P2: [%d, 3, 4] host matrices expected, got %s" % (B, np.shape(P2)))
         pad = img[:, 6:8].to(torch.int64)
         out = []
         for b in range(B):
