@@ -14,7 +14,8 @@ The files are decoded DECODE_WINDOW images at a time (rounded up to whole batche
 one window, the next one decodes on a side stream ordered by events. The one after it has its host half (reading the
 files, their CRCs, staging them in pinned memory: about 2.3-2.4 ms per 800 KB file) done on a worker thread. Each
 window's status is checked before its first batch is yielded, so a malformed file raises ValueError before any
-detection of its window is written; a file the host rejects raises one window earlier still.
+detection of its window is written; a file the host rejects raises one window earlier still. When the decoded split fits
+in free device memory, the first complete pass keeps it and later passes read it back (KittiEvalLoader).
 
 The training loader: `make_data_loader(cfg, is_train=True)` (data/build.py: TrainingSampler, BatchSampler(drop_last=True),
 KITTIDataset with its horizontal flip and right-camera items) from images decoded once into device memory.
@@ -88,6 +89,17 @@ def _stage(paths):
     return PngBatch([read_png(p) for p in paths])
 
 
+def store_budget(sizes, window, device="cuda"):
+    """(store bytes, bytes needed, bytes free) of decoding images of `sizes` ((w, h) each) `window` at a time and keeping
+    them in device memory: the store is every window's images buffer (window_bytes), the need adds the transient filtered
+    buffers of the two windows decode_windows has in flight, the free bytes are torch.cuda.mem_get_info's. Both loaders
+    keep their images only when need <= free."""
+    per_window = [window_bytes(sizes[i:i + window]) for i in range(0, len(sizes), window)]
+    store = int(sum(b for b, _ in per_window))
+    need = store + 2 * max([f for _, f in per_window] + [0])
+    return store, need, torch.cuda.mem_get_info(device)[0]
+
+
 class KittiSplit(object):
     """What the reference's KITTIDataset exposes to the evaluation (engine/inference.py, inference_all_depths): the split
     file, the label directory, the classes and the ids in the split's order."""
@@ -110,6 +122,18 @@ class KittiSplit(object):
 
 
 class KittiEvalLoader(object):
+    """The reference's evaluation loader on the GPU (module docstring), TEST.IMS_PER_BATCH images per batch.
+
+    The first complete pass also keeps what it decoded and encoded: each window's images buffer and every batch's
+    targets. Later passes read them back - no file, no PNG decode, no label or calibration parsing and no host
+    synchronisation per batch, only GpuInputPipeline.images over the kept views - and yield the same batches, bit for
+    bit. Keeping is decided from free device memory, by KittiTrainLoader's rule (store_budget: the images plus the
+    decode's transient buffers against torch.cuda.mem_get_info), before the first window and again before each later
+    one. It is all or nothing: when a window does not fit, what was kept is dropped and every pass streams. KITTI val
+    (3,769 images of about 1242x375) holds about 5.2 GB (`store_bytes`); dropping the loader releases it. The kept
+    passes see the split as it was read: files changed after the first complete pass are not read again. A pass the
+    consumer leaves early keeps nothing."""
+
     def __init__(self, cfg, root, split=None, device="cuda"):
         self.dataset = KittiSplit(cfg, root, cfg.DATASETS.TEST_SPLIT if split is None else split)
         self.batch_size = int(getattr(cfg.TEST, "IMS_PER_BATCH", 1))
@@ -120,6 +144,13 @@ class KittiEvalLoader(object):
         self.pipe = GpuInputPipeline(cfg, device)
         self.encoder = T.GpuTargetEncoder(cfg, device)
         self.max_objs = int(cfg.DATASETS.MAX_OBJECTS)
+        self.store_bytes = None           # the images' device bytes, once a pass has read the headers
+        self._kept = None                 # [(image views, targets, ids)] per batch, after a complete kept pass
+
+    @property
+    def kept(self):
+        """True when the passes read the images and targets kept by the first complete pass"""
+        return self._kept is not None
 
     def __len__(self):
         return -(-len(self.dataset) // self.batch_size)
@@ -142,17 +173,46 @@ class KittiEvalLoader(object):
         enc.check()
         return out
 
+    def _image_sizes(self, paths):
+        """(w, h) of every image from its IHDR, or None when a header cannot be read: that file then raises where the
+        streamed pass reaches it, as it does without keeping"""
+        try:
+            return [read_ihdr(p) for w in paths for p in w]
+        except (OSError, ValueError, NotImplementedError):
+            return None
+
+    def _fits(self, sizes):
+        store, need, free = store_budget(sizes, self.window, self.device)
+        return need <= free
+
     def __iter__(self):
+        if self._kept is not None:
+            for views, targets, ids in self._kept:
+                images, _ = self.pipe.images(views)
+                yield dict(images=to_image_list(images), targets=targets, img_ids=ids)
+            return
         batches = self.batches()
         per = self.window // self.batch_size
         windows = [sum(batches[i:i + per], []) for i in range(0, len(batches), per)]
         paths = [[os.path.join(self.dataset.image_dir, i + ".png") for i in w] for w in windows]
-        for ids, dec in zip(windows, decode_windows(paths, self.device)):
+        sizes = self._image_sizes(paths)
+        kept = None
+        if sizes is not None:
+            self.store_bytes = store_budget(sizes, self.window, self.device)[0]
+            kept = [] if self._fits(sizes) else None
+        for k, (ids, dec) in enumerate(zip(windows, decode_windows(paths, self.device))):
+            if kept is not None and k and not self._fits(sizes[k * self.window:]):
+                kept = None                                       # all or nothing: stream this pass and the next ones
             for j in range(0, len(ids), self.batch_size):
                 b_ids = ids[j:j + self.batch_size]
-                images, _ = self.pipe.images(dec.images[j:j + len(b_ids)])
-                yield dict(images=to_image_list(images),
-                           targets=self._targets(b_ids, dec.sizes[j:j + len(b_ids)]), img_ids=tuple(b_ids))
+                views = dec.images[j:j + len(b_ids)]
+                images, _ = self.pipe.images(views)
+                batch = dict(images=to_image_list(images), targets=self._targets(b_ids, dec.sizes[j:j + len(b_ids)]),
+                             img_ids=tuple(b_ids))
+                if kept is not None:
+                    kept.append((views, batch["targets"], batch["img_ids"]))
+                yield batch
+        self._kept = kept
 
 
 # Images decoded per launch while the training store is built. The build is bound by the host half of the decode (2.5-2.6
@@ -310,11 +370,7 @@ class KittiTrainLoader(object):
         t1 = time.perf_counter()
         self.sizes = np.array([self._ihdr(p) for p in self.files], dtype=np.int64).reshape(-1, 2)
         windows = [self.files[i:i + TRAIN_DECODE_WINDOW] for i in range(0, len(self.files), TRAIN_DECODE_WINDOW)]
-        per_window = [window_bytes([tuple(s) for s in self.sizes[i:i + TRAIN_DECODE_WINDOW]])
-                      for i in range(0, len(self.files), TRAIN_DECODE_WINDOW)]
-        self.store_bytes = int(sum(b for b, _ in per_window))
-        need = self.store_bytes + 2 * max(f for _, f in per_window)
-        free = torch.cuda.mem_get_info(self.device)[0]
+        self.store_bytes, need, free = store_budget([tuple(s) for s in self.sizes], TRAIN_DECODE_WINDOW, self.device)
         if need > free:
             raise MemoryError("KittiTrainLoader: the decoded images of split %r take %d bytes on the device (%d with the "
                               "decode's transient buffers), more than the %d bytes free; streaming is not built"

@@ -71,9 +71,9 @@ class PostProcessor(nn.Module):
             calib.append((float(c.f_u), float(c.f_v), float(c.c_u), float(c.c_v), float(c.b_x), float(c.b_y)))
             size.append((float(t.size[0]), float(t.size[1])))
         key = (tuple(calib), tuple(size), str(device))
-        if self._meta_cache is None or self._meta_cache[0] != key:
-            self._meta_cache = (key, torch.tensor(calib, dtype=torch.float32).to(device),
-                                torch.tensor(size, dtype=torch.float32).to(device))
+        if self._meta_cache is None or self._meta_cache[0] != key:     # copied up without waiting for the device
+            self._meta_cache = (key, torch.tensor(calib, dtype=torch.float32).to(device, non_blocking=True),
+                                torch.tensor(size, dtype=torch.float32).to(device, non_blocking=True))
         pad = torch.stack([torch.as_tensor(t.get_field("pad_size")) for t in targets]).to(device=device, dtype=torch.float32,
                                                                                          non_blocking=True).view(-1, 2)
         meta = (self._meta_cache[1], pad, self._meta_cache[2])

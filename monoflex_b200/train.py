@@ -170,7 +170,10 @@ class Trainer(object):
         if g["update_inside"]:                 # capture only records: undo the host-side bookkeeping of the captured step()
             opt.step_count -= 1
             opt._step_t -= 1
-        g.update(graph=graph, loss_dict={k: v.detach() for k, v in loss_dict.items()}, log=log, plan_h=pred.last_plan)
+        # the graph owns the plans whose buffers it reads: an eval forward between steps (do_eval) replaces the backbone's
+        # and the predictor's cached plan, which would otherwise free the train plans' buffers under the graph
+        g.update(graph=graph, loss_dict={k: v.detach() for k, v in loss_dict.items()}, log=log, plan_h=pred.last_plan,
+                 plan_b=model.backbone.last_plan)
         self._graph = g
         return g
 
