@@ -12,6 +12,7 @@ optimizer param groups and DDP see exactly what they see in the reference (SURVE
   ConvTranspose2d + add        -> one HBM-bound kernel                                 (IDAUp :419-425)
 """
 import math
+import os
 
 import numpy as np
 import torch
@@ -176,10 +177,33 @@ class DLA(nn.Module):
         return y
 
 
+DLA34_URL = "http://dl.yf.io/dla/models/imagenet/dla34-ba72cf86.pth"      # get_model_url('imagenet', 'dla34', 'ba72cf86')
+
+
+def pretrained_path():
+    """where torch.hub's model_zoo.load_url caches the ImageNet DLA-34 weights, which the reference loads"""
+    return os.path.join(torch.hub.get_dir(), "checkpoints", os.path.basename(DLA34_URL))
+
+
+def load_pretrained(model):
+    """DLA.load_pretrained_model (dla_dcn.py:333-344) from the cached file only: an `fc` Conv2d(channels[-1], num_classes, 1)
+    is attached, num_classes being the length of the file's last entry, and the file is loaded with strict=True. `fc` is
+    outside the forward (the reference's DLA.forward never calls it), so training leaves it unchanged. Nothing is
+    downloaded: a missing file raises."""
+    path = pretrained_path()
+    if not os.path.isfile(path):
+        raise RuntimeError("MODEL.PRETRAIN: the ImageNet DLA-34 weights are not cached at %s; download %s to that path "
+                           "(monoflex_b200 never downloads), or set MODEL.PRETRAIN False" % (path, DLA34_URL))
+    weights = torch.load(path, map_location="cpu")
+    num_classes = len(weights[list(weights.keys())[-1]])
+    model.fc = nn.Conv2d(model.channels[-1], num_classes, kernel_size=1, stride=1, padding=0, bias=True)
+    model.load_state_dict(weights)
+    return model
+
+
 def dla34(pretrained=False, **kwargs):
-    if pretrained:
-        raise RuntimeError("MODEL.PRETRAIN downloads ImageNet weights (dla_dcn.py:333-344); load a checkpoint instead")
-    return DLA([1, 1, 1, 2, 2, 1], [16, 32, 64, 128, 256, 512], block=BasicBlock, **kwargs)
+    model = DLA([1, 1, 1, 2, 2, 1], [16, 32, 64, 128, 256, 512], block=BasicBlock, **kwargs)
+    return load_pretrained(model) if pretrained else model
 
 
 def fill_up_weights(up):

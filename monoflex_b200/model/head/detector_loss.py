@@ -129,7 +129,10 @@ class Loss_Computation(object):
         key = (tuple(rows), str(device))
         cache = getattr(self, "_calib_cache", None)
         if cache is None or cache[0] != key:
-            cache = self._calib_cache = (key, torch.tensor(rows, dtype=torch.float32).to(device))
+            rows = torch.tensor(rows, dtype=torch.float32)
+            if torch.device(device).type == "cuda":       # through pinned memory: a new batch's cameras do not block the host
+                rows = rows.pin_memory().to(device, non_blocking=True)
+            cache = self._calib_cache = (key, rows.to(device))
         pad = torch.stack([torch.as_tensor(t.get_field("pad_size")) for t in targets]).to(device=device, dtype=torch.float32,
                                                                                          non_blocking=True).view(B, 2)
         img = torch.cat([cache[1], pad], 1).contiguous()

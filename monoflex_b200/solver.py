@@ -126,6 +126,14 @@ def allreduce_grads(arena, bucket_bytes=32 << 20, group=None, async_op=False):
     return world, handles
 
 
+def _to_device(host, device):
+    """host -> device; to a CUDA device through pinned memory without blocking (torch's host allocator keeps the staging
+    buffer until the copy has run)"""
+    if device.type != "cuda":
+        return host.to(device)
+    return host.pin_memory().to(device, non_blocking=True)
+
+
 class FusedAdamW(torch.optim.Optimizer):
     """torch.optim.AdamW(model_params, lr, betas=(0.9, 0.99), weight_decay) (solver/__init__.py:36-37) with the update of
     ALL tensors in one kernel launch over a ParamArena.
@@ -250,8 +258,8 @@ class FusedAdamW(torch.optim.Optimizer):
         else:
             mult = 1.0
             vals = tuple(0.0 if g is None else (unused * g["lr"] if skip else g["lr"]) for g, skip in zip(groups, self._skip))
-        if vals != self._lr_key:
-            table = self.arena.chunk_table(vals).to(self.arena.params.device)
+        if vals != self._lr_key:            # pinned staging: a schedule that moves the lr does not block the host
+            table = _to_device(self.arena.chunk_table(vals), self.arena.params.device)
             if self._chunk_lr is None or self._chunk_lr.shape != table.shape:
                 self._chunk_lr = table
             else:
@@ -259,7 +267,7 @@ class FusedAdamW(torch.optim.Optimizer):
             self._lr_key = vals
         key = (mult, beta1, self._weight_decay())
         if key != self._hyper_key:
-            self._hyper.copy_(torch.tensor(key + (0.0,), dtype=torch.float64))   # in place, like the table
+            self._hyper.copy_(_to_device(torch.tensor(key + (0.0,), dtype=torch.float64), self._hyper.device))  # in place
             self._hyper_key = key
         return self._chunk_lr
 
@@ -525,6 +533,17 @@ class FusedOneCycleAdam(object):
 
 
 OPTIMIZERS = ("adamw", "adam", "adam_onecycle")
+FUSED_OPTIMIZERS = (FusedAdamW, FusedOneCycleAdam)      # FusedAdam is a FusedAdamW
+
+
+def check_fused(optimizer):
+    """the training step updates the parameter arena of one of these optimisers; a torch.optim optimiser raises TypeError
+    naming the line to change"""
+    if not isinstance(optimizer, FUSED_OPTIMIZERS):
+        raise TypeError("the captured training step needs one of monoflex_b200's fused optimisers (%s), got %s: build it "
+                        "with `from monoflex_b200.solver import build_optimizer, build_scheduler` in place of "
+                        "`from solver import build_optimizer, build_scheduler` (tools/plain_train_net.py)"
+                        % (", ".join(c.__name__ for c in FUSED_OPTIMIZERS), type(optimizer).__name__))
 
 
 def build_optimizer(model, cfg, symmetric_group=None):

@@ -411,3 +411,28 @@ def natural_image(w, h, seed):
         img += (g.uniform(-60, 60, 3) * np.exp(-((x - cx) ** 2 + (y - cy) ** 2) / (2 * r * r))[..., None])
     img += g.normal(0, 4, img.shape)
     return np.clip(img, 0, 255).astype(np.uint8)
+
+
+def dla34_imagenet_weights(seed=0, num_classes=1000):
+    """A seeded stand-in for the ImageNet DLA-34 file (dla34-ba72cf86.pth) with its keys, in its order, and its shapes:
+    the DLA-34 base's parameters and BN statistics (no num_batches_tracked, which the file predates) and the classifier
+    `fc` (Conv2d(512, num_classes, 1)) last. Conv weights at He scale, BN affine and statistics near identity."""
+    from .model.backbone.dla_dcn import dla34
+    g = _rng(seed)
+    base = dla34(pretrained=False)
+    base.fc = torch.nn.Conv2d(base.channels[-1], num_classes, kernel_size=1, bias=True)
+    out = {}
+    for k, v in base.state_dict().items():
+        if k.endswith("num_batches_tracked"):
+            continue
+        shape = tuple(v.shape)
+        if k.endswith("running_var"):
+            a = g.uniform(0.5, 1.5, shape)
+        elif k.endswith("running_mean") or k.endswith("bias"):
+            a = g.normal(0.0, 0.05, shape)
+        elif len(shape) == 1:                                          # BN weight
+            a = g.uniform(0.8, 1.2, shape)
+        else:
+            a = g.standard_normal(shape) * math.sqrt(2.0 / (shape[1] * shape[2] * shape[3]))
+        out[k] = _t(a)
+    return out
