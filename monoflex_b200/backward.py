@@ -47,9 +47,12 @@ def _into(dx, t):
 
 
 def add_rows(dst, src):
-    """dst += src (fp16 rows: Acts or tensors of the same pixel count)"""
+    """dst += src (fp16 rows: Acts or tensors of the same pixel count; src has at least dst's channels)"""
     (d, d_ld), (s, s_ld) = _rows(dst, "dst"), _rows(src, "src")
     M, C = (dst.M, dst.C) if isinstance(dst, engine.Act) else dst.shape
+    sM, sC = (src.M, src.C) if isinstance(src, engine.Act) else src.shape
+    if sM != M or sC < C:
+        raise ValueError("add_rows: source rows [%d, %d] do not cover destination rows [%d, %d]" % (sM, sC, M, C))
     call("mf_add_rows_f16", d, d_ld, s, s_ld, M, C, stream())
 
 
@@ -133,18 +136,23 @@ def conv2d_dgrad_stride2(dy_rows, weight, B, Ho, Wo):
 
 def conv_backward(x, weight, bias, stride, pad, dy, dx=None):
     """y = conv(x, weight, stride, pad) (+ bias) with x an engine.Act and dy = dL/dy rows [B*Ho*Wo, Cout or zero-padded Cout]
-    fp16 -> (dW, dbias or None); dx += dL/dx unless dx is None."""
+    fp16 -> (dW, dbias or None); dx += dL/dx unless dx is None. The stride-2 data gradient is built for 3x3 / pad 1 on
+    even H and W only."""
     cout, cin, k, _ = weight.shape
+    if dx is not None and stride != 1:
+        if (stride, k, pad) != (2, 3, 1):
+            raise NotImplementedError("data gradient of a %dx%d stride-%d pad-%d convolution" % (k, k, stride, pad))
+        if x.H % 2 or x.W % 2:
+            # the four parities cover 2Ho x 2Wo = (H + 1) x (W + 1) pixels; nothing crops them back to H x W
+            raise NotImplementedError("data gradient of a 3x3 stride-2 convolution on an odd %dx%d input" % (x.H, x.W))
     dw = conv2d_wgrad(x, dy, x.B, x.H, x.W, k, stride, pad)[:cout, :cin]
     db = column_sum(dy)[:cout] if bias is not None else None
     if dx is not None:
         ho, wo = (x.H + 2 * pad - k) // stride + 1, (x.W + 2 * pad - k) // stride + 1
         if stride == 1:
             conv2d_dgrad(dy, weight, x.B, ho, wo, pad, dx)
-        elif (stride, k, pad) == (2, 3, 1):
-            add_rows(dx, conv2d_dgrad_stride2(dy, weight, x.B, ho, wo))
         else:
-            raise NotImplementedError("data gradient of a %dx%d stride-%d pad-%d convolution" % (k, k, stride, pad))
+            add_rows(dx, conv2d_dgrad_stride2(dy, weight, x.B, ho, wo))
     return dw, db
 
 
